@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the FourierGrid / DVGO rendering hot path on B200.
+"""bench.py -- headline benchmark of the FourierGrid / DVGO rendering hot path on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference|reference-gpu] [--workload truck|bicycle]
 
@@ -16,7 +16,7 @@ step, inside the timed region).  `roofline` = the dominant hand-written kernel, 
 timed region.  `cpu_baseline` / `--impl reference` = the reference's algorithm on the host cores (CPU oracle port of
 the same step: torch F.grid_sample CPU path + C restatement of the CUDA-only ops) on a bounded ray sample, with the
 thread count that is fastest for it.  `psnr_delta_vs_ref` = second half of the metric (oracle/psnr_check.py).
-`--impl reference-gpu` (informative, not part of the driver contract) = the reference's GPU path on this B200: its
+`--impl reference-gpu` (informative, not part of the driver contract) = the reference's GPU path on this GPU: its
 algorithm op by op with its own CUDA extension from oracle/_ref + ATen / cuBLAS.
 A/B switches (env): UBN_BENCH_TAIL=peer|pipelined|sequential (training-step tail), UBN_BENCH_LOSS=fused|torch,
 UBN_TV_IMPL=1|0 (streaming / element-per-thread TV; scripts/check_tv_stream.py), UBN_RGBNET_MODE=tc3|tc1|simt,
@@ -135,7 +135,7 @@ def load_peaks():
         with open(os.path.join(ROOT, 'MEASURED_PEAKS.json')) as f:
             return float(json.load(f)['hbm_gbs']), 'measured (MEASURED_PEAKS.json)'
     except Exception:
-        return 6650.0, 'fallback (B200_PROFILING.md)'
+        return 3350.0, 'H100 SXM data sheet (HBM3)'
 
 
 def load_tensor_peak():
@@ -143,15 +143,34 @@ def load_tensor_peak():
         with open(os.path.join(ROOT, 'MEASURED_PEAKS.json')) as f:
             return float(json.load(f)['bf16_tflops_sustained']), 'measured sustained bf16 (MEASURED_PEAKS.json)'
     except Exception:
-        return 1400.0, 'fallback (B200_PROFILING.md)'
+        return 989.0, 'H100 SXM data sheet (dense bf16)'
 
 
-def load_traffic(kernel):
-    try:
-        with open(os.path.join(ROOT, 'profiles', 'traffic.json')) as f:
-            return json.load(f).get(kernel)
-    except Exception:
-        return None
+DUMP_KEYS = ('rgb_marched', 'alphainv_last', 'weights', 'ray_id', 'raw_rgb')
+DUMP_SAMPLE = 1 << 20
+
+
+def dump_outputs(out_dir, ret, loss, model):
+    """What one training step hands its caller: the rendered rays (`ret`), the loss and the parameters after the optimizer step.
+    Per-sample arrays and the grids are larger than is useful to store, so they are reduced to a fixed seeded sample of
+    DUMP_SAMPLE elements (the same indices on every run and build); everything is float32, about 30 MB in all."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+
+    def put(name, t):
+        t = t.detach().reshape(-1)
+        if t.numel() > DUMP_SAMPLE:
+            g = torch.Generator().manual_seed(SEED)
+            idx = torch.randint(0, t.numel(), (DUMP_SAMPLE,), generator=g).to(t.device)
+            t = t[idx]
+        np.save(os.path.join(out_dir, name + '.npy'), t.float().cpu().numpy())
+
+    for k in DUMP_KEYS:
+        if isinstance(ret.get(k), torch.Tensor):
+            put(k, ret[k])
+    put('loss', loss.reshape(1))
+    for name, p in model.named_parameters():
+        put('param.' + name, p)
 
 
 # ----------------------------------------------------------------------------------------------------------
@@ -195,7 +214,7 @@ def cpu_reference_step(flavor, kwargs, stepsize, n_rays, threads, steps, warmup)
 
 
 def gpu_reference_step(flavor, kwargs, stepsize, steps, warmup, dev):
-    """SURVEY.md 8(d): "also time the patched reference CUDA path on the same B200 (the real competitor)".
+    """SURVEY.md 8(d): "also time the patched reference CUDA path on the same GPU (the real competitor)".
     The reference's GPU training step op for op: its Python algorithm (oracle.cpu_ref.model_forward on CUDA tensors: ATen
     grid_sample, cuBLAS rgbnet, index_add for torch_scatter) + the reference's OWN CUDA extension compiled from
     /root/reference into oracle/_ref (raw2alpha / alpha2weight / maskcache / cumdist / total_variation / masked Adam),
@@ -409,7 +428,10 @@ def main():
     ap.add_argument('--no-tma', action='store_true', help='(default; kept for old scripts)')
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-reference-gpu', action='store_true', help='skip the reference-GPU baseline leg (oracle/_ref + ATen) of the N = 1 line')
-    ap.add_argument('--only-timed', action='store_true', help='warm-up + timed region only (for ncu captures)')
+    ap.add_argument('--only-timed', action='store_true', help='warm-up + timed region only (for profiler captures)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last timed step computed as DIR/<name>.npy (float32; fixed seeded '
+                         'samples of the grids) for output-for-output comparison of two builds')
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == 'ours' else args.warmup
 
@@ -426,7 +448,6 @@ def main():
             if int(os.environ.get('RANK', '0')) == 0:
                 emit({'impl': args.impl, 'unavailable': 'the reference arm is defined for the training workloads (truck / bicycle) only'})
             return
-        args.steps = min(args.steps, 5)
         return render_workload(args, emit)
     from unboundednerfpytorch_b200 import dist as ubdist
     rank = int(os.environ.get('RANK', '0'))
@@ -457,7 +478,7 @@ def main():
         emit(line)
         return
 
-    # ------------------------------------------------------------------ informative: the reference's GPU path on this B200
+    # ------------------------------------------------------------------ informative: the reference's GPU path on this GPU
     if args.impl == 'reference-gpu':
         if rank != 0:
             return
@@ -525,7 +546,10 @@ def main():
     dev_batch = [t.to(dev) for t in host]
 
     tail_events = []
+    timing = [False]
     survivors = [N_RAYS * N_SAMPLES]
+    last = {}
+    record_last = [False]
 
     def train_step(ro, rd, vd, target, it):
         ret = model(ro, rd, vd, global_step=it, is_train=True, **rk)
@@ -552,6 +576,8 @@ def main():
             ubdist.reduce_tv_step(opt, tv_terms)
         ev[1].record()
         tail_events.append(ev)
+        if record_last[0]:                # --dump-outputs: keep the last timed step's results (only then)
+            last.update(ret=ret, loss=loss)
         return loss
 
     def sync_all():
@@ -574,9 +600,11 @@ def main():
 
     it = [0]
 
-    def dev_step(_):
+    def dev_step(i):
         it[0] += 1
+        record_last[0] = bool(args.dump_outputs) and timing[0] and i == args.steps - 1
         train_step(*dev_batch, it[0])
+        record_last[0] = False
 
     def e2e_step(_):
         it[0] += 1
@@ -594,12 +622,16 @@ def main():
     _cabi.TIMER = _cabi.KernelTimer()
     _cabi.reset_launch_count()
     del tail_events[:]
+    timing[0] = True
     ms_total = timed_region(dev_step, args.steps)
+    timing[0] = False
     tail_ms = sum(a.elapsed_time(b) for a, b in tail_events) / max(len(tail_events), 1)   # all-reduce + TV + Adam per step
     launches = _cabi.launch_count()
     ktimes = _cabi.TIMER.summary()
     _cabi.TIMER = None
     clk = clocks.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last['ret'], last['loss'], model)
     if args.only_timed:
         if rank == 0:
             emit({'only_timed': True, 'ms_per_step': ms_total / args.steps, 'gpu_launches': launches,
@@ -650,29 +682,22 @@ def main():
     # every nominal sample, the feature / rgbnet kernels only the M survivors of cumdist + mask cache + thresholds
     M = survivors[0]
     units = {k: (N_RAYS * N_SAMPLES if k.startswith('march_density') else M) for k in list(abytes) + list(aflops)}
-    traffic_src = 'profiles/traffic.json (static: dram__bytes_read.sum + dram__bytes_write.sum of the committed ncu --set full capture of this kernel on the truck workload, not re-measured in this run)'
 
     def kernel_roof(name, kms):
         if name in abytes:
             ach = abytes[name] * units[name] / (kms * 1e-3) / 1e9
-            traffic = load_traffic(name) if args.workload == 'truck' else None
-            out = {'kernel': name, 'bound': 'hbm', 'achieved': ach, 'peak': peak, 'unit': 'GB/s', 'frac': ach / peak,
-                   'traffic': traffic, 'traffic_source': traffic_src, 'kernel_ms': kms,
+            out = {'kernel': name, 'bound': 'hbm', 'achieved': ach, 'peak': peak, 'unit': 'GB/s', 'frac': ach / peak, 'kernel_ms': kms,
                    'algorithmic_bytes_per_sample': abytes[name], 'samples_per_launch': units[name], 'peak_source': peak_src}
-            if traffic:
-                # the physical side of the same launch: DRAM bytes of the committed ncu capture over this run's kernel time
-                out['dram_achieved'] = traffic / (kms * 1e-3) / 1e9
-                out['dram_frac'] = out['dram_achieved'] / peak
             if out['frac'] > 1.0:
                 out['note'] = ('frac > 1: SURVEY 8d counts every corner record of every sample as HBM traffic; neighbouring samples share '
                                'corners in L1 / L2 (and the scatter merges equal cells in registers), so the kernel moves fewer DRAM bytes '
-                               'than the model -- dram_frac is the physical utilisation')
+                               'than the model')
             return out
         ach = aflops[name] * units[name] / (kms * 1e-3) / 1e12
         return {'kernel': name, 'bound': 'tensor', 'achieved': ach, 'peak': tpeak, 'unit': 'TFLOP/s', 'frac': ach / tpeak,
-                'traffic': load_traffic(name) if args.workload == 'truck' else None, 'traffic_source': traffic_src, 'kernel_ms': kms,
+                'kernel_ms': kms,
                 'algorithmic_flops_per_sample': aflops[name], 'samples_per_launch': units[name],
-                'peak_source': tsrc, 'note': 'tcgen05 kind::tf32 with 3-pass split accumulation (fp32-grade, needed for the 1e-5 parity gate): useful FLOPs are '
+                'peak_source': tsrc, 'note': 'mma.sync TF32 with 3-pass split accumulation (fp32-grade, needed for the 1e-5 parity gate): useful FLOPs are '
                                              'counted once, the tensor pipe executes 3x that at half the bf16 rate; measured against the bf16 peak'}
 
     dom = max(ktimes, key=lambda k: ktimes[k][0]) if ktimes else None
@@ -709,7 +734,7 @@ def main():
             'note': 'NOT the headline: same step with one TF32 pass per product in the rgbnet forward and backward (opt-in training mode, '
                     'PSNR delta gated <= 0.01 dB in tests/test_gpu_models.py); the headline value computes at fp32 grade (3xTF32)'}
     if world == 1 and not args.no_reference_gpu:
-        # the real competitor (SURVEY.md 8d): the reference's GPU path on this same B200 -- its algorithm op by op with its own CUDA
+        # the real competitor (SURVEY.md 8d): the reference's GPU path on this same GPU -- its algorithm op by op with its own CUDA
         # extension (oracle/_ref) + ATen grid_sample + cuBLAS; a baseline leg like cpu_baseline, outside every timed region above
         try:
             torch.cuda.empty_cache()

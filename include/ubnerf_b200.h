@@ -1,5 +1,5 @@
 /*
- * ubnerf_b200.h -- C ABI of libubnerf_b200.so: the B200-native (sm_100a) replacement for the native
+ * ubnerf_b200.h -- C ABI of libubnerf_b200.so: the H100-native (sm_90a) replacement for the native
  * layer of sjtuytc/UnboundedNeRFPytorch's FourierGrid / DVGO rendering hot path.
  *
  * Boundary contract
@@ -309,9 +309,9 @@ int ubn_march_density_fwd(const float* rays_o, const float* rays_d, const float*
 int ubn_exclusive_scan_i32(const int32_t* in, int64_t n, int64_t* offsets, int64_t* scratch, void* stream);
 
 /* Which pass-B kernel family serves 12-channel channels-last feature grids: 0 = warp-cooperative (lane = corner x channel quad),
- * 1 = lane-per-sample for the forward, 2 = lane-per-sample for forward and backward, 3 (the default) / 4 / 5 = lane-per-sample
- * forward + slab-major cooperative scatter (FourierGrid k0 grids: one slab of the gradient live in L2 at a time), each slab swept in 1 / 2 / 4
- * x-ranges; 6 = as 3 with the gather that gives a sample three lanes (one per channel quad), 8 samples per instruction.  Same results to fp32 rounding (the
+ * 1 = lane-per-sample for the forward, 2 = lane-per-sample for forward and backward, 3 / 4 / 5 (the default) = lane-per-sample
+ * forward + slab-major cooperative scatter (FourierGrid k0 grids: one slab of the gradient live at a time), each slab swept in 1 / 2 / 4
+ * x-ranges (a quarter slab of the benchmarked grid fits the H100's L2); 6 = as 3 with the gather that gives a sample three lanes (one per channel quad), 8 samples per instruction.  Same results to fp32 rounding (the
  * lane-per-sample forward is bit-identical to F.grid_sample(...).mean(0)); process-wide, not thread-safe against concurrent
  * launches.  Returns cudaErrorInvalidValue for other values. */
 int ubn_set_feature_kernel(int variant);
@@ -369,15 +369,14 @@ int ubn_march_density_bwd(const float* rays_o, const float* rays_d, const float*
 int ubn_rgbnet_fwd(const float* feat, const float* view_bias, const int64_t* ray_id, const float* W1k, const float* W2,
                    const float* b2, const float* W3, const float* b3, int64_t n_pts, float* rgb, float* h1_save,
                    float* h2_save, void* stream);
-/* Same contract on the tensor cores: the two 128-wide layers run as tcgen05.mma (kind::tf32, M=128 sample tiles,
- * accumulators and the layer-2 A operand in tensor memory).  single_pass = 0: 3xTF32 split accumulation (fp32-grade,
- * meets the 1e-5 parity gate); single_pass bit 0: one TF32 pass (~1e-3 relative); bit 1: the 4-warp form of the kernel (A/B);
+/* Same contract on the tensor cores: the two 128-wide layers run as mma.sync m16n8k8 TF32 (16-sample units per warp,
+ * accumulators and the layer-2 A operand in registers).  single_pass = 0: 3xTF32 split accumulation (fp32-grade,
+ * meets the 1e-5 parity gate); single_pass bit 0: one TF32 pass (~1e-3 relative); bit 1: 4 warps per CTA instead of 8 (A/B);
  * bit 2: h1_save / h2_save are written in the PANEL layout [ceil(n_pts/128)][32 column quads][128 rows][4 floats] -- coalesced
- * for the row-per-thread kernels on both sides -- and must hold ceil(n_pts/128)*128 rows; only ubn_rgbnet_bwd_tc_fused called
+ * for the tensor-core fragments on both sides -- and must hold ceil(n_pts/128)*128 rows; only ubn_rgbnet_bwd_tc_fused called
  * with the same bit reads that layout.  h1_mask (bit 2 only; may be NULL): ceil(n_pts/128)*512 uint32 that receive the ReLU masks
- * of H1, [tile][32-unit chunk][row], bit = unit -- ubn_rgbnet_bwd_tc_fused then gates dH1 with them instead of loading H1 rows;
- * with masks, h1_save itself is written TRANSPOSED ([tile][32 sample quads][128 units][4 samples]) for its one remaining reader,
- * the dW2 launch of ubn_rgbnet_bwd_tc_fused (pass the same h1_mask there). */
+ * of H1, [tile][32-unit chunk][row], bit = unit -- ubn_rgbnet_bwd_tc_fused then gates dH1 with them instead of loading H1 rows
+ * (pass the same h1_mask there). */
 int ubn_rgbnet_fwd_tc(const float* feat, const float* view_bias, const int64_t* ray_id, const float* W1k, const float* W2,
                       const float* b2, const float* W3, const float* b3, int64_t n_pts, float* rgb, float* h1_save,
                       float* h2_save, uint32_t* h1_mask, int single_pass, void* stream);
@@ -389,8 +388,8 @@ int ubn_rgbnet_bwd(const float* feat, const int64_t* ray_id, const float* W1k, c
                    float* grad_W3, float* grad_b3, void* stream);
 
 /* Tensor-core backward, in two launches with the same net effect as ubn_rgbnet_bwd:
- *  ubn_rgbnet_bwd_tc_data : dZ2 -> dH1 = dZ2.W2 (tcgen05, A in tensor memory) -> dZ1 -> dz1_out[n_pts,128]; and
- *                           grad_W2 += dZ2^T.H1 (tcgen05 over shared-memory MN-major chunks; 3xTF32 split).
+ *  ubn_rgbnet_bwd_tc_data : dZ2 -> dH1 = dZ2.W2 (tensor cores, A in registers) -> dZ1 -> dz1_out[n_pts,128]; and
+ *                           grad_W2 += dZ2^T.H1 (split-K tensor-core GEMM over shared-memory chunks; 3xTF32 split).
  *  ubn_rgbnet_bwd_small   : from dz1: grad_feat, grad_view_bias (accumulated), grad_W1k, and grad_b2 / grad_W3 / grad_b3. */
 int ubn_rgbnet_bwd_tc_data(const float* W2, const float* W3, const float* rgb, const float* h1_save, const float* h2_save,
                            const float* grad_rgb, int64_t n_pts, float* dz1_out, float* grad_W2, void* stream);
@@ -399,17 +398,17 @@ int ubn_rgbnet_bwd_small(const float* feat, const int64_t* ray_id, const float* 
                          float* grad_view_bias, float* grad_W1k, float* grad_b2, float* grad_W3, float* grad_b3, void* stream);
 
 /* Tensor-core backward in two launches without any intermediate in HBM (same arguments and net effect as ubn_rgbnet_bwd):
- *  launch 1: dZ2 -> dH1 = dZ2.W2 -> dZ1 -> dX = dZ1.W1k (three tcgen05 GEMMs chained through tensor memory) -> grad_feat, and every
- *            reduction over samples except dW2 (grad_view_bias per ray, grad_W1k, grad_b2, grad_W3, grad_b3) from warp-transposed
- *            32 x 32 chunks of H2 / dZ1 held in shared memory;   launch 2: grad_W2 += dZ2^T.H1 (split-K tcgen05 GEMM).
+ *  launch 1: dZ2 -> dH1 = dZ2.W2 -> dZ1 -> dX = dZ1.W1k (three tensor-core GEMMs chained through registers) -> grad_feat, and every
+ *            reduction over samples except dW2 (grad_view_bias per ray, grad_W1k, grad_b2, grad_W3, grad_b3) as tensor-core GEMMs
+ *            over 16-sample tiles of H2 / dZ1 turned through shared memory;   launch 2: grad_W2 += dZ2^T.H1 (split-K tensor-core GEMM).
  * Replaces ubn_rgbnet_bwd_tc_data + ubn_rgbnet_bwd_small (which round-tripped dZ1 [n_pts,128] through HBM and re-read H2).
  * single_pass bit 0: one TF32 pass per product instead of the 3-pass split (the opt-in reduced-precision training mode);
- * bit 1: launch 1 without warp specialisation (4 warps do the tensor-core chain AND the sample reductions; A/B);
- * bit 2: h1_save / h2_save are in the panel layout of ubn_rgbnet_fwd_tc (not combinable with bit 1: cudaErrorInvalidValue).
+ * bit 1: launch 1 with 4 warps per CTA instead of 8 (A/B);
+ * bit 2: h1_save / h2_save are in the panel layout of ubn_rgbnet_fwd_tc.
  * h2_mask_scratch: NULL, or ceil(n_pts/128)*512 uint32 of scratch.  With bit 2 set and a scratch given, launch 1 leaves the ReLU
  * masks of H2 there ([tile][32-unit chunk][row], bit = unit) and launch 2 rebuilds dZ2 from them (dz3 . W3 gated by the mask)
  * instead of reading h2_save a second time.  h1_mask: NULL, or the masks ubn_rgbnet_fwd_tc wrote (bit 2 only): launch 1 then reads
- * 16 bytes per sample instead of the H1 row and fetches the next tile's H2 row half a tile ahead. */
+ * 16 bytes per sample instead of the H1 row. */
 int ubn_rgbnet_bwd_tc_fused(const float* feat, const int64_t* ray_id, const float* W1k, const float* W2, const float* W3,
                             const float* rgb, const float* h1_save, const float* h2_save, const float* grad_rgb, int64_t n_pts,
                             float* grad_feat, float* grad_view_bias, float* grad_W1k, float* grad_W2, float* grad_b2,

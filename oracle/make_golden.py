@@ -37,6 +37,7 @@ SEED = 777
 def _save(name, obj):
     os.makedirs(OUT, exist_ok=True)
     path = os.path.join(OUT, name)
+    os.makedirs(os.path.dirname(path), exist_ok=True)
     torch.save(obj, path)
     print(f'{name}: {os.path.getsize(path) / 1024:.1f} KiB')
 
@@ -224,7 +225,8 @@ def golden_models():
     rec = _grab(m, ret, lw)
     out['dvgo'] = dict(kwargs=kw, state=m.state_dict(), rays_o=ro, rays_d=rd, viewdirs=vd, render_kwargs=rk2, loss_w=lw,
                        ret=rec, stepdist=0.5 * float(m.voxel_size), sample=[_c(t) for t in samp])
-    _save('l2_models.pt', out)
+    for k, rec in out.items():                 # one file per model record (tests.util.load_golden('l2_models.pt') reassembles them)
+        _save(os.path.join('l2_models', k + '.pt'), rec)
 
 
 from tests.util import cfg1_scene  # noqa: E402  (seeded scene shared with tests/test_gpu_models.py)

@@ -10,7 +10,7 @@
  * Parity pinning: the reference ships NO tests / golden vectors (SURVEY.md section 4), so this
  * restatement is pinned by (a) running the reference's own Python model files here on CPU on top
  * of these functions (oracle/stubs.py -> tests/golden/, script oracle/make_golden.py) and (b) the
- * reference's own CUDA extension compiled for sm_100a (oracle/_ref/, `make ref`) run on the GPU box.
+ * reference's own CUDA extension compiled for sm_90a (oracle/_ref/, `make ref`) run on the GPU.
  *
  * Numerics notes (SURVEY.md Appendix A): device code in the reference is compiled by nvcc with
  * default -fmad=true, so `a*b + c` is contracted into one fma; this file is compiled with

@@ -1,6 +1,6 @@
 // Is sincosf(a) bit-identical to (sinf(a), cosf(a)) on this toolchain / GPU for every float |a| <= 8 (the argument range of the
 // FourierGrid warps 2^k x, |x| <= 1, k <= 3)?  If so the march kernels may share one range reduction per (axis, frequency).
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a scripts/probe_sincos.cu -o scripts/_bin/probe_sincos && scripts/_bin/probe_sincos
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a scripts/probe_sincos.cu -o scripts/_bin/probe_sincos && scripts/_bin/probe_sincos
 #include <cstdio>
 #include <cstdint>
 __global__ void k(unsigned long long* bad_s, unsigned long long* bad_c, uint32_t max_bits) {
@@ -23,7 +23,7 @@ int main() {
   cudaMalloc(&d, 16);
   cudaMemcpy(d, h, 16, cudaMemcpyHostToDevice);
   const uint32_t max_bits = 0x41000000u;   // 8.0f
-  k<<<148 * 16, 256>>>(d, d + 1, max_bits);
+  k<<<132 * 16, 256>>>(d, d + 1, max_bits);
   cudaMemcpy(h, d, 16, cudaMemcpyDeviceToHost);
   printf("{\"probe\": \"sincosf vs sinf/cosf, all floats |a| <= 8\", \"n\": %llu, \"sin_mismatch\": %llu, \"cos_mismatch\": %llu, \"err\": \"%s\"}\n",
          2ull * ((unsigned long long)max_bits + 1), h[0], h[1], cudaGetErrorString(cudaGetLastError()));

@@ -1,5 +1,4 @@
-"""Shared machinery of the at-size parity tests (tests/test_gpu_parity_at_size.py) and of the diagnostic script
-scripts/parity_at_size_report.py: run the BENCHMARKED configurations (bench.py's workloads, 8192 rays x 512 samples) through
+"""Machinery of the at-size parity tests (tests/test_gpu_parity_at_size.py): run the BENCHMARKED configurations (bench.py's workloads, 8192 rays x 512 samples) through
 
   (a) this library's fused CUDA path (models.*.forward + loss + backward), and
   (b) the reference's GPU path op for op: oracle.cpu_ref.model_forward on CUDA tensors with ext = the reference's OWN CUDA

@@ -32,10 +32,10 @@ def test_abi_version_and_counters():
     assert _cabi.launch_count() == 0
 
 
-def test_only_sm100a_code_in_library():
-    """The shipped library carries sm_100a SASS only (no multi-arch fatbin, no PTX-JIT fallback for other GPUs)."""
+def test_only_sm90a_code_in_library():
+    """The shipped library carries sm_90a SASS only (no multi-arch fatbin, no PTX-JIT fallback for other GPUs)."""
     import subprocess
     from unboundednerfpytorch_b200 import build
     out = subprocess.run(['cuobjdump', '-lelf', build.build()], capture_output=True, text=True).stdout
     archs = set(re.findall(r'sm_(\d+a?)', out))
-    assert archs == {'100a'}, archs
+    assert archs == {'90a'}, archs

@@ -139,7 +139,7 @@ def test_unmodified_reference_callers_run_on_this_library(ref_modules, flavor):
             m.k0_total_variation_add_grad(1e-7 / N, True)
         # gradients (incl. the TV term) before the optimiser.  density.grid does not pass through the ReLU MLP: tight.  k0.grid and
         # the rgbnet do: a pre-activation within fp32 rounding of zero flips its ReLU mask between cuBLAS (reference) and the
-        # tcgen05 kernels (ours), which changes that sample's contribution (tests/parity_at_size.py quantifies this against fp64)
+        # tensor-core kernels (ours), which changes that sample's contribution (tests/parity_at_size.py quantifies this against fp64)
         ref_sd, ours_named = dict(ref.named_parameters()), dict(ours.named_parameters())
         assert _stat(ours_named['density.grid'].grad, ref_sd['density.grid'].grad) <= 2e-5
         gk, gr = ours_named['k0.grid'].grad, ref_sd['k0.grid'].grad

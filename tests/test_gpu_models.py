@@ -223,7 +223,7 @@ def test_training_step_reduces_loss():
 
 @pytest.mark.parametrize('mode', ['simt', 'tc3', 'tc3w4', 'tc1', 'tc3+tcbwd', 'tc3+fused', 'tc3+fusedh2', 'tc3+fused4', 'tc1+fused'])
 def test_fused_rgbnet_vs_torch(mode, monkeypatch):
-    """csrc/shade.cu (fp32 FFMA) and csrc/shade_tc.cu (tcgen05: 3xTF32 fp32-grade, single-pass TF32 preview) vs the torch
+    """csrc/shade.cu (fp32 FFMA) and csrc/shade_tc.cu (tensor cores: 3xTF32 fp32-grade, single-pass TF32 preview) vs the torch
     nn.Sequential they replace: forward and every gradient."""
     from unboundednerfpytorch_b200 import models, shade as shade_mod
     monkeypatch.setattr(shade_mod, 'BWD_MODE', {'tcbwd': 'tc3', 'fused': 'fused', 'fusedh2': 'fused', 'fused4': 'fused4'}.get(mode.split('+')[-1], 'simt'))
@@ -308,11 +308,10 @@ def test_density_scatter_variants_agree(flavor, F_, thres):
 
 
 def test_rgbnet_dw2_long_sample_sum_vs_fp64():
-    """dW2 = sum over ALL samples of dZ2^T H1 is a split-K tensor-core GEMM.  tcgen05 adds into its fp32 accumulator with
-    truncation, so one accumulator chain per CTA over hundreds of 32-sample rounds carries a bias that grows linearly with the
-    chain (measured at size in round 2: 1.4e-4 of scale at 295 rounds per CTA, 4.5e-5 at 91, against 2.6e-6 for cuBLAS).
-    k_shade_dw2_tc therefore restarts the MMA accumulator every 4 rounds and keeps an fp32 round-to-nearest running sum in a
-    second block of tensor memory.  This test makes the chains long (1.2 M samples, ~130 rounds per CTA) and judges dW2 -- and
+    """dW2 = sum over ALL samples of dZ2^T H1 is a split-K tensor-core GEMM.  A tensor-core fp32 accumulator need not round to
+    nearest, so one accumulator chain per CTA over hundreds of 32-sample chunks could carry a bias that grows linearly with the
+    chain.  k_shade_dw2_tc therefore restarts the MMA accumulator every 32-sample chunk and keeps an fp32 round-to-nearest
+    running sum in registers.  This test makes the chains long (1.2 M samples, ~280 chunks per CTA) and judges dW2 -- and
     the other sample sums -- against an fp64 evaluation at 1e-5 of the tensor scale."""
     from unboundednerfpytorch_b200 import models, shade as shade_mod
     assert shade_mod.MODE == 'tc3' and shade_mod.BWD_MODE == 'fused'
@@ -505,6 +504,7 @@ def test_feature_kernel_families_agree(flavor, F_, thres):
     ro, rd, vd = seeded_rays(700, 12, DEV)
     rk = dict(near=0., far=1e9, bg=1, rand_bkgd=False, stepsize=0.5, render_depth=True)
     outs, grads = [], []
+    default = ops.get_feature_kernel()
     try:
         for variant in (0, 1, 2, 3, 4, 5, 6):
             ops.set_feature_kernel(variant)
@@ -515,7 +515,7 @@ def test_feature_kernel_families_agree(flavor, F_, thres):
             outs.append(ret)
             grads.append(m.k0.grid.grad.detach().clone())
     finally:
-        ops.set_feature_kernel(3)
+        ops.set_feature_kernel(default)
     for ret in outs[1:]:
         assert torch.equal(ret['ray_id'], outs[0]['ray_id']) and torch.equal(ret['step_id'], outs[0]['step_id'])
         for k in ('weights', 'raw_density', 't'):
@@ -537,7 +537,7 @@ def test_feature_kernel_families_agree(flavor, F_, thres):
             try:
                 (w, last, alpha, dens, k0, ray_id, step_id, t, inner), _ = m._march(ro, rd, 0.5)
             finally:
-                ops.set_feature_kernel(3)
+                ops.set_feature_kernel(default)
             pts, _, _ = m._sample_dense(ro, rd, 0.5)
             want = cpu_ref.fourier_grid_forward(m.k0.grid.detach().contiguous(), pts[ray_id, step_id], m.xyz_min, m.xyz_max,
                                                 F_ if flavor == 'fouriergrid' else 0)

@@ -16,7 +16,7 @@ asserted instead (each measured, see tests/parity_at_size.py and DESIGN.md secti
 * the grid scatters are fp32 atomics in the reference too (ATen grid_sampler_3d_backward): the reference differs from ITSELF from
   run to run.  density.grid grad: within max(1e-5 of scale, 3 x the reference's own run-to-run difference).
 * gradients through the ReLU MLP (k0.grid, rgbnet.*): a pre-activation within rounding distance of zero flips its ReLU mask
-  between ANY two fp32 implementations (cuBLAS vs tcgen05 vs exact), changing that sample's whole contribution.  Judged against
+  between ANY two fp32 implementations (cuBLAS vs tensor-core 3xTF32 vs exact), changing that sample's whole contribution.  Judged against
   an fp64 evaluation of the reference's algorithm: this library deviates from it no more than the reference's fp32 GPU path
   does (max error within 3x, count of elements beyond 1e-5 of scale within 3x), and beyond-tolerance elements vs the reference
   stay below 1e-3 of the tensor."""

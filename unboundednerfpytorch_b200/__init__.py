@@ -1,4 +1,4 @@
-"""unboundednerfpytorch_b200 -- B200-native (sm_100a) volumetric-rendering hot path for the FourierGrid / DVGO
+"""unboundednerfpytorch_b200 -- H100-native (sm_90a) volumetric-rendering hot path for the FourierGrid / DVGO
 models of sjtuytc/UnboundedNeRFPytorch, behind the reference's own extension / autograd / module surface.
 
 Layout: ``csrc/`` hand-written CUDA + the C ABI (include/ubnerf_b200.h) -> ``libubnerf_b200.so``;

@@ -1,4 +1,4 @@
-"""Build libubnerf_b200.so (hand-written sm_100a CUDA + the C ABI of include/ubnerf_b200.h) in-tree.
+"""Build libubnerf_b200.so (hand-written sm_90a CUDA + the C ABI of include/ubnerf_b200.h) in-tree.
 
     python -m unboundednerfpytorch_b200.build [--force]
 
@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libubnerf_b200.so')
 SOURCES = ['ray_ops.cu', 'alpha_ops.cu', 'grid_sweep.cu', 'trilinear.cu', 'march.cu', 'march_feature.cu', 'shade.cu', 'shade_tc.cu', 'ray_gen.cu', 'loss.cu', 'grid_utils.cu', 'render_tma.cu']
 HEADERS = ['common.cuh', 'trilinear.cuh', 'march_common.cuh', os.path.join('..', '..', 'include', 'ubnerf_b200.h')]
-NVCC_FLAGS = ['-std=c++17', '-O3', '-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo',
+NVCC_FLAGS = ['-std=c++17', '-O3', '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo',
               '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=hidden', '--cudart', 'static']
 
 
@@ -34,7 +34,7 @@ def _stale():
 
 
 def build(force=False, verbose=False):
-    """Compile every .cu of the package for sm_100a into one shared object. Returns its path."""
+    """Compile every .cu of the package for sm_90a into one shared object. Returns its path."""
     if not (force or _stale()):
         return LIB
     objdir = os.path.join(HERE, 'build')
@@ -55,7 +55,7 @@ def build(force=False, verbose=False):
         if p.returncode:
             raise RuntimeError(f'nvcc failed on {s}')
         objs.append(obj)
-    cmd = [nvcc, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a', '--cudart', 'static']
+    cmd = [nvcc, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a', '--cudart', 'static']
     subprocess.check_call(cmd)
     return LIB
 

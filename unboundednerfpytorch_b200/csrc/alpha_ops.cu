@@ -4,7 +4,7 @@
 //
 // raw2alpha*: streaming elementwise, one thread per element, coalesced.
 // alpha2weight*: the reference walks each ray with ONE thread (8192 threads total at the benchmark
-//   size = 32 blocks on a 148-SM part, stride-S uncoalesced).  The transmittance recurrence
+//   size = 32 blocks on a 132-SM H100, stride-S uncoalesced).  The transmittance recurrence
 //   T <- float(double(T) * (1. - double(alpha))) with its early stop at T < 1e-3 is order sensitive, so
 //   the sequential evaluation is kept bit-for-bit (i_end is an index output = bit-exact parity target),
 //   but re-mapped: one LANE per ray, 32 rays per warp, 32x32 tiles staged through shared memory so all

@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for libubnerf_b200.so (sm_100a only).
+// common.cuh -- shared helpers for libubnerf_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -7,7 +7,7 @@
 
 namespace ubn {
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSMs = 132;  // H100 SXM
 
 extern thread_local cudaError_t g_last_error;
 void count_launch();

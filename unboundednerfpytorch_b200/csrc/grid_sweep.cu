@@ -502,9 +502,9 @@ static bool launch_tv_stream(const float* param, float* grad, float wy, float wz
   s.sz_i = (int)sz_i; s.sz_j = (int)sz_j; s.row4 = (int)row4; s.inner4 = (int)(inner / 4);
   s.tj = (int)std::max<int64_t>(1, (kTvsThreads * kTvsCols) / row4);
   s.n_jt = (int)((sz_j + s.tj - 1) / s.tj);
-  // enough CTAs for ~8 waves of 2 x 148 resident CTAs, segments no shorter than 16 planes (one halo plane each)
+  // enough CTAs for ~8 waves of 2 x kNumSMs resident CTAs, segments no shorter than 16 planes (one halo plane each)
   const int64_t tiles = lead * s.n_jt;
-  int64_t n_seg = (8 * 2 * 148 + tiles - 1) / tiles;
+  int64_t n_seg = (8 * 2 * kNumSMs + tiles - 1) / tiles;
   n_seg = std::max<int64_t>(1, std::min<int64_t>(n_seg, sz_i / 16));
   s.seg_len = (int)((sz_i + n_seg - 1) / n_seg);
   s.n_seg = (int)((sz_i + s.seg_len - 1) / s.seg_len);
@@ -602,7 +602,7 @@ int ubn_tv_adam_pingpong(const float* param, float* param_out, float* grad, floa
   s.tj = (int)std::max<int64_t>(1, kTaThreads / row4);
   s.n_jt = (int)((sz_j + s.tj - 1) / s.tj);
   const int64_t tiles = lead * s.n_jt;
-  int64_t n_seg = (8 * 2 * 148 + tiles - 1) / tiles;
+  int64_t n_seg = (8 * 2 * kNumSMs + tiles - 1) / tiles;
   n_seg = std::max<int64_t>(1, std::min<int64_t>(n_seg, sz_i / 16));
   s.seg_len = (int)((sz_i + n_seg - 1) / n_seg);
   s.n_seg = (int)((sz_i + s.seg_len - 1) / s.seg_len);

@@ -102,7 +102,7 @@ __global__ void __launch_bounds__(kLossThreads) k_render_loss(
 __global__ void k_render_loss_finish(const double* __restrict__ partial, int n_blocks, int64_t n_rays, float w_main,
                                      float w_entropy, float w_rgbper, float w_freq, float* __restrict__ out) {
   // one warp, fixed order (lane-strided partial sums, then a fixed shuffle tree): deterministic like the single-thread loop it
-  // replaces, which took 92 us for its 592 dependent loads (launch list, profiles/r02_launches_truck.csv)
+  // replaces, whose 592 dependent loads made it one long serial chain
   if (blockIdx.x != 0 || threadIdx.x >= 32) return;
   double a = 0, b = 0, c = 0, e = 0;
   for (int i = threadIdx.x; i < n_blocks; i += 32) { a += partial[4 * i]; b += partial[4 * i + 1]; c += partial[4 * i + 2]; e += partial[4 * i + 3]; }

@@ -241,9 +241,9 @@ constexpr int kMaxChunks = 128;   // S <= 4096
 // kRuns (kP > 0 only): the scatter is a SECOND phase with lane = a run of consecutive samples of the ray.  Phase 1 (reverse scan,
 // lane = sample of a 32-sample chunk) parks the per-sample density gradients in shared memory; in phase 2 every lane walks its
 // ceil(S / 32) consecutive samples slab by slab and keeps the cell it is in open in registers (cell index + its 8 corner sums):
-// samples that stay in the cell -- 40 % of the steps in slab 0 and the lowest sin / cos slabs at half-voxel spacing -- are added in
+// samples that stay in the cell -- a large share of the steps in slab 0 and the lowest sin / cos slabs at half-voxel spacing -- are added in
 // registers, and a cell leaves as four pair reductions only when the ray moves on.  The scatter is bound by the count of L2
-// reduction requests (ncu: 226 M requests, 0.32 sector / slice / clock, issue 21 %), so fewer requests is the only lever.
+// reduction requests (profiled: the L2 reduction path saturates while issue stays low), so fewer requests is the only lever.
 template <int kP, bool kRuns>
 __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_bwd(
     const float* __restrict__ rays_o, const float* __restrict__ rays_d, const float* __restrict__ t_table,
@@ -289,8 +289,8 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_bwd(
     const float wt = valid ? weight[i] : 0.f;
     // reverse sequential accumulation over the scanned samples (alpha2weight_backward order).  The chain is inherently serial
     // (one fp32 fma per scanned sample, in the reference's order), so every lane runs it redundantly on warp-uniform operands.
-    // They used to be fetched with two shuffles per sample from a data-dependent lane (ncu, round 2: mio_throttle + short
-    // scoreboard = 55 % of the kernel's stall samples); now the chunk's 32 (grad, weight) pairs go through 256 bytes of shared
+    // They used to be fetched with two shuffles per sample from a data-dependent lane (profiled: mio_throttle + short
+    // scoreboard stalls dominated); now the chunk's 32 (grad, weight) pairs go through 256 bytes of shared
     // memory and come back as 16 broadcast LDS.128 in a fully unrolled loop.
     const unsigned m = __ballot_sync(0xffffffffu, (f & UBN_FLAG_SCANNED) != 0);
     float my_back = 0.f;

@@ -37,7 +37,7 @@ struct Ray {
 
 // ||v|| exactly as torch's CUDA reduction evaluates x.norm(dim=-1) on 3-vectors: the lanes of the reduced
 // dimension are combined by a shuffle tree, i.e. sqrt((x*x + z*z) + y*y) with every product and sum rounded
-// separately (probed on B200: 0 mismatches in 2^20 random vectors; the "natural" orders mismatch in 12-15 %).
+// separately (scripts/probe_mean_order.py-style probe against torch: the "natural" orders do not match).
 // The reference runs these norms as torch ops (dcvgo.py:240,253,288; FourierGrid_model.py:523,537), so matching
 // them bit-for-bit keeps the threshold decisions downstream (inner mask, cumdist, mask-cache rounding) identical.
 __device__ __forceinline__ float norm3_torch(float x, float y, float z) {
@@ -94,8 +94,8 @@ __device__ __forceinline__ CellR make_cell(float cx, float cy, float cz, int X, 
 
 // Visit the kP slabs of a FourierGrid in natural order with their continuous source indices.  Slabs 2k+1 / 2k+2 are sin / cos
 // of the SAME argument 2^k x, so one sincosf per (axis, frequency) serves both: half the range reductions of separate sinf / cosf
-// calls.  sincosf is bit-identical to the pair on this toolchain for every float |a| <= 8 (scripts/probe_sincos.cu, run on the
-// B200: 0 mismatches in 2.18e9 arguments), so every coordinate -- and with it raw_density -- keeps its bits.
+// calls.  sincosf is bit-identical to the pair on this toolchain for every float |a| <= 8 (scripts/probe_sincos.cu checks all
+// 2.18e9 arguments), so every coordinate -- and with it raw_density -- keeps its bits; the at-size parity tests pin it.
 template <int kP, typename F>
 __device__ __forceinline__ void for_each_slab(const GridView& g, float nx, float ny, float nz, F&& f) {
   f(0, src_index(nx, g.X), src_index(ny, g.Y), src_index(nz, g.Z));

@@ -1,7 +1,7 @@
 // march_feature.cu -- pass B of the fused march (feature-grid read for the surviving samples and its adjoint),
 // second generation.  Same outputs as k_march_feature in march.cu (kept as the generic fallback); restructured after
-// the first ncu capture (profiles/r01_*): the first version ran at 43 % of the algorithmic roofline with an L1 hit
-// rate below 1 % (its per-warp staging buffers forced a 200 KB shared-memory carve-out and every sample touched all P
+// profiling the first version, which ran far below the algorithmic roofline with almost no L1
+// hits (its per-warp staging buffers forced a 200 KB shared-memory carve-out and every sample touched all P
 // slabs before the next sample re-touched the same voxels) and one load in flight per warp.  Here:
 //   * no shared memory at all: the per-(sample, slab) cell (base voxel + 3 fractions) lives in the registers of the
 //     lane that owns the sample and is broadcast with warp shuffles -> the whole 228 KB stays L1;
@@ -186,8 +186,7 @@ static int launch_v2(bool backward, const float* rays_o, const float* rays_d, co
 // =====================================================================================================================
 // Third generation: LANE = SAMPLE.  The cooperative kernels above spend one warp instruction per (sample, slab) -- 24 of 32
 // lanes fetch the 8 x 48-byte corner records of ONE sample, then 12 shuffles reduce the corners: ~17 issue slots and 4 broadcast
-// shuffles per sample-slab, few independent loads in flight per warp (ncu, round 1: issue 46 % busy, DRAM 19 %, 29 % of the
-// warps resident, long-scoreboard bound).  Here every lane owns one surviving sample of the chunk and walks its own 8 corners:
+// shuffles per sample-slab, few independent loads in flight per warp (profiled: few warps resident, long-scoreboard bound).  Here every lane owns one surviving sample of the chunk and walks its own 8 corners:
 //   * 24 independent 128-bit loads per lane and slab (8 corners x 3 channel quads), no shuffles, no cross-lane reduction:
 //     ~4.7 issue slots per sample-slab, and 8-24 loads in flight per LANE instead of per warp;
 //   * adjacent lanes are adjacent samples of a ray (half a voxel apart), so the same-corner loads of a warp instruction
@@ -326,7 +325,7 @@ __global__ void __launch_bounds__(32 * kMarchWarps, 4) k_march_feature_v3(
 
 // =====================================================================================================================
 // Fourth generation of the gather: EIGHT samples per instruction, three lanes per sample (lane = sample j of 8, channel quad q).
-// The lane-per-sample kernel above is bound by L1 wavefronts (ncu: l1tex 68 %, issue 21 %): one LDG.128 of its 24 per slab sends
+// The lane-per-sample kernel above is bound by L1 wavefronts: one LDG.128 of its 24 per slab sends
 // 32 lanes to up to 32 different 128-byte lines.  Here the three quad lanes of a sample read the 48 contiguous bytes of ONE
 // corner record, so an instruction touches 8 records instead of 32 and a slab costs 8 load instructions per 8 samples.  The
 // accumulation stays inside the lane (4 channels of its quad over the 8 corners in ATen's order, slabs in torch-CUDA's mean
@@ -460,10 +459,10 @@ static int launch_v3(bool backward, const float* rays_o, const float* rays_d, co
 
 // =====================================================================================================================
 // Slab-major scatter (variant 3).  The k0 gradient of the truck workload is 9 slabs x 172 MB: with the slab loop inside the
-// kernel every resident warp spreads its reductions over all 1.55 GB, so the 126 MB L2 holds 8 % of the live footprint and
-// nearly every vector reduction costs a DRAM sector fetch + write-back at random addresses (ncu, round 1: 8.9 GB of DRAM
-// traffic, L2 hit 51 %).  Here the SLAB is the slow grid dimension (blockIdx.y): the CTAs of slab s are scheduled before the
-// CTAs of slab s + 1, the live gradient footprint at any moment is ONE slab (73 % of it L2-resident), and every sector of a
+// kernel every resident warp spreads its reductions over all 1.55 GB, far more than the L2 holds, and nearly every vector
+// reduction costs a DRAM sector fetch + write-back at random addresses.  Here the SLAB is the slow grid dimension
+// (blockIdx.y): the CTAs of slab s are scheduled before the CTAs of slab s + 1, the live gradient footprint at any moment is
+// ONE slab (172 MB; split in x-ranges by variants 4 / 5 to fit the H100's 50 MB L2), and every sector of a
 // slab goes to DRAM about once.  Cost: the chunk preamble (flags, sample point, compaction) runs once per slab instead of
 // once, and the 48-byte gradient rows are re-read 9 times (coalesced, L2 hits after the first slab).  Same lane roles and
 // the same addends as k_march_feature_v2<.., true, ..>: the gradients differ only by the atomics' summation order.
@@ -474,8 +473,8 @@ __global__ void __launch_bounds__(32 * kMarchWarps, kMinBlocks) k_march_feature_
     GridView g, MarchParams p, int64_t n_rays, const uint8_t* __restrict__ flags,
     const int64_t* __restrict__ offsets, const float* __restrict__ gfeat, float* __restrict__ grad_grid, int n_split) {
   // n_split > 1: every slab is swept n_split times, pass `part` scattering only the samples whose cell starts in the part-th
-  // x-range of the slab, so the live gradient footprint is 1 / n_split of a slab (86 MB for two parts of a 153^3 x 12 slab:
-  // inside the 126 MB L2) at the price of repeating the chunk preamble
+  // x-range of the slab, so the live gradient footprint is 1 / n_split of a slab (86 / 43 MB for two / four parts of a
+  // 153^3 x 12 slab; the H100's L2 is 50 MB) at the price of repeating the chunk preamble
   const int lane = threadIdx.x & 31;
   const int sl = blockIdx.y / n_split, part = blockIdx.y - sl * n_split;
   const int v_lo = (int)(((int64_t)(g.X - 1) * part) / n_split) * g.Y * g.Z;
@@ -531,12 +530,11 @@ __global__ void __launch_bounds__(32 * kMarchWarps, kMinBlocks) k_march_feature_
       }
       // Consecutive samples of a ray are half a voxel apart in slab 0 and at most that in the sin / cos slabs of the lowest
       // frequency, so neighbours of a group often fall into the SAME cell: their contributions are added in registers and leave as
-      // one vector reduction (the scatter is bound by the number of L2 reduction sectors, ncu: 0.38 sector per slice and clock
-      // with every other unit below 60 %).  The cell index is warp-uniform after the shuffle, so the test costs no divergence.
+      // one vector reduction (the scatter is bound by the number of L2 reduction sectors).  The cell index is warp-uniform after the shuffle, so the test costs no divergence.
       // (Handing the shared FACE of two neighbouring cells over the same way -- four of eight corners, one xor-shuffle per float --
-      // was measured slower: 3.38 vs 2.97 ms.  Half-populated reduction instructions do not halve the cost of an instruction.  So was
-      // a run-length merge carried across groups and chunks: 3.49 ms -- the open run serialises the group's reductions; and so was
-      // pairing neighbours 16 positions apart with alternating issue: 3.08 ms -- fewer merges, and nothing gained from spacing.)
+      // was measured slower: half-populated reduction instructions do not halve the cost of an instruction.  So was a run-length
+      // merge carried across groups and chunks -- the open run serialises the group's reductions; and so was pairing neighbours
+      // 16 positions apart with alternating issue -- fewer merges, and nothing gained from spacing.)
       int vj[kGroup];
       float4 val[kGroup];
 #pragma unroll
@@ -575,7 +573,7 @@ static int launch_bwd_slab(const float* rays_o, const float* rays_d, const float
                            int64_t n_rays, const uint8_t* flags, const int64_t* offsets, const float* gfeat, float* grad_grid,
                            int n_split, cudaStream_t st) {
   const dim3 grid(blocks_for(n_rays, kMarchWarps), kP * n_split);
-  // 8 resident blocks (64 registers) and 1 / P folded into the corner weight: 2.88 vs 2.97 ms (gpu_call_36; groups of 8: 2.93 ms)
+  // 8 resident blocks (64 registers) and 1 / P folded into the corner weight: measured faster than fewer blocks and than groups of 8
   k_march_feature_bwd_slab<kP, 4, 8, true><<<grid, 32 * kMarchWarps, 0, st>>>(rays_o, rays_d, t_table, g, p, n_rays, flags, offsets, gfeat, grad_grid,
                                                                               n_split);
   UBN_LAUNCH_CHECK();
@@ -586,16 +584,16 @@ static int launch_bwd_slab(const float* rays_o, const float* rays_d, const float
 //   0  warp-cooperative gather and scatter (k_march_feature_v2)
 //   1  lane-per-sample gather (k_march_feature_v3) + cooperative scatter
 //   2  lane-per-sample gather and scatter
-//   3  (default) lane-per-sample gather -- the 8-samples-per-instruction k_march_feature_v4 for single-slab grids -- + SLAB-MAJOR
+//   3  lane-per-sample gather -- the 8-samples-per-instruction k_march_feature_v4 for single-slab grids -- + SLAB-MAJOR
 //      cooperative scatter with the equal-cell merge (k_march_feature_bwd_slab)
-//   4 / 5  as 3 with every slab swept in 2 / 4 x-ranges
+//   4 / 5  as 3 with every slab swept in 2 / 4 x-ranges (5 = default)
 //   6  as 3 with k_march_feature_v4 for every slab count
 // The scatter stays cooperative: one warp instruction issues the 24 vector reductions of a sample into 8 x 48 contiguous bytes,
 // whereas lane-per-sample reductions hit 32 unrelated records per instruction.
-// Measured on the truck workload (8192 x 512, 9 slabs; profiles/README.md): gather 3.94 ms (0) -> 1.55 ms (1, 3) / 1.84 ms (6);
-// scatter 4.20 ms (0, 1), 7.48 ms (2), 3.76 ms slab-major -> 2.97 ms with the merge -> 2.88 ms at 8 resident blocks (3),
-// 4.40 / 5.34 ms (4 / 5: the repeated preamble costs more than the L2 hits return).  Bicycle (1 slab): gather 0.255 (v3) -> 0.204 ms (v4).
-static int g_feature_kernel = 3;
+// Scatter of the truck workload (8192 x 512, 9 slabs of 172 MB) on one H100 80GB HBM3 at a 400 W power limit, two alternating
+// runs of bench.py --only-timed --feature-kernel V: 6.61 / 6.61 ms (3), 6.19 / 6.17 ms (4), 5.98 / 5.98 ms (5).  A quarter slab
+// (43 MB) fits the 50 MB L2, and that saves more than the repeated chunk preamble costs, so 5 is the default.
+static int g_feature_kernel = 5;
 void set_feature_kernel(int v) { g_feature_kernel = v; }
 int get_feature_kernel() { return g_feature_kernel; }
 
@@ -617,9 +615,9 @@ int march_feature_v2(bool backward, const float* rays_o, const float* rays_d, co
       default: break;
     }
   }
-  // 8 samples x 3 channel quads per instruction: explicitly (6), and by default (3) for single-slab grids, where it measured 0.204 vs
-  // 0.255 ms (bicycle); on the 9-slab FourierGrid the shuffled cells cost more than the wavefronts save (1.84 vs 1.55 ms)
-  if (g.C == 12 && !backward && (g_feature_kernel == 6 || (g_feature_kernel == 3 && g.P == 1))) {
+  // 8 samples x 3 channel quads per instruction: explicitly (6), and with 3 / 4 / 5 (5 = default) for single-slab grids, where it
+  // measured faster than the lane-per-sample gather; on the 9-slab FourierGrid the shuffled cells cost more than the wavefronts save
+  if (g.C == 12 && !backward && (g_feature_kernel == 6 || (g_feature_kernel >= 3 && g_feature_kernel <= 5 && g.P == 1))) {
     switch (g.P) {
       case 1: return launch_v4<1>(rays_o, rays_d, t_table, g, p, n_rays, flags, offsets, density, alpha, weight, feat, o_density, o_alpha, o_weight, o_ray_id, o_step_id, o_t, o_inner, st);
       case 3: return launch_v4<3>(rays_o, rays_d, t_table, g, p, n_rays, flags, offsets, density, alpha, weight, feat, o_density, o_alpha, o_weight, o_ray_id, o_step_id, o_t, o_inner, st);

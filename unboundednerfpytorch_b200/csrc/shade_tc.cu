@@ -1,1869 +1,635 @@
-// shade_tc.cu -- rgbnet forward on the 5th-generation tensor cores (tcgen05 + TMEM), sm_100a only.
+// shade_tc.cu -- rgbnet forward and backward on the Hopper tensor cores (mma.sync m16n8k8, kind TF32), sm_90a.
 //
-// Same contract as k_shade_fwd (shade.cu): rgb = sigmoid(W3 relu(W2 relu(W1k x + vb[ray]) + b2) + b3), one persistent
-// CTA per SM, 128-sample tiles, weights resident in shared memory -- but the two wide layers run as tcgen05.mma
-// (M = 128 samples, N = 128 hidden units, kind::tf32, fp32 accumulation in tensor memory):
+// Same contract as k_shade_fwd / k_shade_bwd (shade.cu): rgb = sigmoid(W3 relu(W2 relu(W1k x + vb[ray]) + b2) + b3).
+// Every warp owns 16-sample units and keeps the whole activation chain in registers: the accumulator fragment of one
+// layer IS the A fragment of the next.  mma.m16n8k8 gives thread (g = lane / 4, t = lane % 4) the accumulator elements
+// (row g, columns 2t, 2t + 1) and (row g + 8, same columns) of each 8-column tile, and wants A elements (row g, k = t) and
+// (row g, k = t + 4).  The contraction order is free, so k-step s reads hidden units 8 s + 2 t as "k = t" and 8 s + 2 t + 1
+// as "k = t + 4": the layer-1 accumulators of column tile s are the layer-2 A operand of k-step s without a shuffle.
+// The weights are staged once per CTA in shared memory as ready-made B fragments in that same k order (one 16-byte
+// {hi0, hi1, lo0, lo1} load per thread, tile and k-step, conflict-free).
 //
-//   layer 1   D1[128x128] (TMEM)  =  X[128x16]  (smem, K-major)  x  W1k^T          (B = W1k [N][K] smem, K-major)
-//   epilogue  each of the 128 threads owns one TMEM lane = one sample row: tcgen05.ld the row, + vb[ray], ReLU,
-//             split, tcgen05.st back into TMEM as the A operand of layer 2 (activations never touch smem / HBM)
-//   layer 2   D2[128x128] (TMEM)  =  H1[128x128] (TMEM, "TS" form)  x  W2^T         (B = W2 [N][K] smem, K-major)
-//   epilogue  tcgen05.ld the row, + b2, ReLU, 3 dot products with W3 on the CUDA cores (N = 3 is too thin for an MMA),
-//             sigmoid, 12-byte coalesced store.
+// Precision: a single TF32 pass has ~1e-3 relative error, two orders of magnitude above the 1e-5 parity gate.  Every
+// operand is therefore split into hi = tf32(x) and lo = x - hi (exact in fp32) and each product is the 3-term sum
+// hi*hi + lo*hi + hi*lo accumulated in fp32 ("3xTF32", error ~2^-21).  single_pass (UBN_RGBNET_MODE=tc1) runs hi*hi only.
 //
-// Precision: a single TF32 (or BF16) pass has ~1e-3 relative error -- two orders of magnitude above the 1e-5 parity
-// gate.  Every operand is therefore split into hi = tf32(x) and lo = x - hi (exact in fp32) and each product is the
-// 3-term sum hi*hi + lo*hi + hi*lo accumulated in fp32 ("3xTF32", error ~2^-21), at 1/3 of the TF32 tensor rate -- still
-// ~5x the fp32 CUDA-core rate of the FFMA version.  UBN_RGBNET_TF32X1 (mode 1) runs the single-pass variant.
-//
-// Shared-memory operand layout: the canonical no-swizzle K-major UMMA layout: 8-row x 16-byte core matrices, rows of a
-// core matrix 16 B apart, next 8 rows at SBO = 128 B, next 16 bytes of K at LBO = 128 rows * 16 B = 2048 B; i.e. a
-// [K/4 panels][128 rows][4 floats] array.  Descriptor bit layout per cute/arch/mma_sm100_desc.hpp (studied, not copied).
+// Sample reductions of the backward (dW1k, dW3, db2, grad_view_bias) run on the tensor cores too: their contraction
+// index is the sample, which the accumulator layout spreads over g, so the warp turns the 16 x 128 operand through a
+// private shared-memory tile and reads it back as B fragments (sample = k).
 #include <algorithm>
 
 #include "common.cuh"
 
 namespace ubn {
-
 namespace tc {
 
-constexpr int kRows = 128;              // tile rows = TMEM lanes = threads
 constexpr int kHidden = 128;
 constexpr int kFeat = 12;
-constexpr int kK1 = 16;                 // layer-1 K padded to a multiple of 8
-constexpr uint32_t kPanelBytes = kRows * 16;   // one 16-byte K-slice of all 128 rows
-constexpr uint32_t kLBO = kPanelBytes;  // K-direction core-matrix stride
-constexpr uint32_t kSBO = 128;          // M/N-direction 8-row-group stride
+constexpr int kNT = kHidden / 8;        // 8-column tiles of a 128-wide layer
+constexpr int kUnit = 16;               // samples per warp unit (the M of one mma)
+constexpr int kPanelRows = 128;         // row block of the panel save layout
+constexpr int kStride = kHidden + 8;    // floats per row of a shared-memory operand tile (conflict-free both ways)
 
-// smem plan (bytes)
-constexpr uint32_t oW2hi = 0;
-constexpr uint32_t oW2lo = oW2hi + (kHidden / 4) * kPanelBytes;     // 64 KB each
-constexpr uint32_t oW1hi = oW2lo + (kHidden / 4) * kPanelBytes;
-constexpr uint32_t oW1lo = oW1hi + (kK1 / 4) * kPanelBytes;         // 8 KB each
-constexpr uint32_t oA1hi = oW1lo + (kK1 / 4) * kPanelBytes;
-constexpr uint32_t oA1lo = oA1hi + (kK1 / 4) * kPanelBytes;
-constexpr uint32_t oW3 = oA1lo + (kK1 / 4) * kPanelBytes;           // [3][128] fp32
-constexpr uint32_t oB2 = oW3 + 3 * kHidden * 4;
-constexpr uint32_t oBar = oB2 + kHidden * 4;                        // mbarrier (8 B) + tmem base (4 B)
-constexpr uint32_t oPart = oBar + 16;                               // [128][4] layer-3 partial sums (8-warp forward)
-constexpr uint32_t oStg = oPart + kRows * 16;                       // up to 8 warps x 4.5 KB store-transpose tiles
-constexpr uint32_t kSmemBytes = oStg + 8 * 32 * 36 * 4;
-
-// TMEM column plan (512 columns x 128 lanes x 32 bit)
-constexpr uint32_t cD1 = 0, cA2hi = 128, cA2lo = 256, cD2 = 384;
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
-  // start address [0,14), LBO [16,30), SBO [32,46) (all >> 4), descriptor version 1 at [46,48), no swizzle
-  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)(kLBO >> 4) << 16) | ((uint64_t)(kSBO >> 4) << 32) |
-         (1ull << 46);
-}
-
-// instruction descriptor: D = fp32 (c_format 1 @4), A = B = TF32 (format 2 @7, @10), K-major both, N>>3 @17, M>>4 @24
-constexpr uint32_t kIdesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(kHidden >> 3) << 17) | ((uint32_t)(kRows >> 4) << 24);
-
-// The MMA-issuing thread is picked with elect.sync inside a warp-uniform branch.  With `if (threadIdx.x == 0)` the compiler cannot
-// prove the instruction's uniform-register operands warp-uniform and wraps EVERY tcgen05.mma in an ELECT / BRA.U.ANY waterfall
-// loop (SASS); a phase trace of the backward kernel (scripts/trace_ws.cu) showed 143 cycles per 128x128x8 MMA issued that way
-// against the tensor pipe's 64-cycle floor, and 55 cycles per N = 16 MMA (floor 8).  With elect.sync the UTCHMMAs issue back to back.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred px;\n\telect.sync _|px, 0xffffffff;\n\tselp.u32 %0, 1, 0, px;\n\t}\n" : "=r"(pred));
-  return pred != 0;
-}
-
-// ask L2 for `bytes` (a multiple of 16, 16-byte aligned address) of global memory; no destination, no completion to wait for
-__device__ __forceinline__ void l2_prefetch(const void* gptr, uint32_t bytes) {
-  if (bytes) asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gptr), "r"(bytes) : "memory");
-}
-
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(kIdesc), "r"(accumulate)
-      : "memory");
-}
-
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(kIdesc), "r"(accumulate)
-      : "memory");
-}
-
-__device__ __forceinline__ void mma_commit(uint32_t bar_smem) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar_smem) : "memory");
-}
-
-__device__ __forceinline__ void mbar_init(uint32_t bar_smem, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar_smem), "r"(count) : "memory");
-}
-
-__device__ __forceinline__ void mbar_wait(uint32_t bar_smem, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t}\n" ::"r"(bar_smem),
-      "r"(parity)
-      : "memory");
-}
-
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// 32 lanes x 32 columns: thread t of the warp gets lane (warp base + t), 32 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+// B-fragment tables (uint4 per lane): [n-tile][k-step][32 lanes]
+constexpr uint32_t kFragW2 = kNT * kNT * 32 * 16;          // 128 KB
+constexpr uint32_t kFragW1 = kNT * 2 * 32 * 16;            // layer 1: K = 12 (2 k-steps), N = 128
+constexpr uint32_t kFragW1T = 2 * kNT * 32 * 16;           // dX: K = 128, N = 12 (2 n-tiles)
 
 __device__ __forceinline__ uint32_t tf32_hi_bits(float x) { return __float_as_uint(x) & 0xFFFFE000u; }
 
-// A thread owns one sample row, so a direct 128-bit store instruction would scatter 32 x 16 bytes over 32 rows (half-used
-// sectors, ncu: 23 % DRAM throughput while writing 4.3 GB).  Instead the warp transposes its 32 rows x 32 columns chunk
-// through a 4.5 KB staging tile so that every store instruction writes 4 rows x 128 contiguous bytes.
-constexpr int kStgStride = 36;                       // floats per staged row (16-byte aligned, conflict-free for 128-bit access)
-constexpr uint32_t kStgBytesPerWarp = 32 * kStgStride * 4;
-__device__ __forceinline__ void warp_store_chunk(float* stg, const float (&v)[32], float* __restrict__ gmem_row0, int col0,
-                                                 int64_t n_valid_rows, int lane) {
-#pragma unroll
-  for (int q = 0; q < 8; ++q)
-    *reinterpret_cast<float4*>(stg + lane * kStgStride + q * 4) = make_float4(v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]);
-  __syncwarp();
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int r = 4 * i + (lane >> 3);
-    const float4 t = *reinterpret_cast<const float4*>(stg + r * kStgStride + (lane & 7) * 4);
-    if (r < n_valid_rows) *reinterpret_cast<float4*>(gmem_row0 + (int64_t)r * kHidden + col0 + (lane & 7) * 4) = t;
-  }
-  __syncwarp();
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// write one weight matrix W[N=128][K] (row-major, K contiguous) into the hi / lo K-major panel arrays
-__device__ void stage_weights(const float* __restrict__ W, int K, int Kpad, uint8_t* hi, uint8_t* lo, int tid, int nthreads) {
-  for (int i = tid; i < kHidden * Kpad; i += nthreads) {
-    const int n = i / Kpad, k = i % Kpad;
-    const float w = (k < K) ? W[n * K + k] : 0.f;
-    const uint32_t hb = tf32_hi_bits(w);
-    const float l = w - __uint_as_float(hb);
-    const uint32_t off = (uint32_t)(k >> 2) * kPanelBytes + (uint32_t)n * 16 + (uint32_t)(k & 3) * 4;
-    *reinterpret_cast<uint32_t*>(hi + off) = hb;
-    *reinterpret_cast<float*>(lo + off) = l;
+__device__ __forceinline__ void split4(const float (&v)[4], uint32_t (&hi)[4], uint32_t (&lo)[4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    hi[i] = tf32_hi_bits(v[i]);
+    lo[i] = __float_as_uint(v[i] - __uint_as_float(hi[i]));
   }
 }
 
-// kHalves = 2: EIGHT warps per CTA.  Warps w and w + 4 address the same quarter of the TMEM lanes (a warp may touch lanes
-// 32 (w % 4) .. + 31), so they split every sample row of the tile by COLUMNS: half 0 owns hidden units 0..63, half 1 owns 64..127
-// in both epilogues; the three layer-3 dot products are combined through 1.5 KB of shared memory.  With four warps each scheduler
-// has a single warp and every TMEM / shared-memory latency of the epilogues is exposed; eight warps halve the epilogue time.
-// kPanel: the two [n,128] activation saves are written in the PANEL layout  [tile][32 column quads][128 rows][4]  (the K-major
-// panel order of the tensor-core operands) instead of row-major: the thread that owns a sample row stores its 16-byte quads
-// directly (a warp instruction covers 32 consecutive rows of one quad = 512 contiguous bytes), and the backward kernels' row-per-
-// thread loads are coalesced the same way.  Row-major saves cost the backward 32 x 32 L1 wavefronts per thread row (one 128-byte
-// line per lane and instruction: 8 k L1 cycles per 128-sample tile, phase trace in scripts/trace_ws.cu) and the forward a
-// shared-memory transpose per chunk.  The buffers must then hold ceil(n / 128) * 128 rows.
-template <bool kSave, bool kThreePass, int kHalves, bool kPanel>
-__global__ void __launch_bounds__(kRows * kHalves, 1) k_shade_fwd_tc(
+// d += a . b with (a, b) given as hi / lo halves; kThree adds the two cross terms
+template <bool kThree>
+__device__ __forceinline__ void mma3(float (&d)[4], const uint32_t (&ah)[4], const uint32_t (&al)[4], uint4 b) {
+  if (kThree) {
+    mma_tf32(d, al, b.x, b.y);
+    mma_tf32(d, ah, b.z, b.w);
+  }
+  mma_tf32(d, ah, b.x, b.y);
+}
+
+// Stage B[k][n] (k < K, n < N; zero outside) as B fragments for k-steps reading units 8 s + 2 t / 8 s + 2 t + 1:
+// lane (g, t) of (n-tile j, k-step s) gets {hi(B[8s+2t][8j+g]), hi(B[8s+2t+1][8j+g]), lo(..), lo(..)}.
+// B[k][n] = trans ? W[n * ld + k] : W[k * ld + n].
+__device__ void stage_frags(const float* __restrict__ W, int ld, bool trans, int K, int N, int n_ksteps, int n_ntiles,
+                            uint4* dst, int tid, int nthreads) {
+  for (int i = tid; i < n_ntiles * n_ksteps * 32; i += nthreads) {
+    const int lane = i & 31, s = (i >> 5) % n_ksteps, j = (i >> 5) / n_ksteps;
+    const int n = 8 * j + (lane >> 2), k0 = 8 * s + 2 * (lane & 3);
+    float w[2];
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int k = k0 + e;
+      w[e] = (k < K && n < N) ? (trans ? W[n * ld + k] : W[k * ld + n]) : 0.f;
+    }
+    const uint32_t h0 = tf32_hi_bits(w[0]), h1 = tf32_hi_bits(w[1]);
+    dst[i] = make_uint4(h0, h1, __float_as_uint(w[0] - __uint_as_float(h0)), __float_as_uint(w[1] - __uint_as_float(h1)));
+  }
+}
+
+// acc[NT] += X . B, X given in accumulator layout (x[s] = column tile s of the previous layer), B from stage_frags
+template <int KS, int NT, bool kThree>
+__device__ __forceinline__ void warp_gemm(float (&acc)[NT][4], const float (&x)[KS][4], const uint4* __restrict__ frag, int lane) {
+#pragma unroll
+  for (int s = 0; s < KS; ++s) {
+    const float av[4] = {x[s][0], x[s][2], x[s][1], x[s][3]};
+    uint32_t ah[4], al[4];
+    split4(av, ah, al);
+#pragma unroll
+    for (int j = 0; j < NT; ++j) mma3<kThree>(acc[j], ah, al, frag[(j * KS + s) * 32 + lane]);
+  }
+}
+
+// element offset of (row, col) in a save buffer: row-major [n][128], or the panel layout [n/128][32 quads][128 rows][4]
+template <bool kPanel>
+__device__ __forceinline__ int64_t save_idx(int64_t row, int col) {
+  if (kPanel) return (row >> 7) * (kPanelRows * kHidden) + (int64_t)(col >> 2) * (kPanelRows * 4) + (row & 127) * 4 + (col & 3);
+  return row * kHidden + col;
+}
+
+// ReLU mask words: [n/128][4 chunks of 32 units][128 rows], bit e = unit 32 c + e
+__device__ __forceinline__ int64_t mask_idx(int64_t row, int chunk) { return (row >> 7) * 512 + chunk * 128 + (row & 127); }
+
+// OR of this thread's bits of chunk c (units 8 j + 2 t, + 1 for j = 4 c .. 4 c + 3) over the four t lanes of a row
+__device__ __forceinline__ uint32_t mask_chunk(const float (&h)[kNT][4], int c, int e0, int t) {
+  uint32_t w = 0;
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj) {
+    const int j = 4 * c + jj;
+    w |= (h[j][e0] > 0.f ? 1u : 0u) << (8 * jj + 2 * t);
+    w |= (h[j][e0 + 1] > 0.f ? 1u : 0u) << (8 * jj + 2 * t + 1);
+  }
+  w |= __shfl_xor_sync(0xffffffffu, w, 1);
+  w |= __shfl_xor_sync(0xffffffffu, w, 2);
+  return w;
+}
+
+// ---- forward ---------------------------------------------------------------------------------------------------------
+constexpr uint32_t oFW2 = 0;
+constexpr uint32_t oFW1 = oFW2 + kFragW2;
+constexpr uint32_t oFW3 = oFW1 + kFragW1;                 // [3][128]
+constexpr uint32_t oFB2 = oFW3 + 3 * kHidden * 4;
+constexpr uint32_t kSmemFwd = oFB2 + kHidden * 4;
+
+template <bool kSave, bool kThree, int kWarps, bool kPanel>
+__global__ void __launch_bounds__(32 * kWarps, 1) k_shade_fwd_tc(
     const float* __restrict__ feat, const float* __restrict__ vb, const int64_t* __restrict__ ray_id,
     const float* __restrict__ W1k, const float* __restrict__ W2, const float* __restrict__ b2,
     const float* __restrict__ W3, const float* __restrict__ b3, int64_t n_pts, float* __restrict__ rgb,
     float* __restrict__ h1_out, float* __restrict__ h2_out, uint32_t* __restrict__ h1_mask) {
-  constexpr int kThreads = kRows * kHalves;
-  constexpr int kChunksPerHalf = (kHidden / 32) / kHalves;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int rtid = tid & (kRows - 1), half = tid >> 7;          // row within the tile, column half
-  float* sW3 = reinterpret_cast<float*>(smem + oW3);
-  float* sB2 = reinterpret_cast<float*>(smem + oB2);
-  float* sPart = reinterpret_cast<float*>(smem + oPart);        // [128][4] layer-3 partials of half 1
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + oBar);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + oBar + 8);
-  const uint32_t bar_addr = smem_u32(bar);
+  extern __shared__ __align__(16) uint8_t smem[];
+  const int tid = threadIdx.x, lane = tid & 31, g = lane >> 2, t = lane & 3;
+  const uint4* fW2 = reinterpret_cast<const uint4*>(smem + oFW2);
+  const uint4* fW1 = reinterpret_cast<const uint4*>(smem + oFW1);
+  float* sW3 = reinterpret_cast<float*>(smem + oFW3);
+  float* sB2 = reinterpret_cast<float*>(smem + oFB2);
+  stage_frags(W2, kHidden, true, kHidden, kHidden, kNT, kNT, reinterpret_cast<uint4*>(smem + oFW2), tid, 32 * kWarps);
+  stage_frags(W1k, kFeat, true, kFeat, kHidden, 2, kNT, reinterpret_cast<uint4*>(smem + oFW1), tid, 32 * kWarps);
+  for (int i = tid; i < 3 * kHidden; i += 32 * kWarps) sW3[i] = W3[i];
+  for (int i = tid; i < kHidden; i += 32 * kWarps) sB2[i] = b2[i];
+  __syncthreads();
+  const float b3v[3] = {b3[0], b3[1], b3[2]};
 
-  // ---- one-time setup: weights (split hi/lo, K-major panels), barrier, TMEM ----
-  stage_weights(W2, kHidden, kHidden, smem + oW2hi, smem + oW2lo, tid, kThreads);
-  stage_weights(W1k, kFeat, kK1, smem + oW1hi, smem + oW1lo, tid, kThreads);
+  const int64_t n_units = (n_pts + kUnit - 1) / kUnit;
+  for (int64_t u = (int64_t)blockIdx.x * kWarps + (tid >> 5); u < n_units; u += (int64_t)gridDim.x * kWarps) {
+    const int64_t row[2] = {u * kUnit + g, u * kUnit + g + 8};
+    const bool live[2] = {row[0] < n_pts, row[1] < n_pts};
+    // layer 1: X in accumulator layout, column tile s = features 8 s .. 8 s + 7 (12..15 are zero)
+    float x[2][4];
+#pragma unroll
+    for (int s = 0; s < 2; ++s)
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        float2 v = make_float2(0.f, 0.f);
+        if (live[r] && 8 * s + 2 * t < kFeat) v = *reinterpret_cast<const float2*>(feat + row[r] * kFeat + 8 * s + 2 * t);
+        x[s][2 * r] = v.x;
+        x[s][2 * r + 1] = v.y;
+      }
+    const int64_t ray[2] = {live[0] ? ray_id[row[0]] : 0, live[1] ? ray_id[row[1]] : 0};
+    float h[kNT][4];
+#pragma unroll
+    for (int j = 0; j < kNT; ++j) h[j][0] = h[j][1] = h[j][2] = h[j][3] = 0.f;
+    warp_gemm<2, kNT, kThree>(h, x, fW1, lane);
+    // epilogue 1: + vb[ray], ReLU
+#pragma unroll
+    for (int j = 0; j < kNT; ++j)
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const float2 bias = __ldg(reinterpret_cast<const float2*>(vb + ray[r] * kHidden + 8 * j + 2 * t));
+        h[j][2 * r] = fmaxf(h[j][2 * r] + bias.x, 0.f);
+        h[j][2 * r + 1] = fmaxf(h[j][2 * r + 1] + bias.y, 0.f);
+        if (kSave && live[r])
+          *reinterpret_cast<float2*>(h1_out + save_idx<kPanel>(row[r], 8 * j + 2 * t)) = make_float2(h[j][2 * r], h[j][2 * r + 1]);
+      }
+    if (kSave && kPanel && h1_mask) {
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const uint32_t w = mask_chunk(h, c, 2 * r, t);
+          if (t == 0 && live[r]) h1_mask[mask_idx(row[r], c)] = w;
+        }
+    }
+    // layer 2
+    float z[kNT][4];
+#pragma unroll
+    for (int j = 0; j < kNT; ++j) z[j][0] = z[j][1] = z[j][2] = z[j][3] = 0.f;
+    warp_gemm<kNT, kNT, kThree>(z, h, fW2, lane);
+    // epilogue 2: + b2, ReLU, layer 3 (N = 3: CUDA cores), sigmoid
+    float p[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+#pragma unroll
+    for (int j = 0; j < kNT; ++j) {
+      const int c = 8 * j + 2 * t;
+      const float2 bb = *reinterpret_cast<const float2*>(sB2 + c);
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const float a0 = fmaxf(z[j][2 * r] + bb.x, 0.f), a1 = fmaxf(z[j][2 * r + 1] + bb.y, 0.f);
+        if (kSave && live[r]) *reinterpret_cast<float2*>(h2_out + save_idx<kPanel>(row[r], c)) = make_float2(a0, a1);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) p[r][i] = fmaf(a1, sW3[i * kHidden + c + 1], fmaf(a0, sW3[i * kHidden + c], p[r][i]));
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r)
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+        p[r][i] += __shfl_xor_sync(0xffffffffu, p[r][i], 1);
+        p[r][i] += __shfl_xor_sync(0xffffffffu, p[r][i], 2);
+      }
+    if (t == 0) {
+#pragma unroll
+      for (int r = 0; r < 2; ++r)
+        if (live[r]) {
+          float* o = rgb + row[r] * 3;
+#pragma unroll
+          for (int i = 0; i < 3; ++i) o[i] = 1.f / (1.f + expf(-(p[r][i] + b3v[i])));
+        }
+    }
+  }
+}
+
+// ---- backward, launch 1 --------------------------------------------------------------------------------------------------
+//   dz3 = g_rgb * rgb (1 - rgb);  dZ2 = (dz3 . W3) * [H2 > 0];  dH1 = dZ2 . W2;  dZ1 = dH1 * [H1 > 0]
+//   kDz1Out: write dZ1 [n,128] row-major and stop (ubn_rgbnet_bwd_small finishes on the CUDA cores); otherwise also
+//   dX = dZ1 . W1k and every sample reduction except dW2:  dW1k^T = X^T . dZ1,  grad_view_bias[ray] += sum dZ1 of the
+//   ray (segment indicators as extra A rows),  dW3 = dz3^T . H2,  db2 = sum_i W3[i] * (dz3_i^T . [H2 > 0]),  db3 = sum dz3.
+namespace bk {
+constexpr uint32_t oW2 = 0;                                // dH1 = dZ2 . W2: B[k][n] = W2[k][n]
+constexpr uint32_t oW1T = oW2 + kFragW2;                   // dX = dZ1 . W1k: B[k][n] = W1k[k][n]
+constexpr uint32_t oW3 = oW1T + kFragW1T;
+constexpr uint32_t oAccW1 = oW3 + 3 * kHidden * 4;         // [12][128] dW1k^T partials
+constexpr uint32_t oAccW3 = oAccW1 + kFeat * kHidden * 4;  // [3][128]
+constexpr uint32_t oAccB2 = oAccW3 + 3 * kHidden * 4;      // [128]
+constexpr uint32_t oAccB3 = oAccB2 + kHidden * 4;          // [4]
+constexpr uint32_t oTile = oAccB3 + 16;                    // per warp [16][kStride]
+constexpr uint32_t kTileBytes = kUnit * kStride * 4;
+constexpr uint32_t smem_bytes(int warps) { return oTile + warps * kTileBytes; }
+}  // namespace bk
+
+// B fragment of the warp tile S[16][kStride] (sample = k): k-step s, column tile j -> S[8 s + t][8 j + g], S[8 s + t + 4][..]
+__device__ __forceinline__ void tile_frag(const float* S, int s, int j, int g, int t, uint32_t (&hi)[2], uint32_t (&lo)[2]) {
+  const float v[2] = {S[(8 * s + t) * kStride + 8 * j + g], S[(8 * s + t + 4) * kStride + 8 * j + g]};
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    hi[e] = tf32_hi_bits(v[e]);
+    lo[e] = __float_as_uint(v[e] - __uint_as_float(hi[e]));
+  }
+}
+
+// store a [16][128] accumulator-layout block into the warp tile
+__device__ __forceinline__ void tile_store(float* S, const float (&v)[kNT][4], int g, int t) {
+#pragma unroll
+  for (int j = 0; j < kNT; ++j) {
+    *reinterpret_cast<float2*>(S + g * kStride + 8 * j + 2 * t) = make_float2(v[j][0], v[j][1]);
+    *reinterpret_cast<float2*>(S + (g + 8) * kStride + 8 * j + 2 * t) = make_float2(v[j][2], v[j][3]);
+  }
+}
+
+template <bool kThree, int kWarps, bool kPanel, bool kMask1, bool kDz1Out>
+__global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc(
+    const float* __restrict__ feat, const int64_t* __restrict__ ray_id, const float* __restrict__ W1k,
+    const float* __restrict__ W2, const float* __restrict__ W3, const float* __restrict__ rgb,
+    const float* __restrict__ h1_save, const float* __restrict__ h2_save, const float* __restrict__ grad_rgb, int64_t n_pts,
+    float* __restrict__ grad_feat, float* __restrict__ grad_view_bias, float* __restrict__ grad_W1k, float* __restrict__ grad_b2,
+    float* __restrict__ grad_W3, float* __restrict__ grad_b3, uint32_t* __restrict__ h2_mask, const uint32_t* __restrict__ h1_mask,
+    float* __restrict__ dz1_out) {
+  extern __shared__ __align__(16) uint8_t smem[];
+  constexpr int kThreads = 32 * kWarps;
+  const int tid = threadIdx.x, lane = tid & 31, g = lane >> 2, t = lane & 3, warp = tid >> 5;
+  const uint4* fW2 = reinterpret_cast<const uint4*>(smem + bk::oW2);
+  const uint4* fW1T = reinterpret_cast<const uint4*>(smem + bk::oW1T);
+  float* sW3 = reinterpret_cast<float*>(smem + bk::oW3);
+  float* accW1 = reinterpret_cast<float*>(smem + bk::oAccW1);
+  float* accW3 = reinterpret_cast<float*>(smem + bk::oAccW3);
+  float* accB2 = reinterpret_cast<float*>(smem + bk::oAccB2);
+  float* accB3 = reinterpret_cast<float*>(smem + bk::oAccB3);
+  float* S = reinterpret_cast<float*>(smem + bk::oTile + warp * bk::kTileBytes);
+  stage_frags(W2, kHidden, false, kHidden, kHidden, kNT, kNT, reinterpret_cast<uint4*>(smem + bk::oW2), tid, kThreads);
+  if (!kDz1Out) stage_frags(W1k, kFeat, false, kHidden, kFeat, kNT, 2, reinterpret_cast<uint4*>(smem + bk::oW1T), tid, kThreads);
   for (int i = tid; i < 3 * kHidden; i += kThreads) sW3[i] = W3[i];
-  if (tid < kHidden) sB2[tid] = b2[tid];
-  if (tid == 0) {
-    mbar_init(bar_addr, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_slot)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  fence_async_smem();
-  tc_fence_before();
+  for (int i = tid; i < (kFeat + 3 + 1) * kHidden + 4; i += kThreads) accW1[i] = 0.f;   // accW1 .. accB3 are contiguous
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t lane_base = (uint32_t)((warp & 3) * 32) << 16;      // this warp's TMEM lane quarter
-  const float b3x = b3[0], b3y = b3[1], b3z = b3[2];
-  uint32_t phase = 0;
 
-  const uint64_t dW1hi = make_desc(smem_u32(smem + oW1hi)), dW1lo = make_desc(smem_u32(smem + oW1lo));
-  const uint64_t dA1hi = make_desc(smem_u32(smem + oA1hi)), dA1lo = make_desc(smem_u32(smem + oA1lo));
-  const uint64_t dW2hi = make_desc(smem_u32(smem + oW2hi)), dW2lo = make_desc(smem_u32(smem + oW2lo));
-  constexpr uint64_t kStep = (uint64_t)((2 * kPanelBytes) >> 4);   // one K=8 step = two 16-byte panels
-
-  const int64_t n_tiles = (n_pts + kRows - 1) / kRows;
-  // The X rows and ray ids of a tile are fetched ONE TILE AHEAD into registers (right after the previous tile's layer-1 MMA is
-  // issued), so the HBM latency of these loads is off the critical path of the serial  stage -> MMA -> epilogue  chain.
-  constexpr int kPanelsPerHalf = (kK1 / 4) / kHalves;
-  float4 xnext[kPanelsPerHalf];
-  int64_t ray_next = 0;
-  auto fetch_x = [&](int64_t t) {
-    const int64_t r = t * kRows + rtid;
-    const bool ok = t < n_tiles && r < n_pts;
+  const int64_t n_units = (n_pts + kUnit - 1) / kUnit;
+  for (int64_t u = (int64_t)blockIdx.x * kWarps + warp; u < n_units; u += (int64_t)gridDim.x * kWarps) {
+    const int64_t r0 = u * kUnit;
+    const int64_t row[2] = {r0 + g, r0 + g + 8};
+    const bool live[2] = {row[0] < n_pts, row[1] < n_pts};
+    float dz3[2][3];
 #pragma unroll
-    for (int pp = 0; pp < kPanelsPerHalf; ++pp) {
-      const int pnl = half * kPanelsPerHalf + pp;
-      xnext[pp] = make_float4(0, 0, 0, 0);
-      if (ok && pnl < 3) xnext[pp] = __ldg(reinterpret_cast<const float4*>(feat + r * kFeat + pnl * 4));
-    }
-    ray_next = ok ? ray_id[r] : 0;
-  };
-  fetch_x(blockIdx.x);
-  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    const int64_t row = tile * kRows + rtid;
-    const bool live = row < n_pts;
-    // ---- stage the X tile: row `rtid`, 12 features (+4 zero pad), split hi / lo; with two halves each stages two panels ----
+    for (int r = 0; r < 2; ++r)
 #pragma unroll
-    for (int pp = 0; pp < kPanelsPerHalf; ++pp) {
-      const int pnl = half * kPanelsPerHalf + pp;
-      const float4 v = xnext[pp];
-      uint4 hi;
-      float4 lo;
-      hi.x = tf32_hi_bits(v.x); hi.y = tf32_hi_bits(v.y); hi.z = tf32_hi_bits(v.z); hi.w = tf32_hi_bits(v.w);
-      lo.x = v.x - __uint_as_float(hi.x); lo.y = v.y - __uint_as_float(hi.y);
-      lo.z = v.z - __uint_as_float(hi.z); lo.w = v.w - __uint_as_float(hi.w);
-      *reinterpret_cast<uint4*>(smem + oA1hi + pnl * kPanelBytes + rtid * 16) = hi;
-      *reinterpret_cast<float4*>(smem + oA1lo + pnl * kPanelBytes + rtid * 16) = lo;
-    }
-    const int64_t my_ray = ray_next;
-    fence_async_smem();        // generic-proxy smem writes -> visible to the tensor core (async proxy)
-    tc_fence_before();
-    __syncthreads();
-    // ---- layer 1 MMA (one thread issues) ----
-    if (warp == 0 && elect_one()) {   // one elected lane of a CONVERGED warp: plain UTCHMMA issue (see elect_one)
-      tc_fence_after();
-#pragma unroll
-      for (int ks = 0; ks < kK1 / 8; ++ks) {
-        mma_ss(tmem + cD1, dA1hi + ks * kStep, dW1hi + ks * kStep, ks > 0);
-        if (kThreePass) {
-          mma_ss(tmem + cD1, dA1lo + ks * kStep, dW1hi + ks * kStep, 1);
-          mma_ss(tmem + cD1, dA1hi + ks * kStep, dW1lo + ks * kStep, 1);
-        }
+      for (int i = 0; i < 3; ++i) {
+        const float y = live[r] ? rgb[row[r] * 3 + i] : 0.f;
+        dz3[r][i] = live[r] ? grad_rgb[row[r] * 3 + i] * y * (1.f - y) : 0.f;
       }
-      mma_commit(bar_addr);
-    }
-    fetch_x(tile + gridDim.x);
-    mbar_wait(bar_addr, phase);
-    phase ^= 1;
-    tc_fence_after();
-    // ---- epilogue 1: + vb[ray], ReLU, split, back into TMEM as the layer-2 A operand (this half's columns) ----
-#pragma unroll 1
-    for (int cc = 0; cc < kChunksPerHalf; ++cc) {
-      const int c = half * kChunksPerHalf + cc;
-      float v[32];
-      tmem_ld32(tmem + lane_base + cD1 + c * 32, v);
-      uint32_t hi[32], lo[32];
-      const float4* vrow = reinterpret_cast<const float4*>(vb + my_ray * kHidden + c * 32);
+    // dZ2 in accumulator layout; H2 values kept for dW3 below (through the warp tile)
+    float d2[kNT][4];
+    uint32_t m2[2][4] = {{0u, 0u, 0u, 0u}, {0u, 0u, 0u, 0u}};
 #pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const float4 bias = __ldg(vrow + q);
-        float h0 = fmaxf(v[q * 4] + bias.x, 0.f), h1v = fmaxf(v[q * 4 + 1] + bias.y, 0.f);
-        float h2v = fmaxf(v[q * 4 + 2] + bias.z, 0.f), h3 = fmaxf(v[q * 4 + 3] + bias.w, 0.f);
-        v[q * 4] = h0; v[q * 4 + 1] = h1v; v[q * 4 + 2] = h2v; v[q * 4 + 3] = h3;
-        const float hs[4] = {h0, h1v, h2v, h3};
+    for (int j = 0; j < kNT; ++j) {
+      const int c = 8 * j + 2 * t;
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const uint32_t hb = tf32_hi_bits(hs[e]);
-          hi[q * 4 + e] = hb;
-          lo[q * 4 + e] = __float_as_uint(hs[e] - __uint_as_float(hb));
+      for (int r = 0; r < 2; ++r) {
+        const float2 hv = live[r] ? *reinterpret_cast<const float2*>(h2_save + save_idx<kPanel>(row[r], c)) : make_float2(0.f, 0.f);
+        const float hv2[2] = {hv.x, hv.y};
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float dh = dz3[r][0] * sW3[c + e] + dz3[r][1] * sW3[kHidden + c + e] + dz3[r][2] * sW3[2 * kHidden + c + e];
+          d2[j][2 * r + e] = hv2[e] > 0.f ? dh : 0.f;
+          if (hv2[e] > 0.f) m2[r][j >> 2] |= 1u << (8 * (j & 3) + 2 * t + e);
         }
+        if (!kDz1Out) *reinterpret_cast<float2*>(S + (g + 8 * r) * kStride + c) = hv;   // H2 tile for dW3 / db2
       }
-      tmem_st32(tmem + lane_base + cA2hi + c * 32, hi);
-      if (kThreePass) tmem_st32(tmem + lane_base + cA2lo + c * 32, lo);
-      // ---- layer 2 MMA, issued K-chunk by K-chunk: as soon as every warp has its 32-column piece of H1 in tensor memory, the
-      // K-steps that read those columns go to the tensor pipe and run while the next pieces are still being produced (the whole
-      // layer used to be issued after the last piece: 48 MMAs = ~3 k cycles of a ~12 k cycle tile with every warp waiting) ----
-      tmem_st_wait();
-      tc_fence_before();
-      __syncthreads();
-      if (warp == 0 && elect_one()) {   // one elected lane of a CONVERGED warp: plain UTCHMMA issue (see elect_one)
-        tc_fence_after();
+    }
+    if (h2_mask) {
 #pragma unroll
-        for (int hh = 0; hh < kHalves; ++hh) {
+      for (int r = 0; r < 2; ++r)
 #pragma unroll
-          for (int k4 = 0; k4 < 4; ++k4) {
-            const int ks = (hh * kChunksPerHalf + cc) * 4 + k4;
-            mma_ts(tmem + cD2, tmem + cA2hi + ks * 8, dW2hi + ks * kStep, (cc > 0 || hh > 0 || k4 > 0) ? 1u : 0u);
-            if (kThreePass) {
-              mma_ts(tmem + cD2, tmem + cA2lo + ks * 8, dW2hi + ks * kStep, 1);
-              mma_ts(tmem + cD2, tmem + cA2hi + ks * 8, dW2lo + ks * kStep, 1);
-            }
+        for (int c = 0; c < 4; ++c) {
+          uint32_t w = m2[r][c];
+          w |= __shfl_xor_sync(0xffffffffu, w, 1);
+          w |= __shfl_xor_sync(0xffffffffu, w, 2);
+          if (t == 0 && live[r]) h2_mask[mask_idx(row[r], c)] = w;
+        }
+    }
+    if (!kDz1Out) {
+      __syncwarp();
+      // dW3 = dz3^T . H2 and E = dz3^T . [H2 > 0] (db2 = sum_i W3[i] * E[i]): A rows 0..2 = dz3^T, sample = k
+      uint32_t ah[4], al[4];
+      {
+        // a0 = A[g][t], a1 = A[g + 8][t], a2 = A[g][t + 4], a3 = A[g + 8][t + 4]; A[i][k] = dz3 of sample k (rows >= 3: 0)
+        // dz3 of sample k lives in lane (g = k % 8, any t) as dz3[k / 8][.]
+        float av[2][4];
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+          float a[4];
+#pragma unroll
+          for (int q = 0; q < 2; ++q) {                      // k = t (q = 0) or t + 4 (q = 1), sample 8 s + k
+            const int src = 4 * (t + 4 * q);                 // lane holding sample row (t + 4 q) of this half
+            float v0 = __shfl_sync(0xffffffffu, dz3[s][0], src), v1 = __shfl_sync(0xffffffffu, dz3[s][1], src),
+                  v2 = __shfl_sync(0xffffffffu, dz3[s][2], src);
+            a[2 * q] = g == 0 ? v0 : g == 1 ? v1 : g == 2 ? v2 : 0.f;
+            a[2 * q + 1] = 0.f;                              // rows g + 8 >= 8: unused
+          }
+          av[s][0] = a[0]; av[s][1] = a[1]; av[s][2] = a[2]; av[s][3] = a[3];
+        }
+        float dW3a[kNT][4], Ea[kNT][4];
+#pragma unroll
+        for (int j = 0; j < kNT; ++j) dW3a[j][0] = dW3a[j][1] = dW3a[j][2] = dW3a[j][3] = Ea[j][0] = Ea[j][1] = Ea[j][2] = Ea[j][3] = 0.f;
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+          split4(av[s], ah, al);
+#pragma unroll
+          for (int j = 0; j < kNT; ++j) {
+            uint32_t bh[2], bl[2];
+            tile_frag(S, s, j, g, t, bh, bl);
+            mma3<kThree>(dW3a[j], ah, al, make_uint4(bh[0], bh[1], bl[0], bl[1]));
+            const uint32_t one = 0x3f800000u;
+            const uint32_t mb0 = __uint_as_float(bh[0]) + __uint_as_float(bl[0]) > 0.f ? one : 0u;
+            const uint32_t mb1 = __uint_as_float(bh[1]) + __uint_as_float(bl[1]) > 0.f ? one : 0u;
+            if (kThree) mma_tf32(Ea[j], al, mb0, mb1);
+            mma_tf32(Ea[j], ah, mb0, mb1);
           }
         }
-        if (cc == kChunksPerHalf - 1) mma_commit(bar_addr);
-      }
-      // the activation save goes out while the tensor pipe works on this piece
-      if (kSave) {
-        if (kPanel && h1_mask) {
-          // ReLU mask of this row's 32-unit piece for the backward's dZ1 = dH1 * [H1 > 0] (bit e = unit 32 c + e): the first
-          // backward launch then reads 16 bytes per sample instead of the 512-byte H1 row.  0 - h is negative exactly when
-          // h > 0 (h = max(x, 0) is +0 or positive), and a funnel shift appends its sign bit: two instructions per unit.
-          uint32_t w = 0;
+        if (g < 3) {
 #pragma unroll
-          for (int e = 31; e >= 0; --e) w = __funnelshift_l(__float_as_uint(__fsub_rn(0.f, v[e])), w, 1);
-          h1_mask[tile * 512 + c * 128 + rtid] = live ? w : 0u;
-          // With the masks the VALUES of H1 have one reader left, the dW2 launch, whose operand rows are (unit k, four consecutive
-          // samples).  So H1 is saved TRANSPOSED, [tile][32 sample quads][128 units][4 samples]: the warp turns its 32 x 32 piece
-          // through its 4.5 KB staging tile and every store instruction writes 512 contiguous bytes; the dW2 launch then fetches an
-          // operand row with ONE coalesced 16-byte load instead of four scattered 4-byte loads (which were half of the L1 wavefronts
-          // of that kernel: l1tex 89 % busy, ncu).
-          float* stg = reinterpret_cast<float*>(smem + oStg + warp * kStgBytesPerWarp);
-          const int ln = tid & 31;
+          for (int j = 0; j < kNT; ++j) {
+            const int c = 8 * j + 2 * t;
+            atomicAdd(accW3 + g * kHidden + c, dW3a[j][0]);
+            atomicAdd(accW3 + g * kHidden + c + 1, dW3a[j][1]);
+            atomicAdd(accB2 + c, sW3[g * kHidden + c] * Ea[j][0]);
+            atomicAdd(accB2 + c + 1, sW3[g * kHidden + c + 1] * Ea[j][1]);
+          }
+        }
 #pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<float4*>(stg + ln * kStgStride + q * 4) = make_float4(v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]);
-          __syncwarp();
-          float* dstT = h1_out + tile * (kRows * kHidden) + (int64_t)(8 * (warp & 3)) * (kHidden * 4) + (c * 32 + ln) * 4;
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<float4*>(dstT + q * (kHidden * 4)) =
-                make_float4(stg[(4 * q) * kStgStride + ln], stg[(4 * q + 1) * kStgStride + ln], stg[(4 * q + 2) * kStgStride + ln],
-                            stg[(4 * q + 3) * kStgStride + ln]);
-          __syncwarp();
-        } else if (kPanel) {
-          float4* dst = reinterpret_cast<float4*>(h1_out + tile * (kRows * kHidden) + (int64_t)(c * 8) * (kRows * 4) + rtid * 4);
-#pragma unroll
-          for (int q = 0; q < 8; ++q) dst[q * kRows] = make_float4(v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]);
-        } else {
-          warp_store_chunk(reinterpret_cast<float*>(smem + oStg + warp * kStgBytesPerWarp), v,
-                           h1_out + (tile * kRows + (warp & 3) * 32) * kHidden, c * 32, n_pts - (tile * kRows + (warp & 3) * 32), tid & 31);
+        for (int i = 0; i < 3; ++i) {                        // db3: the four t-lanes of a row hold the same dz3
+          float s3 = dz3[0][i] + dz3[1][i];
+          s3 += __shfl_xor_sync(0xffffffffu, s3, 4);
+          s3 += __shfl_xor_sync(0xffffffffu, s3, 8);
+          s3 += __shfl_xor_sync(0xffffffffu, s3, 16);
+          if (lane == i) atomicAdd(accB3 + i, s3);
         }
       }
+      __syncwarp();
     }
-    mbar_wait(bar_addr, phase);
-    phase ^= 1;
-    tc_fence_after();
-    // ---- epilogue 2: + b2, ReLU, layer 3 on CUDA cores (this half's columns), sigmoid ----
-    float p0 = 0.f, p1 = 0.f, p2 = 0.f;
-#pragma unroll 1
-    for (int cc = 0; cc < kChunksPerHalf; ++cc) {
-      const int c = half * kChunksPerHalf + cc;
-      float v[32];
-      tmem_ld32(tmem + lane_base + cD2 + c * 32, v);
+    // dH1 = dZ2 . W2
+    float d1[kNT][4];
 #pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const float4 bb = *reinterpret_cast<const float4*>(sB2 + c * 32 + q * 4);
-        const float4 wa = *reinterpret_cast<const float4*>(sW3 + c * 32 + q * 4);
-        const float4 wb = *reinterpret_cast<const float4*>(sW3 + kHidden + c * 32 + q * 4);
-        const float4 wc = *reinterpret_cast<const float4*>(sW3 + 2 * kHidden + c * 32 + q * 4);
-        const float h0 = fmaxf(v[q * 4] + bb.x, 0.f), h1v = fmaxf(v[q * 4 + 1] + bb.y, 0.f);
-        const float h2v = fmaxf(v[q * 4 + 2] + bb.z, 0.f), h3 = fmaxf(v[q * 4 + 3] + bb.w, 0.f);
-        v[q * 4] = h0; v[q * 4 + 1] = h1v; v[q * 4 + 2] = h2v; v[q * 4 + 3] = h3;
-        p0 = fmaf(h3, wa.w, fmaf(h2v, wa.z, fmaf(h1v, wa.y, fmaf(h0, wa.x, p0))));
-        p1 = fmaf(h3, wb.w, fmaf(h2v, wb.z, fmaf(h1v, wb.y, fmaf(h0, wb.x, p1))));
-        p2 = fmaf(h3, wc.w, fmaf(h2v, wc.z, fmaf(h1v, wc.y, fmaf(h0, wc.x, p2))));
-      }
-      if (kSave) {
-        if (kPanel) {
-          float4* dst = reinterpret_cast<float4*>(h2_out + tile * (kRows * kHidden) + (int64_t)(c * 8) * (kRows * 4) + rtid * 4);
+    for (int j = 0; j < kNT; ++j) d1[j][0] = d1[j][1] = d1[j][2] = d1[j][3] = 0.f;
+    warp_gemm<kNT, kNT, kThree>(d1, d2, fW2, lane);
+    // dZ1 = dH1 * [H1 > 0]
+    if (kMask1) {
 #pragma unroll
-          for (int q = 0; q < 8; ++q) dst[q * kRows] = make_float4(v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]);
-        } else {
-          warp_store_chunk(reinterpret_cast<float*>(smem + oStg + warp * kStgBytesPerWarp), v,
-                           h2_out + (tile * kRows + (warp & 3) * 32) * kHidden, c * 32, n_pts - (tile * kRows + (warp & 3) * 32), tid & 31);
+      for (int r = 0; r < 2; ++r) {
+        uint32_t w[4] = {0u, 0u, 0u, 0u};
+        if (live[r]) {
+#pragma unroll
+          for (int c = 0; c < 4; ++c) w[c] = h1_mask[mask_idx(row[r], c)];
         }
+#pragma unroll
+        for (int j = 0; j < kNT; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if (!((w[j >> 2] >> (8 * (j & 3) + 2 * t + e)) & 1u)) d1[j][2 * r + e] = 0.f;
       }
-    }
-    if (kHalves == 2) {
-      // the fp32 sum order of the 4-warp kernel is (columns 0..127 in one FMA chain); here it is chain(0..63) + chain(64..127):
-      // same terms, one extra rounding -- inside the 1e-5 parity tolerance like every other re-association of this dot product
-      if (half == 1) *reinterpret_cast<float4*>(sPart + rtid * 4) = make_float4(p0, p1, p2, 0.f);
-      tc_fence_before();
-      __syncthreads();
-      if (half == 0) {
-        const float4 o = *reinterpret_cast<const float4*>(sPart + rtid * 4);
-        p0 += o.x; p1 += o.y; p2 += o.z;
-      }
-    }
-    if (live && half == 0) {
-      float* o = rgb + row * 3;
-      o[0] = 1.f / (1.f + expf(-(p0 + b3x)));
-      o[1] = 1.f / (1.f + expf(-(p1 + b3y)));
-      o[2] = 1.f / (1.f + expf(-(p2 + b3z)));
-    }
-    // all TMEM reads of this tile are complete (wait::ld inside tmem_ld32) before the next tile's MMAs overwrite D1 / D2
-    tc_fence_before();
-    __syncthreads();
-  }
-
-  // ---- teardown ----
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem) : "memory");
-  }
-}
-
-
-// =====================================================================================================================
-// Backward on the tensor cores (data gradient + the big weight gradient):
-//   dZ2 = (dz3 . W3) * [H2 > 0]                         per row, CUDA cores (rank-3 update), split hi/lo -> TMEM
-//   dH1 = dZ2 . W2            (TS MMA: A = dZ2 in TMEM, B = W2^T staged once per CTA as K-major hi/lo panels)
-//   dZ1 = dH1 * [H1 > 0]      epilogue, streamed to HBM for the small-gradient kernel (k_shade_bwd_small, shade.cu)
-//   dW2 += dZ2^T . H1         contraction over SAMPLES: both operands must present the sample index as K.  Per tile, 4
-//                             rounds of 32 samples: dZ2 (A, M = hidden j) and H1 (B, N = hidden k), hi and lo, are
-//                             staged K-major (transposing 4-byte stores), then 4 K-steps x 3 split passes of
-//                             tcgen05.mma accumulate into a TMEM region that persists for the whole kernel.  (The
-//                             no-swizzle MN-major descriptor form, which would allow 16-byte staging stores, returned
-//                             all-zero accumulators for kind::tf32 on this part and toolchain -- probed on hardware.)
-// TMEM: [0,128) dZ2 hi, [128,256) dZ2 lo, [256,384) dH1, [384,512) dW2 accumulator.
-// =====================================================================================================================
-namespace bw {
-constexpr uint32_t kChunkK = 32;                              // samples per dW2 round
-constexpr uint32_t kChunkBytes = (kChunkK / 4) * kPanelBytes; // 8 K-major panels = 16 KB per staged operand
-constexpr uint32_t oWThi = 0;                                 // W2^T K-major panels (B of the dH1 MMA)
-constexpr uint32_t oWTlo = oWThi + (kHidden / 4) * kPanelBytes;
-constexpr uint32_t oCAhi = oWTlo + (kHidden / 4) * kPanelBytes;
-constexpr uint32_t oCAlo = oCAhi + kChunkBytes;
-constexpr uint32_t oCBhi = oCAlo + kChunkBytes;
-constexpr uint32_t oCBlo = oCBhi + kChunkBytes;
-constexpr uint32_t oW3b = oCBlo + kChunkBytes;                // [3][128] fp32
-constexpr uint32_t oBarB = oW3b + 3 * kHidden * 4;
-constexpr uint32_t kSmemBytesB = oBarB + 16;
-constexpr uint32_t cZhi = 0, cZlo = 128, cDH = 256, cDW = 384;
-
-}  // namespace bw
-
-template <bool kRounds>
-__global__ void __launch_bounds__(kRows, 1) k_shade_bwd_tc(
-    const float* __restrict__ W2, const float* __restrict__ W3, const float* __restrict__ rgb,
-    const float* __restrict__ h1, const float* __restrict__ h2, const float* __restrict__ g_rgb, int64_t n_pts,
-    float* __restrict__ dz1_out, float* __restrict__ gW2) {
-  using namespace bw;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  float* sW3 = reinterpret_cast<float*>(smem + oW3b);
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + oBarB);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + oBarB + 8);
-  const uint32_t bar_addr = smem_u32(bar);
-
-  // W2^T as the K-major B operand of dH1[s][k] = sum_j dZ2[s][j] W2[j][k]:  B[n = k][kk = j] = W2[j][k]
-  for (int i = tid; i < kHidden * kHidden; i += kRows) {
-    const int j = i / kHidden, k = i % kHidden;            // coalesced read of W2[j][k]
-    const float w = W2[i];
-    const uint32_t hb = tf32_hi_bits(w);
-    const uint32_t off = (uint32_t)(j >> 2) * kPanelBytes + (uint32_t)k * 16 + (uint32_t)(j & 3) * 4;
-    *reinterpret_cast<uint32_t*>(smem + oWThi + off) = hb;
-    *reinterpret_cast<float*>(smem + oWTlo + off) = w - __uint_as_float(hb);
-  }
-  for (int i = tid; i < 3 * kHidden; i += kRows) sW3[i] = W3[i];
-  if (tid == 0) {
-    mbar_init(bar_addr, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_slot)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  fence_async_smem();
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-  uint32_t phase = 0;
-  const uint64_t dWThi = make_desc(smem_u32(smem + oWThi)), dWTlo = make_desc(smem_u32(smem + oWTlo));
-  const uint64_t dCAhi = make_desc(smem_u32(smem + oCAhi)), dCAlo = make_desc(smem_u32(smem + oCAlo));
-  const uint64_t dCBhi = make_desc(smem_u32(smem + oCBhi)), dCBlo = make_desc(smem_u32(smem + oCBlo));
-  constexpr uint64_t kStepK = (uint64_t)((2 * kPanelBytes) >> 4);   // K-major operand: 8 K-elements = 2 panels
-  bool dw_started = false;
-
-  const int64_t n_tiles = (n_pts + kRows - 1) / kRows;
-  const int64_t per_cta = (n_tiles + gridDim.x - 1) / gridDim.x;
-  const int64_t tile_end = min(n_tiles, (int64_t)(blockIdx.x + 1) * per_cta);
-  for (int64_t tile = (int64_t)blockIdx.x * per_cta; tile < tile_end; ++tile) {
-    const int64_t row = tile * kRows + tid;
-    const bool live = row < n_pts;
-    float d0 = 0.f, d1 = 0.f, d2 = 0.f;
-    if (live) {
-      const float* o = rgb + row * 3;
-      const float* g = g_rgb + row * 3;
-      d0 = g[0] * (o[0] * (1.f - o[0]));
-      d1 = g[1] * (o[1] * (1.f - o[1]));
-      d2 = g[2] * (o[2] * (1.f - o[2]));
-    }
-    // ---- dZ2 row -> TMEM (A operand of the dH1 MMA).  The kernel is load-latency bound with 4 warps per SM, so the whole
-    //      512-byte H2 row is requested up front (32 independent 128-bit loads in flight per thread) ----
-    float4 hrow[kHidden / 4];
+    } else {
 #pragma unroll
-    for (int q = 0; q < kHidden / 4; ++q) {
-      hrow[q] = make_float4(0, 0, 0, 0);
-      if (live) hrow[q] = __ldg(reinterpret_cast<const float4*>(h2 + row * kHidden + q * 4));
-    }
+      for (int j = 0; j < kNT; ++j)
 #pragma unroll
-    for (int c = 0; c < kHidden / 32; ++c) {
-      uint32_t hi[32], lo[32];
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const float4 hv = hrow[c * 8 + q];
-        const float4 wa = *reinterpret_cast<const float4*>(sW3 + c * 32 + q * 4);
-        const float4 wb = *reinterpret_cast<const float4*>(sW3 + kHidden + c * 32 + q * 4);
-        const float4 wc = *reinterpret_cast<const float4*>(sW3 + 2 * kHidden + c * 32 + q * 4);
-        const float z[4] = {hv.x > 0.f ? fmaf(d2, wc.x, fmaf(d1, wb.x, d0 * wa.x)) : 0.f,
-                            hv.y > 0.f ? fmaf(d2, wc.y, fmaf(d1, wb.y, d0 * wa.y)) : 0.f,
-                            hv.z > 0.f ? fmaf(d2, wc.z, fmaf(d1, wb.z, d0 * wa.z)) : 0.f,
-                            hv.w > 0.f ? fmaf(d2, wc.w, fmaf(d1, wb.w, d0 * wa.w)) : 0.f};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const uint32_t hb = tf32_hi_bits(z[e]);
-          hi[q * 4 + e] = hb;
-          lo[q * 4 + e] = __float_as_uint(z[e] - __uint_as_float(hb));
+        for (int r = 0; r < 2; ++r) {
+          const float2 hv = live[r] ? *reinterpret_cast<const float2*>(h1_save + save_idx<kPanel>(row[r], 8 * j + 2 * t))
+                                    : make_float2(0.f, 0.f);
+          if (!(hv.x > 0.f)) d1[j][2 * r] = 0.f;
+          if (!(hv.y > 0.f)) d1[j][2 * r + 1] = 0.f;
         }
-      }
-      tmem_st32(tmem + lane_base + cZhi + c * 32, hi);
-      tmem_st32(tmem + lane_base + cZlo + c * 32, lo);
     }
-    tmem_st_wait();
-    tc_fence_before();
-    __syncthreads();
-    // ---- dH1 = dZ2 . W2 ----
-    if (warp == 0 && elect_one()) {   // one elected lane of a CONVERGED warp: plain UTCHMMA issue (see elect_one)
-      tc_fence_after();
-#pragma unroll 4
-      for (int ks = 0; ks < kHidden / 8; ++ks) {
-        mma_ts(tmem + cDH, tmem + cZhi + ks * 8, dWThi + ks * kStepK, ks > 0);
-        mma_ts(tmem + cDH, tmem + cZlo + ks * 8, dWThi + ks * kStepK, 1);
-        mma_ts(tmem + cDH, tmem + cZhi + ks * 8, dWTlo + ks * kStepK, 1);
-      }
-      mma_commit(bar_addr);
+    if (kDz1Out) {
+#pragma unroll
+      for (int j = 0; j < kNT; ++j)
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+          if (live[r]) *reinterpret_cast<float2*>(dz1_out + row[r] * kHidden + 8 * j + 2 * t) = make_float2(d1[j][2 * r], d1[j][2 * r + 1]);
+      continue;
     }
-    // the H1 row is requested while the tensor pipe works (the H2 registers are dead by now)
-#pragma unroll
-    for (int q = 0; q < kHidden / 4; ++q) {
-      hrow[q] = make_float4(0, 0, 0, 0);
-      if (live) hrow[q] = __ldg(reinterpret_cast<const float4*>(h1 + row * kHidden + q * 4));
-    }
-    mbar_wait(bar_addr, phase);
-    phase ^= 1;
-    tc_fence_after();
-    // ---- dZ1 = dH1 * [H1 > 0] -> HBM ----
-#pragma unroll
-    for (int c = 0; c < kHidden / 32; ++c) {
-      float v[32];
-      tmem_ld32(tmem + lane_base + cDH + c * 32, v);
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const float4 hv = hrow[c * 8 + q];
-        v[q * 4] = hv.x > 0.f ? v[q * 4] : 0.f; v[q * 4 + 1] = hv.y > 0.f ? v[q * 4 + 1] : 0.f;
-        v[q * 4 + 2] = hv.z > 0.f ? v[q * 4 + 2] : 0.f; v[q * 4 + 3] = hv.w > 0.f ? v[q * 4 + 3] : 0.f;
-      }
-      warp_store_chunk(reinterpret_cast<float*>(smem + oCAhi + warp * kStgBytesPerWarp), v,
-                       dz1_out + (tile * kRows + warp * 32) * kHidden, c * 32, n_pts - (tile * kRows + warp * 32), lane);
-    }
-    // ---- dW2 += dZ2^T . H1 : 4 rounds of 32 samples (K = sample index) ----
-    // Both operands are staged K-major: A[m = hidden j][k = sample], B[n = hidden k][k = sample]; element (row, s) lives at
-    // panel s/4, row*16 + (s%4)*4.  In round r the 8 rows 8r..8r+7 of every warp are staged by ALL 32 lanes of that
-    // warp: lane l serves row 8r + (l & 7) and the hidden units j = 4*jj + (l >> 3) (jj < 32) -- this assignment spreads the
-    // 4-byte stores over 16 banks x 2 panels (2-way conflict) instead of 8 lanes hammering 4 banks.
-#pragma unroll 1
-    for (int r = 0; kRounds && r < 4; ++r) {
-      const int src = 8 * r + (lane & 7);
-      const float e0 = __shfl_sync(0xffffffffu, d0, src), e1 = __shfl_sync(0xffffffffu, d1, src), e2 = __shfl_sync(0xffffffffu, d2, src);
-      const int64_t row_s = tile * kRows + warp * 32 + src;
-      const bool live_s = row_s < n_pts;
-      const uint32_t s_local = (uint32_t)warp * 8 + (uint32_t)(lane & 7);
-      const uint32_t soff = (s_local >> 2) * kPanelBytes + (s_local & 3) * 4;
-      const int q = lane >> 3;
-#pragma unroll 8
-      for (int jj = 0; jj < kHidden / 4; ++jj) {
-        const int j = jj * 4 + q;
-        float hv2 = 0.f, hv1 = 0.f;
-        if (live_s) {
-          hv2 = __ldg(h2 + row_s * kHidden + j);
-          hv1 = __ldg(h1 + row_s * kHidden + j);
-        }
-        const float z = hv2 > 0.f ? fmaf(e2, sW3[2 * kHidden + j], fmaf(e1, sW3[kHidden + j], e0 * sW3[j])) : 0.f;
-        const uint32_t zh = tf32_hi_bits(z), hh = tf32_hi_bits(hv1);
-        const uint32_t off = soff + (uint32_t)j * 16;
-        *reinterpret_cast<uint32_t*>(smem + oCAhi + off) = zh;
-        *reinterpret_cast<float*>(smem + oCAlo + off) = z - __uint_as_float(zh);
-        *reinterpret_cast<uint32_t*>(smem + oCBhi + off) = hh;
-        *reinterpret_cast<float*>(smem + oCBlo + off) = hv1 - __uint_as_float(hh);
-      }
-      fence_async_smem();
-      tc_fence_before();
-      __syncthreads();
-      if (warp == 0 && elect_one()) {   // one elected lane of a CONVERGED warp: plain UTCHMMA issue (see elect_one)
-        tc_fence_after();
-#pragma unroll
-        for (int ks = 0; ks < (int)(kChunkK / 8); ++ks) {
-          mma_ss(tmem + cDW, dCAhi + ks * kStepK, dCBhi + ks * kStepK, (dw_started || ks > 0) ? 1u : 0u);
-          mma_ss(tmem + cDW, dCAlo + ks * kStepK, dCBhi + ks * kStepK, 1);
-          mma_ss(tmem + cDW, dCAhi + ks * kStepK, dCBlo + ks * kStepK, 1);
-        }
-        mma_commit(bar_addr);
-      }
-      dw_started = true;
-      mbar_wait(bar_addr, phase);     // the chunk buffers are rewritten by the next round
-      phase ^= 1;
-      tc_fence_after();
-    }
-    tc_fence_before();
-    __syncthreads();
-  }
-
-  // ---- flush dW2: thread j owns row j of the accumulator ----
-  if (dw_started) {
-#pragma unroll 1
-    for (int c = 0; c < kHidden / 32; ++c) {
-      float v[32];
-      tmem_ld32(tmem + lane_base + cDW + c * 32, v);
-#pragma unroll
-      for (int e = 0; e < 32; ++e) atomicAdd(gW2 + tid * kHidden + c * 32 + e, v[e]);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem) : "memory");
-  }
-}
-
-
-// =====================================================================================================================
-// Fused data-path backward: everything except dW2 in ONE kernel, nothing but dX written back.
-//   dZ2 = (dz3 . W3) * [H2 > 0]        row-owner threads, CUDA cores  -> TMEM (hi / lo), A operand of
-//   dH1 = dZ2 . W2                     TS MMA, B = W2^T K-major panels (as k_shade_bwd_tc)
-//   dZ1 = dH1 * [H1 > 0]               epilogue -> TMEM (hi / lo) again, A operand of
-//   dX  = dZ1 . W1k                    TS MMA with N = 16 (12 used), B = W1k^T K-major panels  -> g_feat
-// and every reduction over SAMPLES that k_shade_bwd_small did in a second pass over dZ1 / H2 (4.2 + 2.1 GB of re-reads, 2.1 GB
-// of dZ1 writes): each warp transposes its 32-row x 32-column chunk through a 4.5 KB staging tile, after which LANE = COLUMN
-// (hidden unit) and the sample sums are plain per-lane loops:
-//   db2[j]  += sum_s dZ2[s][j]               dW3[c][j] += sum_s dz3[s][c] H2[s][j]         (from the staged H2 chunk)
-//   dvb[ray][j] += sum_{s in ray} dZ1[s][j]  dW1k[j][c] += sum_s dZ1[s][j] X[s][c]         (from the staged dZ1 chunk)
-// CTA-level partials live in shared memory and are flushed once.  dZ1 never reaches HBM.
-// TMEM: [0,128) A hi, [128,256) A lo (dZ2, then dZ1), [256,384) dH1, [384,400) dX.
-// =====================================================================================================================
-namespace bf {
-constexpr uint32_t kPanelN16 = 16 * 16;                         // one 16-byte K-slice of the 16 rows of W1k^T
-constexpr uint32_t oVThi = 0;
-constexpr uint32_t oVTlo = oVThi + (kHidden / 4) * kPanelBytes;
-constexpr uint32_t oV1hi = oVTlo + (kHidden / 4) * kPanelBytes;
-constexpr uint32_t oV1lo = oV1hi + (kHidden / 4) * kPanelN16;
-constexpr uint32_t oStgF = oV1lo + (kHidden / 4) * kPanelN16;   // 4 warps x 32 x 36 floats
-constexpr uint32_t oXf = oStgF + 4 * kStgBytesPerWarp;          // [128][12] fp32
-constexpr uint32_t oDz3 = oXf + kRows * kFeat * 4;              // [128][4]
-constexpr uint32_t oRayF = oDz3 + kRows * 16;                   // int[128]
-constexpr uint32_t oW3f = oRayF + kRows * 4;                    // [3][128]
-constexpr uint32_t oAccW1 = oW3f + 3 * kHidden * 4;             // [128][12]
-constexpr uint32_t oAccW3 = oAccW1 + kHidden * kFeat * 4;       // [3][128]
-constexpr uint32_t oAccB2 = oAccW3 + 3 * kHidden * 4;           // [128]
-constexpr uint32_t oAccB3 = oAccB2 + kHidden * 4;               // [4]
-constexpr uint32_t oBarF = oAccB3 + 16;
-constexpr uint32_t kSmemBytesF = oBarF + 16;
-constexpr uint32_t cAhi = 0, cAlo = 128, cDHf = 256, cDX = 384;
-constexpr uint32_t kIdescN16 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(16 >> 3) << 17) | ((uint32_t)(kRows >> 4) << 24);
-}  // namespace bf
-
-__device__ __forceinline__ uint64_t make_desc_lbo(uint32_t smem_addr, uint32_t lbo) {
-  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(kSBO >> 4) << 32) | (1ull << 46);
-}
-
-__device__ __forceinline__ void mma_ts_idesc(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// 32 lanes x 16 columns
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-      "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-      "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-      "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15]))
-      : "memory");
-}
-
-// stage this warp's 32 x 32 chunk (thread = row) so that afterwards lane = column: stg[row * 36 + col]
-__device__ __forceinline__ void warp_stage_chunk(float* stg, const float4 (&q)[8], int lane) {
-#pragma unroll
-  for (int i = 0; i < 8; ++i) *reinterpret_cast<float4*>(stg + lane * kStgStride + i * 4) = q[i];
-  __syncwarp();
-}
-
-template <bool kThree>
-__global__ void __launch_bounds__(kRows, 1) k_shade_bwd_fused(
-    const float* __restrict__ feat, const int64_t* __restrict__ ray_id, const float* __restrict__ W1k,
-    const float* __restrict__ W2, const float* __restrict__ W3, const float* __restrict__ rgb,
-    const float* __restrict__ h1, const float* __restrict__ h2, const float* __restrict__ g_rgb, int64_t n_pts,
-    float* __restrict__ g_feat, float* __restrict__ g_vb, float* __restrict__ gW1k, float* __restrict__ gb2,
-    float* __restrict__ gW3, float* __restrict__ gb3) {
-  using namespace bf;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  float* sW3 = reinterpret_cast<float*>(smem + oW3f);
-  float* sX = reinterpret_cast<float*>(smem + oXf);
-  float4* sDz3 = reinterpret_cast<float4*>(smem + oDz3);
-  int* sRay = reinterpret_cast<int*>(smem + oRayF);
-  float* sAccW1 = reinterpret_cast<float*>(smem + oAccW1);
-  float* sAccW3 = reinterpret_cast<float*>(smem + oAccW3);
-  float* sAccB2 = reinterpret_cast<float*>(smem + oAccB2);
-  float* sAccB3 = reinterpret_cast<float*>(smem + oAccB3);
-  float* stg = reinterpret_cast<float*>(smem + oStgF + warp * kStgBytesPerWarp);
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + oBarF);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + oBarF + 8);
-  const uint32_t bar_addr = smem_u32(bar);
-
-  // W2^T as the K-major B operand of dH1[s][k] = sum_j dZ2[s][j] W2[j][k]:  B[n = k][kk = j] = W2[j][k]
-  for (int i = tid; i < kHidden * kHidden; i += kRows) {
-    const int j = i / kHidden, k = i % kHidden;
-    const float w = W2[i];
-    const uint32_t hb = tf32_hi_bits(w);
-    const uint32_t off = (uint32_t)(j >> 2) * kPanelBytes + (uint32_t)k * 16 + (uint32_t)(j & 3) * 4;
-    *reinterpret_cast<uint32_t*>(smem + oVThi + off) = hb;
-    *reinterpret_cast<float*>(smem + oVTlo + off) = w - __uint_as_float(hb);
-  }
-  // W1k^T as the K-major B operand of dX[s][c] = sum_j dZ1[s][j] W1k[j][c]:  B[n = c][kk = j] = W1k[j][c], rows 12..15 zero
-  for (int i = tid; i < kHidden * 16; i += kRows) {
-    const int j = i >> 4, c = i & 15;
-    const float w = (c < kFeat) ? W1k[j * kFeat + c] : 0.f;
-    const uint32_t hb = tf32_hi_bits(w);
-    const uint32_t off = (uint32_t)(j >> 2) * kPanelN16 + (uint32_t)c * 16 + (uint32_t)(j & 3) * 4;
-    *reinterpret_cast<uint32_t*>(smem + oV1hi + off) = hb;
-    *reinterpret_cast<float*>(smem + oV1lo + off) = w - __uint_as_float(hb);
-  }
-  for (int i = tid; i < 3 * kHidden; i += kRows) { sW3[i] = W3[i]; sAccW3[i] = 0.f; }
-  for (int i = tid; i < kHidden * kFeat; i += kRows) sAccW1[i] = 0.f;
-  sAccB2[tid] = 0.f;
-  if (tid < 4) sAccB3[tid] = 0.f;
-  if (tid == 0) {
-    mbar_init(bar_addr, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_slot)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  fence_async_smem();
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-  uint32_t phase = 0;
-  const uint64_t dWThi = make_desc(smem_u32(smem + oVThi)), dWTlo = make_desc(smem_u32(smem + oVTlo));
-  const uint64_t dW1hi = make_desc_lbo(smem_u32(smem + oV1hi), kPanelN16), dW1lo = make_desc_lbo(smem_u32(smem + oV1lo), kPanelN16);
-  constexpr uint64_t kStepK = (uint64_t)((2 * kPanelBytes) >> 4);
-  constexpr uint64_t kStepK16 = (uint64_t)((2 * kPanelN16) >> 4);
-  float b3a = 0.f, b3b = 0.f, b3c = 0.f;      // db3 partial of this thread's rows
-
-  const int64_t n_tiles = (n_pts + kRows - 1) / kRows;
-  const int64_t per_cta = (n_tiles + gridDim.x - 1) / gridDim.x;
-  const int64_t tile_end = min(n_tiles, (int64_t)(blockIdx.x + 1) * per_cta);
-  for (int64_t tile = (int64_t)blockIdx.x * per_cta; tile < tile_end; ++tile) {
-    const int64_t row = tile * kRows + tid;
-    const bool live = row < n_pts;
-    float d0 = 0.f, d1 = 0.f, d2 = 0.f;
-    int my_ray = -1;
+    // dX = dZ1 . W1k
     {
-      float4 x0 = make_float4(0, 0, 0, 0), x1 = x0, x2 = x0;
-      if (live) {
-        const float* o = rgb + row * 3;
-        const float* g = g_rgb + row * 3;
-        d0 = g[0] * (o[0] * (1.f - o[0]));
-        d1 = g[1] * (o[1] * (1.f - o[1]));
-        d2 = g[2] * (o[2] * (1.f - o[2]));
-        my_ray = (int)ray_id[row];
-        const float4* xr = reinterpret_cast<const float4*>(feat + row * kFeat);
-        x0 = __ldg(xr); x1 = __ldg(xr + 1); x2 = __ldg(xr + 2);
-      }
-      sDz3[tid] = make_float4(d0, d1, d2, 0.f);
-      sRay[tid] = my_ray;
-      float4* xs = reinterpret_cast<float4*>(sX + tid * kFeat);
-      xs[0] = x0; xs[1] = x1; xs[2] = x2;
-      b3a += d0; b3b += d1; b3c += d2;
+      float dx[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+      warp_gemm<kNT, 2, kThree>(dx, d1, fW1T, lane);
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+          if (live[r] && 8 * j + 2 * t < kFeat)
+            *reinterpret_cast<float2*>(grad_feat + row[r] * kFeat + 8 * j + 2 * t) = make_float2(dx[j][2 * r], dx[j][2 * r + 1]);
     }
-    // ---- H2 row: dZ2 -> TMEM, and (staged, lane = column) db2 / dW3 ----
-    float4 hrow[kHidden / 4];
-#pragma unroll
-    for (int q = 0; q < kHidden / 4; ++q) {
-      hrow[q] = make_float4(0, 0, 0, 0);
-      if (live) hrow[q] = __ldg(reinterpret_cast<const float4*>(h2 + row * kHidden + q * 4));
-    }
-    __syncwarp();      // sDz3 / sRay / sX rows of this warp are complete (each warp only reads its own 32 rows)
-#pragma unroll
-    for (int c = 0; c < kHidden / 32; ++c) {
-      uint32_t hi[32], lo[32];
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const float4 hv = hrow[c * 8 + q];
-        const float4 wa = *reinterpret_cast<const float4*>(sW3 + c * 32 + q * 4);
-        const float4 wb = *reinterpret_cast<const float4*>(sW3 + kHidden + c * 32 + q * 4);
-        const float4 wc = *reinterpret_cast<const float4*>(sW3 + 2 * kHidden + c * 32 + q * 4);
-        const float z[4] = {hv.x > 0.f ? fmaf(d2, wc.x, fmaf(d1, wb.x, d0 * wa.x)) : 0.f,
-                            hv.y > 0.f ? fmaf(d2, wc.y, fmaf(d1, wb.y, d0 * wa.y)) : 0.f,
-                            hv.z > 0.f ? fmaf(d2, wc.z, fmaf(d1, wb.z, d0 * wa.z)) : 0.f,
-                            hv.w > 0.f ? fmaf(d2, wc.w, fmaf(d1, wb.w, d0 * wa.w)) : 0.f};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const uint32_t hb = tf32_hi_bits(z[e]);
-          hi[q * 4 + e] = hb;
-          lo[q * 4 + e] = __float_as_uint(z[e] - __uint_as_float(hb));
-        }
-      }
-      tmem_st32(tmem + lane_base + cAhi + c * 32, hi);
-      tmem_st32(tmem + lane_base + cAlo + c * 32, lo);
-      // lane = hidden unit j of this chunk: sums over the warp's 32 samples
-      {
-        float4 q8[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) q8[q] = hrow[c * 8 + q];
-        warp_stage_chunk(stg, q8, lane);
-        const int j = c * 32 + lane;
-        const float w3a = sW3[j], w3b = sW3[kHidden + j], w3c = sW3[2 * kHidden + j];
-        float a0 = 0.f, a1 = 0.f, a2 = 0.f, ab = 0.f;
-#pragma unroll 8
-        for (int sidx = 0; sidx < 32; ++sidx) {
-          const float h = stg[sidx * kStgStride + lane];
-          const float4 dz = sDz3[warp * 32 + sidx];
-          a0 = fmaf(dz.x, h, a0); a1 = fmaf(dz.y, h, a1); a2 = fmaf(dz.z, h, a2);
-          ab += h > 0.f ? fmaf(dz.z, w3c, fmaf(dz.y, w3b, dz.x * w3a)) : 0.f;
-        }
-        atomicAdd(sAccW3 + j, a0); atomicAdd(sAccW3 + kHidden + j, a1); atomicAdd(sAccW3 + 2 * kHidden + j, a2);
-        atomicAdd(sAccB2 + j, ab);
-        __syncwarp();
-      }
-    }
-    tmem_st_wait();
-    tc_fence_before();
-    __syncthreads();
-    // ---- dH1 = dZ2 . W2 ----
-    if (warp == 0 && elect_one()) {   // one elected lane of a CONVERGED warp: plain UTCHMMA issue (see elect_one)
-      tc_fence_after();
-#pragma unroll 4
-      for (int ks = 0; ks < kHidden / 8; ++ks) {
-        mma_ts(tmem + cDHf, tmem + cAhi + ks * 8, dWThi + ks * kStepK, ks > 0);
-        if (kThree) {
-          mma_ts(tmem + cDHf, tmem + cAlo + ks * 8, dWThi + ks * kStepK, 1);
-          mma_ts(tmem + cDHf, tmem + cAhi + ks * 8, dWTlo + ks * kStepK, 1);
-        }
-      }
-      mma_commit(bar_addr);
-    }
-#pragma unroll
-    for (int q = 0; q < kHidden / 4; ++q) {
-      hrow[q] = make_float4(0, 0, 0, 0);
-      if (live) hrow[q] = __ldg(reinterpret_cast<const float4*>(h1 + row * kHidden + q * 4));
-    }
-    // is the whole warp inside one ray?  (the common case: 128-sample tiles, hundreds of samples per ray)
-    const int ray0 = __shfl_sync(0xffffffffu, my_ray, 0);
-    const bool one_ray = __all_sync(0xffffffffu, my_ray == ray0) && ray0 >= 0;
-    mbar_wait(bar_addr, phase);
-    phase ^= 1;
-    tc_fence_after();
-    // ---- dZ1 = dH1 * [H1 > 0]: -> TMEM (A of the dX MMA); staged: dvb, dW1k ----
-#pragma unroll
-    for (int c = 0; c < kHidden / 32; ++c) {
-      float v[32];
-      tmem_ld32(tmem + lane_base + cDHf + c * 32, v);
-      uint32_t hi[32], lo[32];
-      float4 q8[8];
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const float4 hv = hrow[c * 8 + q];
-        q8[q].x = hv.x > 0.f ? v[q * 4] : 0.f; q8[q].y = hv.y > 0.f ? v[q * 4 + 1] : 0.f;
-        q8[q].z = hv.z > 0.f ? v[q * 4 + 2] : 0.f; q8[q].w = hv.w > 0.f ? v[q * 4 + 3] : 0.f;
-        const float zs[4] = {q8[q].x, q8[q].y, q8[q].z, q8[q].w};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const uint32_t hb = tf32_hi_bits(zs[e]);
-          hi[q * 4 + e] = hb;
-          lo[q * 4 + e] = __float_as_uint(zs[e] - __uint_as_float(hb));
-        }
-      }
-      tmem_st32(tmem + lane_base + cAhi + c * 32, hi);      // the dH1 MMA has completed: the dZ2 operand columns are free
-      tmem_st32(tmem + lane_base + cAlo + c * 32, lo);
-      warp_stage_chunk(stg, q8, lane);
-      const int j = c * 32 + lane;
-      // dvb[ray][j]: per-ray sums of column j over the warp's rows (rows are sorted by ray)
-      if (one_ray) {
-        float sum = 0.f;
-#pragma unroll 8
-        for (int sidx = 0; sidx < 32; ++sidx) sum += stg[sidx * kStgStride + lane];
-        atomicAdd(g_vb + (int64_t)ray0 * kHidden + j, sum);
-      } else {
-        float run = 0.f;
-        int run_ray = -1;
-        for (int sidx = 0; sidx < 32; ++sidx) {
-          const int r = sRay[warp * 32 + sidx];          // warp-uniform
-          if (r != run_ray) {
-            if (run_ray >= 0) atomicAdd(g_vb + (int64_t)run_ray * kHidden + j, run);
-            run_ray = r;
-            run = 0.f;
-          }
-          run += stg[sidx * kStgStride + lane];
-        }
-        if (run_ray >= 0) atomicAdd(g_vb + (int64_t)run_ray * kHidden + j, run);
-      }
-      // dW1k[j][0..11] += sum_s dZ1[s][j] X[s][0..11]
-      float acc[kFeat];
-#pragma unroll
-      for (int k = 0; k < kFeat; ++k) acc[k] = 0.f;
-#pragma unroll 4
-      for (int sidx = 0; sidx < 32; ++sidx) {
-        const float d = stg[sidx * kStgStride + lane];
-        const float4* xs = reinterpret_cast<const float4*>(sX + (warp * 32 + sidx) * kFeat);
-        const float4 xa = xs[0], xb = xs[1], xc = xs[2];
-        acc[0] = fmaf(d, xa.x, acc[0]); acc[1] = fmaf(d, xa.y, acc[1]); acc[2] = fmaf(d, xa.z, acc[2]); acc[3] = fmaf(d, xa.w, acc[3]);
-        acc[4] = fmaf(d, xb.x, acc[4]); acc[5] = fmaf(d, xb.y, acc[5]); acc[6] = fmaf(d, xb.z, acc[6]); acc[7] = fmaf(d, xb.w, acc[7]);
-        acc[8] = fmaf(d, xc.x, acc[8]); acc[9] = fmaf(d, xc.y, acc[9]); acc[10] = fmaf(d, xc.z, acc[10]); acc[11] = fmaf(d, xc.w, acc[11]);
-      }
-#pragma unroll
-      for (int k = 0; k < kFeat; ++k) atomicAdd(sAccW1 + j * kFeat + k, acc[k]);
-      __syncwarp();
-    }
-    tmem_st_wait();
-    tc_fence_before();
-    __syncthreads();
-    // ---- dX = dZ1 . W1k  (N = 16) ----
-    if (warp == 0 && elect_one()) {   // one elected lane of a CONVERGED warp: plain UTCHMMA issue (see elect_one)
-      tc_fence_after();
-#pragma unroll 4
-      for (int ks = 0; ks < kHidden / 8; ++ks) {
-        mma_ts_idesc(tmem + cDX, tmem + cAhi + ks * 8, dW1hi + ks * kStepK16, kIdescN16, ks > 0);
-        if (kThree) {
-          mma_ts_idesc(tmem + cDX, tmem + cAlo + ks * 8, dW1hi + ks * kStepK16, kIdescN16, 1);
-          mma_ts_idesc(tmem + cDX, tmem + cAhi + ks * 8, dW1lo + ks * kStepK16, kIdescN16, 1);
-        }
-      }
-      mma_commit(bar_addr);
-    }
-    mbar_wait(bar_addr, phase);
-    phase ^= 1;
-    tc_fence_after();
+    // dW1k^T = X^T . dZ1 (A rows 0..11) and per-ray sums of dZ1 (A rows 12..15 = indicators of up to 4 ray segments)
+    tile_store(S, d1, g, t);
+    __syncwarp();                                             // the tile is read back across lanes as B fragments below
+    const int64_t my_ray = (lane < kUnit && r0 + lane < n_pts) ? ray_id[r0 + lane] : -1;
+    const int64_t prev_ray = __shfl_up_sync(0xffffffffu, my_ray, 1);
+    const uint32_t starts = __ballot_sync(0xffffffffu, lane < kUnit && my_ray >= 0 && (lane == 0 || prev_ray != my_ray));
+    const bool segs_fit = __popc(starts) <= 4;
     {
-      float v[16];
-      tmem_ld16(tmem + lane_base + cDX, v);
-      if (live) {
-        float4* o = reinterpret_cast<float4*>(g_feat + row * kFeat);
-        o[0] = make_float4(v[0], v[1], v[2], v[3]);
-        o[1] = make_float4(v[4], v[5], v[6], v[7]);
-        o[2] = make_float4(v[8], v[9], v[10], v[11]);
-      }
-    }
-    tc_fence_before();
-    __syncthreads();     // TMEM reads done, smem row tables free for the next tile
-  }
-
-  // ---- flush the CTA partials ----
-  atomicAdd(sAccB3 + 0, b3a); atomicAdd(sAccB3 + 1, b3b); atomicAdd(sAccB3 + 2, b3c);
-  __syncthreads();
-  for (int i = tid; i < kHidden * kFeat; i += kRows) atomicAdd(gW1k + i, sAccW1[i]);
-  for (int i = tid; i < 3 * kHidden; i += kRows) atomicAdd(gW3 + i, sAccW3[i]);
-  atomicAdd(gb2 + tid, sAccB2[tid]);
-  if (tid < 3) atomicAdd(gb3 + tid, sAccB3[tid]);
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem) : "memory");
-  }
-}
-
-
-// =====================================================================================================================
-// k_shade_bwd_fused, warp-specialised: the sample reductions of the kernel above cost as much as its tensor-core chain when the
-// same four warps do both (measured: 18.5 us per 128-sample tile against 9.5 us for the chain alone -- one warp per scheduler
-// cannot hide the shared-memory latency of the column loops).  Here the CTA has EIGHT warps:
-//   warps 0-3 (row warps, thread = sample row): dZ2 -> TMEM, dH1 MMA, dZ1 -> TMEM, dX MMA, dX store -- and after computing a
-//       32 x 32 chunk of H2 / dZ1 they only STAGE it in shared memory (double-buffered per warp) and signal an mbarrier;
-//   warps 4-7 (column warps, lane = hidden unit): consume the staged chunks of "their" row warp: db2 / dW3 from H2 chunks, dvb
-//       (per ray) / dW1k from dZ1 chunks, releasing each buffer through a second mbarrier.
-// The two halves run concurrently on the four schedulers (two warps each).  Per-tile row tables (dz3, ray id, X) are
-// double-buffered by tile parity; the producer can run at most two chunks ahead, so a table is never overwritten while in use.
-// =====================================================================================================================
-namespace bf2 {
-constexpr uint32_t oVThi = 0;
-constexpr uint32_t oVTlo = oVThi + (kHidden / 4) * kPanelBytes;
-constexpr uint32_t oV1hi = oVTlo + (kHidden / 4) * kPanelBytes;
-constexpr uint32_t oV1lo = oV1hi + (kHidden / 4) * bf::kPanelN16;
-constexpr uint32_t oStg2 = oV1lo + (kHidden / 4) * bf::kPanelN16;   // [4 row warps][2][32 x 36 floats]
-constexpr uint32_t oX2 = oStg2 + 8 * kStgBytesPerWarp;              // [2][128][12]
-constexpr uint32_t oDz32 = oX2 + 2 * kRows * kFeat * 4;             // [2][128] float4
-constexpr uint32_t oRay2 = oDz32 + 2 * kRows * 16;                  // [2][128] int
-constexpr uint32_t oW32 = oRay2 + 2 * kRows * 4;                    // [3][128]
-constexpr uint32_t oAccW1b = oW32 + 3 * kHidden * 4;
-constexpr uint32_t oAccW3b = oAccW1b + kHidden * kFeat * 4;
-constexpr uint32_t oAccB2b = oAccW3b + 3 * kHidden * 4;
-constexpr uint32_t oAccB3b = oAccB2b + kHidden * 4;
-constexpr uint32_t oFull = oAccB3b + 16;                             // [4][2] mbarriers
-constexpr uint32_t oEmpty = oFull + 64;                              // [4][2]
-constexpr uint32_t oBar2 = oEmpty + 64;                              // MMA mbarrier + TMEM slot
-constexpr uint32_t kSmemBytesF2 = oBar2 + 16;
-}  // namespace bf2
-
-// Phase timestamps of CTA 0 (tiles 4..7 of its range) for scripts/trace_ws.cu; compiled out of the library.
-#ifdef UBN_WS_TRACE
-__device__ long long g_ws_trace[4 * 8 * 64];
-#define WS_T(slot)                                                                                                   \
-  do {                                                                                                               \
-    const int64_t tt_ = tile - tile_begin - 4;                                                                       \
-    if (blockIdx.x == 0 && lane == 0 && tt_ >= 0 && tt_ < 4) g_ws_trace[(tt_ * 8 + warp) * 64 + (slot)] = clock64(); \
-  } while (0)
-#else
-#define WS_T(slot)
-#endif
-
-__device__ __forceinline__ void mbar_arrive(uint32_t bar_smem) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar_smem) : "memory");
-}
-__device__ __forceinline__ void row_warps_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
-
-// kPanel: h1 / h2 in the panel layout of k_shade_fwd_tc<.., kPanel = true>.  kMask1 (panel only): dZ1 = dH1 * [H1 > 0] takes the mask
-// bits the forward left in h1_mask instead of loading the H1 row, and the register row that H1 used to occupy in phase 2 receives
-// the NEXT tile's H2 row half a tile ahead of its use (phase trace, profiles/r02_trace_ws_phases.txt: 2.7 k of a tile's 16.6 k
-// cycles were the row warps waiting for H2 at the tile start, another 2.5 k pushing the 32 H1 loads through a busy LSU).
-template <bool kThree, bool kPanel, bool kMask1>     // kMask1 also means: db2 is summed by the dW2 launch (which rebuilds dZ2 anyway)
-__global__ void __launch_bounds__(2 * kRows, 1) k_shade_bwd_fused_ws(
-    const float* __restrict__ feat, const int64_t* __restrict__ ray_id, const float* __restrict__ W1k,
-    const float* __restrict__ W2, const float* __restrict__ W3, const float* __restrict__ rgb,
-    const float* __restrict__ h1, const float* __restrict__ h2, const float* __restrict__ g_rgb, int64_t n_pts,
-    float* __restrict__ g_feat, float* __restrict__ g_vb, float* __restrict__ gW1k, float* __restrict__ gb2,
-    float* __restrict__ gW3, float* __restrict__ gb3, uint32_t* __restrict__ h2_mask, const uint32_t* __restrict__ h1_mask) {
-  using namespace bf2;
-  using bf::cAhi; using bf::cAlo; using bf::cDHf; using bf::cDX; using bf::kIdescN16; using bf::kPanelN16;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const bool is_row = warp < 4;
-  const int rw = warp & 3;                                  // the row warp this warp is / serves
-  float* sW3 = reinterpret_cast<float*>(smem + oW32);
-  float* sAccW1 = reinterpret_cast<float*>(smem + oAccW1b);
-  float* sAccW3 = reinterpret_cast<float*>(smem + oAccW3b);
-  float* sAccB2 = reinterpret_cast<float*>(smem + oAccB2b);
-  float* sAccB3 = reinterpret_cast<float*>(smem + oAccB3b);
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + oBar2);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + oBar2 + 8);
-  const uint32_t bar_addr = smem_u32(bar);
-  const uint32_t full0 = smem_u32(smem + oFull + rw * 16), empty0 = smem_u32(smem + oEmpty + rw * 16);   // + 8 * buffer
-
-  for (int i = tid; i < kHidden * kHidden; i += 2 * kRows) {
-    const int j = i / kHidden, k = i % kHidden;
-    const float w = W2[i];
-    const uint32_t hb = tf32_hi_bits(w);
-    const uint32_t off = (uint32_t)(j >> 2) * kPanelBytes + (uint32_t)k * 16 + (uint32_t)(j & 3) * 4;
-    *reinterpret_cast<uint32_t*>(smem + oVThi + off) = hb;
-    *reinterpret_cast<float*>(smem + oVTlo + off) = w - __uint_as_float(hb);
-  }
-  for (int i = tid; i < kHidden * 16; i += 2 * kRows) {
-    const int j = i >> 4, c = i & 15;
-    const float w = (c < kFeat) ? W1k[j * kFeat + c] : 0.f;
-    const uint32_t hb = tf32_hi_bits(w);
-    const uint32_t off = (uint32_t)(j >> 2) * kPanelN16 + (uint32_t)c * 16 + (uint32_t)(j & 3) * 4;
-    *reinterpret_cast<uint32_t*>(smem + oV1hi + off) = hb;
-    *reinterpret_cast<float*>(smem + oV1lo + off) = w - __uint_as_float(hb);
-  }
-  for (int i = tid; i < 3 * kHidden; i += 2 * kRows) { sW3[i] = W3[i]; sAccW3[i] = 0.f; }
-  for (int i = tid; i < kHidden * kFeat; i += 2 * kRows) sAccW1[i] = 0.f;
-  if (tid < kHidden) sAccB2[tid] = 0.f;
-  if (tid < 4) sAccB3[tid] = 0.f;
-  if (tid == 0) {
-    mbar_init(bar_addr, 1);
-    for (int q = 0; q < 8; ++q) {
-      mbar_init(smem_u32(smem + oFull + q * 8), 1);
-      mbar_init(smem_u32(smem + oEmpty + q * 8), 1);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_slot)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  fence_async_smem();
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-
-  const int64_t n_tiles = (n_pts + kRows - 1) / kRows;
-  const int64_t per_cta = (n_tiles + gridDim.x - 1) / gridDim.x;
-  const int64_t tile_begin = (int64_t)blockIdx.x * per_cta, tile_end = min(n_tiles, tile_begin + per_cta);
-  uint32_t seq = 0;                                         // chunk-phase counter of this (row warp, column warp) pair
-
-  if (is_row) {
-    // ================================================= row warps =================================================
-    const int rtid = tid;                                   // 0..127 = row within the tile
-    const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-    uint32_t phase = 0;
-    const uint64_t dWThi = make_desc(smem_u32(smem + oVThi)), dWTlo = make_desc(smem_u32(smem + oVTlo));
-    const uint64_t dW1hi = make_desc_lbo(smem_u32(smem + oV1hi), kPanelN16), dW1lo = make_desc_lbo(smem_u32(smem + oV1lo), kPanelN16);
-    constexpr uint64_t kStepK = (uint64_t)((2 * kPanelBytes) >> 4);
-    constexpr uint64_t kStepK16 = (uint64_t)((2 * kPanelN16) >> 4);
-    float b3a = 0.f, b3b = 0.f, b3c = 0.f;
-    auto publish = [&](const float4 (&q8)[8]) {            // stage one 32 x 32 chunk for the column warp
-      const uint32_t b = seq & 1, use = seq >> 1;
-      if (use > 0) mbar_wait(empty0 + 8 * b, (use - 1) & 1);
-      float* stg = reinterpret_cast<float*>(smem + oStg2 + (rw * 2 + b) * kStgBytesPerWarp);
+      float acc[kNT][4];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) *reinterpret_cast<float4*>(stg + lane * kStgStride + i * 4) = q8[i];
-      __syncwarp();
-      if (lane == 0) mbar_arrive(full0 + 8 * b);
-      ++seq;
-    };
-    float4 hrow[kHidden / 4];                                // this thread's H2 row (phase 1) / H1 row (phase 2 without masks)
-    auto load_h2_row = [&](int64_t t) {
-      const int64_t r = t * kRows + rtid;
-      const bool ok = t < tile_end && r < n_pts;
+      for (int j = 0; j < kNT; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
 #pragma unroll
-      for (int q = 0; q < kHidden / 4; ++q) {
-        hrow[q] = make_float4(0, 0, 0, 0);
-        if (ok)
-          hrow[q] = __ldg(reinterpret_cast<const float4*>(kPanel ? h2 + t * (kRows * kHidden) + (int64_t)q * (kRows * 4) + rtid * 4
-                                                                 : h2 + r * kHidden + q * 4));
-      }
-    };
-    if (kMask1) load_h2_row(tile_begin);
-    for (int64_t tile = tile_begin; tile < tile_end; ++tile) {
-      const int tp = (int)((tile - tile_begin) & 1);
-      float* sX = reinterpret_cast<float*>(smem + oX2) + tp * kRows * kFeat;
-      float4* sDz3 = reinterpret_cast<float4*>(smem + oDz32) + tp * kRows;
-      int* sRay = reinterpret_cast<int*>(smem + oRay2) + tp * kRows;
-      const int64_t row = tile * kRows + rtid;
-      const bool live = row < n_pts;
-      float d0 = 0.f, d1 = 0.f, d2 = 0.f;
-      WS_T(0);
-      // the next tile's operands are contiguous (128 consecutive rows): one lane asks L2 for them now, a whole tile ahead of
-      // their use, so that the row loads below (32 LDG.128 per thread, the serial head of every tile) hit L2 instead of HBM
-      if (warp == 1 && tile + 1 < tile_end && elect_one()) {
-        const int64_t r0 = (tile + 1) * kRows;
-        const uint32_t nr = (uint32_t)min((int64_t)kRows, n_pts - r0);
-        if (!kMask1) {
-          l2_prefetch(h2 + r0 * kHidden, (kPanel ? (uint32_t)kRows : nr) * kHidden * 4);   // panel layout: rows interleaved, buffer padded
-          l2_prefetch(h1 + r0 * kHidden, (kPanel ? (uint32_t)kRows : nr) * kHidden * 4);
-        } else if (tile + 2 < tile_end) {     // the H2 row of tile + 1 is fetched into registers during THIS tile: ask L2 two tiles ahead
-          l2_prefetch(h2 + (r0 + kRows) * kHidden, (uint32_t)kRows * kHidden * 4);
+      for (int s = 0; s < 2; ++s) {
+        float av[4];
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {                         // sample k = 8 s + t + 4 q
+          const int64_t rr = r0 + 8 * s + t + 4 * q;
+          const int ks = 8 * s + t + 4 * q;
+          const bool ok = rr < n_pts;
+          av[2 * q] = ok ? feat[rr * kFeat + g] : 0.f;                         // A row g: feature g
+          float lo = 0.f;                                                       // A row g + 8: feature g + 8 or segment g - 4
+          if (ok) {
+            if (g < 4) lo = feat[rr * kFeat + g + 8];
+            else if (segs_fit) lo = (__popc(starts & ((2u << ks) - 1u)) - 1 == g - 4) ? 1.f : 0.f;
+          }
+          av[2 * q + 1] = lo;
         }
-        l2_prefetch(feat + r0 * kFeat, nr * kFeat * 4);
-        l2_prefetch(rgb + r0 * 3, (nr * 12) & ~15u);
-        l2_prefetch(g_rgb + r0 * 3, (nr * 12) & ~15u);
-        l2_prefetch(ray_id + r0, nr * 8);
-      }
-      if (!kMask1) load_h2_row(tile);                        // H2 row first: the longest wait of the tile starts at once
-      uint32_t m1[kHidden / 32] = {0u, 0u, 0u, 0u};          // ReLU mask of my H1 row
-      if (kMask1 && live) {
+        const float a[4] = {av[0], av[1], av[2], av[3]};
+        uint32_t ah[4], al[4];
+        split4(a, ah, al);
 #pragma unroll
-        for (int c = 0; c < kHidden / 32; ++c) m1[c] = __ldg(h1_mask + tile * 512 + c * 128 + rtid);
+        for (int j = 0; j < kNT; ++j) {
+          uint32_t bh[2], bl[2];
+          tile_frag(S, s, j, g, t, bh, bl);
+          mma3<kThree>(acc[j], ah, al, make_uint4(bh[0], bh[1], bl[0], bl[1]));
+        }
       }
+#pragma unroll
+      for (int j = 0; j < kNT; ++j) {
+        const int c = 8 * j + 2 * t;
+        atomicAdd(accW1 + g * kHidden + c, acc[j][0]);
+        atomicAdd(accW1 + g * kHidden + c + 1, acc[j][1]);
+        if (g < 4) {
+          atomicAdd(accW1 + (g + 8) * kHidden + c, acc[j][2]);
+          atomicAdd(accW1 + (g + 8) * kHidden + c + 1, acc[j][3]);
+        }
+      }
+      // ray of segment q = the ray of its first sample (every lane shuffles: warp-uniform)
+      int64_t seg_ray[4];
       {
-        int my_ray = -1;
-        float4 x0 = make_float4(0, 0, 0, 0), x1 = x0, x2 = x0;
-        if (live) {
-          const float* o = rgb + row * 3;
-          const float* g = g_rgb + row * 3;
-          d0 = g[0] * (o[0] * (1.f - o[0]));
-          d1 = g[1] * (o[1] * (1.f - o[1]));
-          d2 = g[2] * (o[2] * (1.f - o[2]));
-          my_ray = (int)ray_id[row];
-          const float4* xr = reinterpret_cast<const float4*>(feat + row * kFeat);
-          x0 = __ldg(xr); x1 = __ldg(xr + 1); x2 = __ldg(xr + 2);
-        }
-        sDz3[rtid] = make_float4(d0, d1, d2, 0.f);
-        sRay[rtid] = my_ray;
-        float4* xs = reinterpret_cast<float4*>(sX + rtid * kFeat);
-        xs[0] = x0; xs[1] = x1; xs[2] = x2;
-        b3a += d0; b3b += d1; b3c += d2;
-      }
-      WS_T(1);
+        uint32_t m = starts;
 #pragma unroll
-      for (int c = 0; c < kHidden / 32; ++c) {
-        uint32_t hi[32], lo[32];
-        float4 q8[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const float4 hv = hrow[c * 8 + q];
-          q8[q] = hv;
-          const float4 wa = *reinterpret_cast<const float4*>(sW3 + c * 32 + q * 4);
-          const float4 wb = *reinterpret_cast<const float4*>(sW3 + kHidden + c * 32 + q * 4);
-          const float4 wc = *reinterpret_cast<const float4*>(sW3 + 2 * kHidden + c * 32 + q * 4);
-          const float z[4] = {hv.x > 0.f ? fmaf(d2, wc.x, fmaf(d1, wb.x, d0 * wa.x)) : 0.f,
-                              hv.y > 0.f ? fmaf(d2, wc.y, fmaf(d1, wb.y, d0 * wa.y)) : 0.f,
-                              hv.z > 0.f ? fmaf(d2, wc.z, fmaf(d1, wb.z, d0 * wa.z)) : 0.f,
-                              hv.w > 0.f ? fmaf(d2, wc.w, fmaf(d1, wb.w, d0 * wa.w)) : 0.f};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const uint32_t hb = tf32_hi_bits(z[e]);
-            hi[q * 4 + e] = hb;
-            lo[q * 4 + e] = __float_as_uint(z[e] - __uint_as_float(hb));
-          }
-        }
-        tmem_st32(tmem + lane_base + cAhi + c * 32, hi);
-        if (kThree) tmem_st32(tmem + lane_base + cAlo + c * 32, lo);
-        // dH1 = dZ2 . W2 is issued K-chunk by K-chunk: the four K-steps that read this 32-column piece of dZ2 start as soon as
-        // all four row warps have stored it and run on the tensor pipe while the next piece is computed (issued after the last
-        // piece, the 48 MMAs = ~3 k cycles were pure waiting for the row warps)
-        tmem_st_wait();
-        tc_fence_before();
-        row_warps_sync();
-        if (warp == 0 && elect_one()) {   // one elected lane of a CONVERGED warp: plain UTCHMMA issue (see elect_one)
-          tc_fence_after();
-#pragma unroll
-          for (int k4 = 0; k4 < 4; ++k4) {
-            const int ks = c * 4 + k4;
-            mma_ts(tmem + cDHf, tmem + cAhi + ks * 8, dWThi + ks * kStepK, ks > 0);
-            if (kThree) {
-              mma_ts(tmem + cDHf, tmem + cAlo + ks * 8, dWThi + ks * kStepK, 1);
-              mma_ts(tmem + cDHf, tmem + cAhi + ks * 8, dWTlo + ks * kStepK, 1);
-            }
-          }
-          if (c == kHidden / 32 - 1) mma_commit(bar_addr);
-        }
-        publish(q8);                                        // H2 chunk -> db2 / dW3 on the column warp
-        WS_T(2 + c);
-      }
-      WS_T(6);
-      if (kMask1) {
-        load_h2_row(tile + 1);                               // the H2 row is consumed: the next tile's goes into the same registers now
-      } else {
-#pragma unroll
-        for (int q = 0; q < kHidden / 4; ++q) {
-          hrow[q] = make_float4(0, 0, 0, 0);
-          if (live)
-            hrow[q] = __ldg(reinterpret_cast<const float4*>(kPanel ? h1 + tile * (kRows * kHidden) + (int64_t)q * (kRows * 4) + rtid * 4
-                                                                   : h1 + row * kHidden + q * 4));
+        for (int q = 0; q < 4; ++q) {
+          const int src = m ? __ffs(m) - 1 : 0;
+          seg_ray[q] = __shfl_sync(0xffffffffu, my_ray, src);
+          if (!m) seg_ray[q] = -1;
+          m &= m - 1;
         }
       }
-      WS_T(7);
-      mbar_wait(bar_addr, phase);
-      phase ^= 1;
-      tc_fence_after();
-      WS_T(8);
+      if (segs_fit && g >= 4) {
+        const int64_t ray = seg_ray[g - 4];
+        if (ray >= 0) {
 #pragma unroll
-      for (int c = 0; c < kHidden / 32; ++c) {
-        float v[32];
-        tmem_ld32(tmem + lane_base + cDHf + c * 32, v);
-        uint32_t hi[32], lo[32];
-        float4 q8[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          if (kMask1) {
-            const uint32_t mb = m1[c] >> (q * 4);
-            q8[q].x = (mb & 1u) ? v[q * 4] : 0.f; q8[q].y = (mb & 2u) ? v[q * 4 + 1] : 0.f;
-            q8[q].z = (mb & 4u) ? v[q * 4 + 2] : 0.f; q8[q].w = (mb & 8u) ? v[q * 4 + 3] : 0.f;
-          } else {
-            const float4 hv = hrow[c * 8 + q];
-            q8[q].x = hv.x > 0.f ? v[q * 4] : 0.f; q8[q].y = hv.y > 0.f ? v[q * 4 + 1] : 0.f;
-            q8[q].z = hv.z > 0.f ? v[q * 4 + 2] : 0.f; q8[q].w = hv.w > 0.f ? v[q * 4 + 3] : 0.f;
-          }
-          const float zs[4] = {q8[q].x, q8[q].y, q8[q].z, q8[q].w};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const uint32_t hb = tf32_hi_bits(zs[e]);
-            hi[q * 4 + e] = hb;
-            lo[q * 4 + e] = __float_as_uint(zs[e] - __uint_as_float(hb));
+          for (int j = 0; j < kNT; ++j) {
+            atomicAdd(grad_view_bias + ray * kHidden + 8 * j + 2 * t, acc[j][2]);
+            atomicAdd(grad_view_bias + ray * kHidden + 8 * j + 2 * t + 1, acc[j][3]);
           }
         }
-        tmem_st32(tmem + lane_base + cAhi + c * 32, hi);
-        if (kThree) tmem_st32(tmem + lane_base + cAlo + c * 32, lo);
-        publish(q8);                                        // dZ1 chunk -> dvb / dW1k on the column warp
-        WS_T(9 + c);
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      row_warps_sync();
-      WS_T(13);
-      if (warp == 0 && elect_one()) {   // one elected lane of a CONVERGED warp: plain UTCHMMA issue (see elect_one)
-        tc_fence_after();
-#pragma unroll 4
-        for (int ks = 0; ks < kHidden / 8; ++ks) {
-          mma_ts_idesc(tmem + cDX, tmem + cAhi + ks * 8, dW1hi + ks * kStepK16, kIdescN16, ks > 0);
-          if (kThree) {
-            mma_ts_idesc(tmem + cDX, tmem + cAlo + ks * 8, dW1hi + ks * kStepK16, kIdescN16, 1);
-            mma_ts_idesc(tmem + cDX, tmem + cAhi + ks * 8, dW1lo + ks * kStepK16, kIdescN16, 1);
-          }
-        }
-        mma_commit(bar_addr);
-      }
-      WS_T(14);
-      mbar_wait(bar_addr, phase);
-      phase ^= 1;
-      tc_fence_after();
-      WS_T(15);
-      {
-        float v[16];
-        tmem_ld16(tmem + lane_base + cDX, v);
-        if (live) {
-          float4* o = reinterpret_cast<float4*>(g_feat + row * kFeat);
-          o[0] = make_float4(v[0], v[1], v[2], v[3]);
-          o[1] = make_float4(v[4], v[5], v[6], v[7]);
-          o[2] = make_float4(v[8], v[9], v[10], v[11]);
-        }
-      }
-      tc_fence_before();
-      row_warps_sync();                                     // TMEM reads done before the next tile's stores
-      WS_T(16);
-    }
-    atomicAdd(sAccB3 + 0, b3a); atomicAdd(sAccB3 + 1, b3b); atomicAdd(sAccB3 + 2, b3c);
-  } else {
-    // ================================================ column warps ================================================
-    auto acquire = [&]() -> const float* {
-      const uint32_t b = seq & 1, use = seq >> 1;
-      mbar_wait(full0 + 8 * b, use & 1);
-      return reinterpret_cast<const float*>(smem + oStg2 + (rw * 2 + b) * kStgBytesPerWarp);
-    };
-    auto release = [&]() {
-      __syncwarp();
-      if (lane == 0) mbar_arrive(empty0 + 8 * (seq & 1));
-      ++seq;
-    };
-    // Every column warp owns the same (32 rows of its row warp) x (all 128 hidden units) strip in every tile, so the
-    // per-hidden-unit sums of lane j live in REGISTERS for the whole kernel (64 per lane) and reach shared memory once, at the
-    // end.  (They used to be shared-memory atomics after every chunk: ncu attributed 24 % of the kernel's stall samples and
-    // 60 % of its shared-memory wavefronts to those 16 four-way-conflicting ATOMS per chunk.)
-    float accW1[kHidden / 32][kFeat], accW3[kHidden / 32][3], accB2[kHidden / 32];
-#pragma unroll
-    for (int c = 0; c < kHidden / 32; ++c) {
-#pragma unroll
-      for (int k = 0; k < kFeat; ++k) accW1[c][k] = 0.f;
-      accW3[c][0] = accW3[c][1] = accW3[c][2] = 0.f;
-      accB2[c] = 0.f;
-    }
-    for (int64_t tile = tile_begin; tile < tile_end; ++tile) {
-      const int tp = (int)((tile - tile_begin) & 1);
-      const float* sX = reinterpret_cast<const float*>(smem + oX2) + tp * kRows * kFeat;
-      const float4* sDz3 = reinterpret_cast<const float4*>(smem + oDz32) + tp * kRows;
-      const int* sRay = reinterpret_cast<const int*>(smem + oRay2) + tp * kRows;
-      // ---- H2 chunks: db2[j] += sum_s dZ2[s][j],  dW3[c][j] += sum_s dz3[s][c] H2[s][j] ----
-#pragma unroll
-      for (int c = 0; c < kHidden / 32; ++c) {
-        WS_T(c);
-        const float* stg = acquire();
-        WS_T(8 + c);
-        const int j = c * 32 + lane;
-        const float w3a = sW3[j], w3b = sW3[kHidden + j], w3c = sW3[2 * kHidden + j];
-        float a0 = accW3[c][0], a1 = accW3[c][1], a2 = accW3[c][2], ab = accB2[c];
-        uint32_t my_mask = 0;                               // lane s: bit j = [H2[s][32 c + j] > 0]
-#pragma unroll 8
-        for (int sidx = 0; sidx < 32; ++sidx) {
-          const float h = stg[sidx * kStgStride + lane];
-          const float4 dz = sDz3[rw * 32 + sidx];
-          a0 = fmaf(dz.x, h, a0); a1 = fmaf(dz.y, h, a1); a2 = fmaf(dz.z, h, a2);
-          if (!kMask1) ab += h > 0.f ? fmaf(dz.z, w3c, fmaf(dz.y, w3b, dz.x * w3a)) : 0.f;
-          const uint32_t b = __ballot_sync(0xffffffffu, h > 0.f);      // the ReLU mask of sample sidx over this chunk's 32 units
-          if (lane == sidx) my_mask = b;
-        }
-        release();
-        // ReLU masks of H2 for the dW2 kernel, [tile][chunk][row] (one 128-byte store per warp and chunk): with them dW2 rebuilds
-        // dZ2 from dz3 and W3 without reading the 2.1 GB of H2 a second time
-        if (h2_mask) h2_mask[tile * 512 + c * 128 + rw * 32 + lane] = my_mask;
-        WS_T(16 + c);
-        accW3[c][0] = a0; accW3[c][1] = a1; accW3[c][2] = a2; accB2[c] = ab;
-      }
-      // ---- dZ1 chunks: dvb[ray][j] += sum_{s in ray} dZ1[s][j],  dW1k[j][0..11] += sum_s dZ1[s][j] X[s][0..11] ----
-#pragma unroll
-      for (int c = 0; c < kHidden / 32; ++c) {
-        WS_T(4 + c);
-        const float* stg = acquire();                       // acquire first: the tile's tables are visible from here on
-        WS_T(12 + c);
-        const int my_ray = sRay[rw * 32 + lane];
-        const int ray0 = __shfl_sync(0xffffffffu, my_ray, 0);
-        const bool one_ray = __all_sync(0xffffffffu, my_ray == ray0) && ray0 >= 0;
-        const int j = c * 32 + lane;
-        float run = 0.f;
-        int run_ray = one_ray ? ray0 : -1;
-#define UBN_DW1K_FMA()                                                                                     \
-        do {                                                                                               \
-          const float4* xs = reinterpret_cast<const float4*>(sX + (rw * 32 + sidx) * kFeat);               \
-          const float4 xa = xs[0], xb = xs[1], xc = xs[2];                                                 \
-          accW1[c][0] = fmaf(d, xa.x, accW1[c][0]); accW1[c][1] = fmaf(d, xa.y, accW1[c][1]);              \
-          accW1[c][2] = fmaf(d, xa.z, accW1[c][2]); accW1[c][3] = fmaf(d, xa.w, accW1[c][3]);              \
-          accW1[c][4] = fmaf(d, xb.x, accW1[c][4]); accW1[c][5] = fmaf(d, xb.y, accW1[c][5]);              \
-          accW1[c][6] = fmaf(d, xb.z, accW1[c][6]); accW1[c][7] = fmaf(d, xb.w, accW1[c][7]);              \
-          accW1[c][8] = fmaf(d, xc.x, accW1[c][8]); accW1[c][9] = fmaf(d, xc.y, accW1[c][9]);              \
-          accW1[c][10] = fmaf(d, xc.z, accW1[c][10]); accW1[c][11] = fmaf(d, xc.w, accW1[c][11]);          \
-        } while (0)
-        if (one_ray) {
-          // the common case (S samples per ray >> 32): straight-line body, so the unrolled iterations' LDS are hoisted above the
-          // FMAs (with the ray-change test in the loop every iteration waited for its own loads: 94 cycles per sample)
-#pragma unroll 8
-          for (int sidx = 0; sidx < 32; ++sidx) {
-            const float d = stg[sidx * kStgStride + lane];
-            run += d;
-            UBN_DW1K_FMA();
-          }
-        } else {
-#pragma unroll 2
-          for (int sidx = 0; sidx < 32; ++sidx) {
-            const float d = stg[sidx * kStgStride + lane];
-            const int r = sRay[rw * 32 + sidx];
-            if (r != run_ray) {                             // warp-uniform branch
-              if (run_ray >= 0) atomicAdd(g_vb + (int64_t)run_ray * kHidden + j, run);
-              run_ray = r;
-              run = 0.f;
-            }
-            run += d;
-            UBN_DW1K_FMA();
-          }
-        }
-#undef UBN_DW1K_FMA
-        release();
-        WS_T(20 + c);
-        if (run_ray >= 0) atomicAdd(g_vb + (int64_t)run_ray * kHidden + j, run);
       }
     }
-    // the four column warps hold partials of the SAME hidden units (different rows): combine them in shared memory, [k][j]
-    // layout so that the 32 lanes of one atomic hit 32 banks
+    if (!segs_fit) {                                          // more than 4 rays in 16 samples: per-sample adds
 #pragma unroll
-    for (int c = 0; c < kHidden / 32; ++c) {
-      const int j = c * 32 + lane;
+      for (int r = 0; r < 2; ++r) {
+        if (!live[r]) continue;
+        const int64_t ray = ray_id[row[r]];
 #pragma unroll
-      for (int k = 0; k < kFeat; ++k) atomicAdd(sAccW1 + k * kHidden + j, accW1[c][k]);
-      atomicAdd(sAccW3 + j, accW3[c][0]); atomicAdd(sAccW3 + kHidden + j, accW3[c][1]);
-      atomicAdd(sAccW3 + 2 * kHidden + j, accW3[c][2]);
-      atomicAdd(sAccB2 + j, accB2[c]);
+        for (int j = 0; j < kNT; ++j) {
+          atomicAdd(grad_view_bias + ray * kHidden + 8 * j + 2 * t, d1[j][2 * r]);
+          atomicAdd(grad_view_bias + ray * kHidden + 8 * j + 2 * t + 1, d1[j][2 * r + 1]);
+        }
+      }
     }
+    __syncwarp();
   }
-
-  // ---- flush the CTA partials ----
+  if (kDz1Out) return;
   __syncthreads();
-  for (int i = tid; i < kHidden * kFeat; i += 2 * kRows)      // sAccW1 is [k][j]; gW1k is [j][k]
-    atomicAdd(gW1k + i, sAccW1[(i % kFeat) * kHidden + i / kFeat]);
-  for (int i = tid; i < 3 * kHidden; i += 2 * kRows) atomicAdd(gW3 + i, sAccW3[i]);
-  if (!kMask1 && tid < kHidden) atomicAdd(gb2 + tid, sAccB2[tid]);
-  if (tid < 3) atomicAdd(gb3 + tid, sAccB3[tid]);
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem) : "memory");
+  for (int i = tid; i < kFeat * kHidden; i += kThreads) {        // accW1 is dW1k^T: [feature][unit]
+    const int f = i / kHidden, c = i % kHidden;
+    atomicAdd(grad_W1k + c * kFeat + f, accW1[i]);
   }
+  for (int i = tid; i < 3 * kHidden; i += kThreads) atomicAdd(grad_W3 + i, accW3[i]);
+  for (int i = tid; i < kHidden; i += kThreads) atomicAdd(grad_b2 + i, accB2[i]);
+  if (tid < 3) atomicAdd(grad_b3 + tid, accB3[tid]);
 }
 
-
-// ---- dW2 += dZ2^T . H1 as its own split-K GEMM ----------------------------------------------------------------------
-// Round = 32 consecutive samples.  Warp w stages rows 4w..4w+3; lane l serves row (l & 3) and hidden units j = 8*jj + (l >> 2)
-// (jj < 16): for one store instruction the 32 lanes hit 32 distinct banks of one K-major panel (conflict free).
-// The kernel is bound by the load/store pipe (ncu: l1tex 68 %, long-scoreboard stalls): every thread prefetches the next round's
-// 32 values into registers before it waits for the tensor pipe to release the single staging buffer, and one lane asks L2 for the
-// next 128-sample tile of both saves (cp.async.bulk.prefetch) while the current one is consumed.
-//
-// ACCUMULATION LENGTH.  The tensor core adds into its fp32 accumulator with TRUNCATION, not round-to-nearest: a chain of n
-// accumulating MMAs carries a systematic bias of ~n/2 ulp of the running value.  Harmless for the K = 128 chains of the other
-// kernels (48 MMAs: ~1.4e-6), but a split-K GEMM over samples is one chain per CTA -- 3 540 MMAs on the truck workload -- and the
-// round-2 parity run at size measured exactly that: dW2 off by 1.4e-4 of its scale on truck (295 rounds per CTA), 4.5e-5 on bicycle
-// (91 rounds), linear in the chain length, against 2.6e-6 for the reference's cuBLAS path (tests/test_gpu_parity_at_size.py).
-// So the MMA accumulator is restarted every kFlush = 4 rounds (48 MMAs) and the group results are summed with ordinary fp32
-// round-to-nearest adds into a RUNNING SUM that lives in a second 128-column block of tensor memory (tcgen05.ld / add / tcgen05.st
-// by the eight warps: TMEM as a 64 KB private scratchpad; no registers held across rounds, no shared memory, no HBM / L2 traffic).
-// 256 TMEM columns per CTA -> two co-resident CTAs per SM.
+// ---- backward, launch 2: dW2 += dZ2^T . H1 -------------------------------------------------------------------------------
+// A split-K GEMM over samples: each CTA takes 32-sample chunks, stages dZ2 (rebuilt from dz3, W3 and H2 or its ReLU masks) and
+// H1 as [32][kStride] tiles, and warp w accumulates output rows 16 w .. 16 w + 15.  The MMA accumulator restarts every chunk
+// and is added into an fp32 running sum, so the tensor core never carries a long accumulation chain.
 namespace dw {
-constexpr int kThreadsDW = 256;
-constexpr uint32_t kK = 32;
-constexpr uint32_t kOpBytes = (kK / 4) * kPanelBytes;          // 16 KB per operand
-constexpr uint32_t oW3d = 4 * kOpBytes;                        // A hi, A lo, B hi, B lo
-constexpr uint32_t oBarD = oW3d + 3 * kHidden * 4;             // mbarrier + tmem slot
-constexpr uint32_t kSmemBytesD = oBarD + 16;
-constexpr int kCtasPerSM = 2;
-constexpr int kFlush = 4;                                      // rounds per MMA accumulation chain (= one 128-sample tile)
-constexpr uint32_t cAcc = 0, cSum = 128;                       // TMEM columns: MMA accumulator, running fp32 sum
+constexpr int kThreads = 256;
+constexpr int kK = 32;
+constexpr uint32_t oW3 = 0;
+constexpr uint32_t oA = oW3 + 3 * kHidden * 4;
+constexpr uint32_t oB = oA + kK * kStride * 4;
+constexpr uint32_t kSmem = oB + kK * kStride * 4;
 }  // namespace dw
 
-template <bool kThree, bool kPanel>
-__global__ void __launch_bounds__(dw::kThreadsDW, dw::kCtasPerSM) k_shade_dw2_tc(
-    const float* __restrict__ W3, const float* __restrict__ rgb, const float* __restrict__ h1, const float* __restrict__ h2,
-    const float* __restrict__ g_rgb, int64_t n_pts, float* __restrict__ gW2) {
-  using namespace dw;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  float* sW3 = reinterpret_cast<float*>(smem + oW3d);
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + oBarD);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + oBarD + 8);
-  const uint32_t bar_addr = smem_u32(bar);
-  for (int i = tid; i < 3 * kHidden; i += kThreadsDW) sW3[i] = W3[i];
-  if (tid == 0) {
-    mbar_init(bar_addr, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 256;" ::"r"(smem_u32(tmem_slot)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  fence_async_smem();
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  constexpr uint64_t kStepK = (uint64_t)((2 * kPanelBytes) >> 4);
-  const uint64_t dAhi = make_desc(smem_u32(smem)), dAlo = make_desc(smem_u32(smem + kOpBytes));
-  const uint64_t dBhi = make_desc(smem_u32(smem + 2 * kOpBytes)), dBlo = make_desc(smem_u32(smem + 3 * kOpBytes));
-
-  // contiguous range of rounds per CTA, aligned to whole 128-sample tiles (kFlush rounds) so that a chain never straddles CTAs
-  const int64_t n_rounds = (n_pts + kK - 1) / kK;
-  const int64_t n_groups = (n_rounds + kFlush - 1) / kFlush;
-  const int64_t g_per_cta = (n_groups + gridDim.x - 1) / gridDim.x;
-  const int64_t r_begin = (int64_t)blockIdx.x * g_per_cta * kFlush, r_end = min(n_rounds, r_begin + g_per_cta * kFlush);
-  uint32_t phase = 0;
-  const uint32_t s_local = (uint32_t)warp * 4 + (uint32_t)(lane & 3);
-  const uint32_t soff = (s_local >> 2) * kPanelBytes + (s_local & 3) * 4;
-  const int q = lane >> 2;
-  // this warp's share of the 128 x 128 result in tensor memory: lane quarter (warp & 3), column half (warp >> 2)
-  const uint32_t my_tmem = tmem + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(warp >> 2) * 64;
-
-  float p2[kHidden / 8], p1[kHidden / 8], pd[3];     // prefetched h2 / h1 values and dz3 of my row for the coming round
-  auto prefetch = [&](int64_t rd) {
-    const int64_t row = rd * kK + s_local;
-    const bool live = rd < r_end && row < n_pts;
-    pd[0] = pd[1] = pd[2] = 0.f;
-    if (live) {
-      const float* o = rgb + row * 3;
-      const float* g = g_rgb + row * 3;
-      pd[0] = g[0] * (o[0] * (1.f - o[0]));
-      pd[1] = g[1] * (o[1] * (1.f - o[1]));
-      pd[2] = g[2] * (o[2] * (1.f - o[2]));
-    }
+template <bool kThree, bool kPanel, bool kMask2>
+__global__ void __launch_bounds__(dw::kThreads, 1) k_shade_dw2_tc(
+    const float* __restrict__ W3, const float* __restrict__ rgb, const float* __restrict__ h1_save,
+    const float* __restrict__ h2_save, const uint32_t* __restrict__ h2_mask, const float* __restrict__ grad_rgb, int64_t n_pts,
+    float* __restrict__ grad_W2) {
+  extern __shared__ __align__(16) uint8_t smem[];
+  const int tid = threadIdx.x, lane = tid & 31, g = lane >> 2, t = lane & 3, warp = tid >> 5;
+  float* sW3 = reinterpret_cast<float*>(smem + dw::oW3);
+  float* sA = reinterpret_cast<float*>(smem + dw::oA);    // dZ2 [sample][unit]
+  float* sB = reinterpret_cast<float*>(smem + dw::oB);    // H1  [sample][unit]
+  for (int i = tid; i < 3 * kHidden; i += dw::kThreads) sW3[i] = W3[i];
+  float sum[kNT][4];
 #pragma unroll
-    for (int jj = 0; jj < kHidden / 8; ++jj) {
-      const int j = jj * 8 + q;
-      const int64_t idx = kPanel ? (row >> 7) * (int64_t)(kRows * kHidden) + (int64_t)(j >> 2) * (kRows * 4) + (row & 127) * 4 + (j & 3)
-                                 : row * kHidden + j;
-      p2[jj] = live ? __ldg(h2 + idx) : 0.f;
-      p1[jj] = live ? __ldg(h1 + idx) : 0.f;
-    }
-  };
-  // fold the finished chain (MMA accumulator) into the running sum; `first`: the sum block is still uninitialised
-  auto fold = [&](bool first) {
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {           // 16-column pieces keep the transient register footprint small
-      float v[16], sum[16];
-      tmem_ld16(my_tmem + cAcc + c * 16, v);
-      if (!first) {
-        tmem_ld16(my_tmem + cSum + c * 16, sum);
+  for (int j = 0; j < kNT; ++j) sum[j][0] = sum[j][1] = sum[j][2] = sum[j][3] = 0.f;
+  const int sr = tid >> 3;                                 // staging: sample row, 4 float4 column groups per thread
+  const int64_t n_chunks = (n_pts + dw::kK - 1) / dw::kK;
+  for (int64_t ch = blockIdx.x; ch < n_chunks; ch += gridDim.x) {
+    __syncthreads();                                       // previous chunk's fragment reads done (and sW3 staged)
+    const int64_t r = ch * dw::kK + sr;
+    const bool ok = r < n_pts;
+    float dz3[3] = {0.f, 0.f, 0.f};
+    if (ok) {
 #pragma unroll
-        for (int e = 0; e < 16; ++e) v[e] = __fadd_rn(sum[e], v[e]);
+      for (int i = 0; i < 3; ++i) {
+        const float y = rgb[r * 3 + i];
+        dz3[i] = grad_rgb[r * 3 + i] * y * (1.f - y);
       }
-      tmem_st16(my_tmem + cSum + c * 16, v);
-    }
-    tmem_st_wait();
-  };
-  if (r_begin < r_end) prefetch(r_begin);
-  bool pending = false;
-  int n_folded = 0;
-  for (int64_t rd = r_begin; rd < r_end; ++rd) {
-    const int i = (int)(rd - r_begin);
-    float c2[kHidden / 8], c1[kHidden / 8];
-#pragma unroll
-    for (int jj = 0; jj < kHidden / 8; ++jj) { c2[jj] = p2[jj]; c1[jj] = p1[jj]; }
-    const float d0 = pd[0], d1 = pd[1], d2 = pd[2];
-    prefetch(rd + 1);                       // loads for the next round fly while this round is staged and multiplied
-    if ((i % kFlush) == 0 && warp == 1 && rd + kFlush < r_end && elect_one()) {     // next tile of both saves -> L2
-      const int64_t r0 = (rd + kFlush) * kK;
-      const uint32_t nr = (uint32_t)min((int64_t)kRows, n_pts - r0);
-      l2_prefetch(h2 + r0 * kHidden, (kPanel ? (uint32_t)kRows : nr) * kHidden * 4);
-      l2_prefetch(h1 + r0 * kHidden, (kPanel ? (uint32_t)kRows : nr) * kHidden * 4);
-    }
-    if (pending) {                          // tensor pipe must have finished reading the staging buffer
-      mbar_wait(bar_addr, phase);
-      phase ^= 1;
-    }
-    if (i > 0 && (i % kFlush) == 0) {       // the chain of the previous kFlush rounds is complete: fold it, restart the accumulator
-      tc_fence_after();
-      fold(n_folded == 0);
-      ++n_folded;
     }
 #pragma unroll
-    for (int jj = 0; jj < kHidden / 8; ++jj) {
-      const int j = jj * 8 + q;
-      const float z = c2[jj] > 0.f ? fmaf(d2, sW3[2 * kHidden + j], fmaf(d1, sW3[kHidden + j], d0 * sW3[j])) : 0.f;
-      const uint32_t zh = tf32_hi_bits(z), hh = tf32_hi_bits(c1[jj]);
-      const uint32_t off = soff + (uint32_t)j * 16;
-      *reinterpret_cast<uint32_t*>(smem + off) = zh;
-      *reinterpret_cast<float*>(smem + kOpBytes + off) = z - __uint_as_float(zh);
-      *reinterpret_cast<uint32_t*>(smem + 2 * kOpBytes + off) = hh;
-      *reinterpret_cast<float*>(smem + 3 * kOpBytes + off) = c1[jj] - __uint_as_float(hh);
-    }
-    fence_async_smem();
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0 && elect_one()) {   // one elected lane of a CONVERGED warp: plain UTCHMMA issue (see elect_one)
-      tc_fence_after();
-      const bool fresh = (i % kFlush) == 0;
+    for (int q = 0; q < 4; ++q) {
+      const int c = 32 * q + 4 * (tid & 7);
+      float4 h1 = make_float4(0.f, 0.f, 0.f, 0.f), d = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (ok) {
+        h1 = *reinterpret_cast<const float4*>(h1_save + save_idx<kPanel>(r, c));
+        float hv[4];
+        if (kMask2) {
+          const uint32_t w = h2_mask[mask_idx(r, c >> 5)] >> (c & 31);
 #pragma unroll
-      for (int ks = 0; ks < (int)(kK / 8); ++ks) {
-        mma_ss(tmem + cAcc, dAhi + ks * kStepK, dBhi + ks * kStepK, (!fresh || ks > 0) ? 1u : 0u);
-        if (kThree) {
-          mma_ss(tmem + cAcc, dAlo + ks * kStepK, dBhi + ks * kStepK, 1);
-          mma_ss(tmem + cAcc, dAhi + ks * kStepK, dBlo + ks * kStepK, 1);
+          for (int e = 0; e < 4; ++e) hv[e] = ((w >> e) & 1u) ? 1.f : 0.f;
+        } else {
+          const float4 h2 = *reinterpret_cast<const float4*>(h2_save + save_idx<kPanel>(r, c));
+          hv[0] = h2.x; hv[1] = h2.y; hv[2] = h2.z; hv[3] = h2.w;
         }
-      }
-      mma_commit(bar_addr);
-    }
-    pending = true;
-  }
-  if (pending) {
-    mbar_wait(bar_addr, phase);
-    tc_fence_after();
-    fold(n_folded == 0);
-#pragma unroll 1
-    for (int c = 0; c < 2; ++c) {
-      float v[32];
-      tmem_ld32(my_tmem + cSum + c * 32, v);
-      float* dst = gW2 + ((warp & 3) * 32 + lane) * kHidden + (warp >> 2) * 64 + c * 32;
+        float dv[4];
 #pragma unroll
-      for (int e = 0; e < 32; ++e) atomicAdd(dst + e, v[e]);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 256;" ::"r"(tmem) : "memory");
-}
-
-// ---- dW2 from the ReLU masks: the default second launch of the fused backward (panel-layout saves) -----------------------
-// Same GEMM, same chains and running sum as k_shade_dw2_tc, different staging.  That kernel re-reads both activation saves
-// (4.3 GB) and transposes them into the K-major operand panels with 4-byte loads and 4-byte shared-memory stores: 144 load/store
-// instructions per thread and 32-sample round, the load/store pipe at 68 % (ncu) with the tensor pipe at 25 %.  Here
-//   * dZ2 is REBUILT instead of loaded: dZ2[s][j] = [H2[s][j] > 0] (dz3[s] . W3[:, j]).  The masks come from the first launch
-//     (the column warps of k_shade_bwd_fused_ws ballot them while they reduce H2: 2 KB per 128-sample tile instead of 64 KB);
-//     dz3 of a thread's four samples from 96 bytes of rgb / grad_rgb; the W3 columns live in registers;
-//   * a thread owns (hidden unit j, four consecutive samples): the four K-slots of one operand row are ONE 16-byte shared-memory
-//     store, a warp's 32 rows are 512 contiguous bytes (conflict free), and H1 is fetched as 4-byte words of four adjacent rows.
-// Per thread and round: 26 loads + 3 broadcast-free register rebuilds + 16 STS.128, i.e. 3.4x fewer load/store instructions, and
-// H2 is not read at all.
-template <bool kThree>
-__global__ void __launch_bounds__(dw::kThreadsDW, dw::kCtasPerSM) k_shade_dw2_mask_tc(
-    const float* __restrict__ W3, const float* __restrict__ rgb, const float* __restrict__ h1,
-    const uint32_t* __restrict__ h2_mask, const float* __restrict__ g_rgb, int64_t n_pts, float* __restrict__ gW2,
-    float* __restrict__ gb2) {
-  using namespace dw;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + oBarD);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + oBarD + 8);
-  const uint32_t bar_addr = smem_u32(bar);
-  if (tid == 0) {
-    mbar_init(bar_addr, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 256;" ::"r"(smem_u32(tmem_slot)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  fence_async_smem();
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  constexpr uint64_t kStepK = (uint64_t)((2 * kPanelBytes) >> 4);
-  const uint64_t dAhi = make_desc(smem_u32(smem)), dAlo = make_desc(smem_u32(smem + kOpBytes));
-  const uint64_t dBhi = make_desc(smem_u32(smem + 2 * kOpBytes)), dBlo = make_desc(smem_u32(smem + 3 * kOpBytes));
-
-  const int64_t n_rounds = (n_pts + kK - 1) / kK;
-  const int64_t n_groups = (n_rounds + kFlush - 1) / kFlush;
-  const int64_t g_per_cta = (n_groups + gridDim.x - 1) / gridDim.x;
-  const int64_t r_begin = (int64_t)blockIdx.x * g_per_cta * kFlush, r_end = min(n_rounds, r_begin + g_per_cta * kFlush);
-  uint32_t phase = 0;
-  const uint32_t my_tmem = tmem + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(warp >> 2) * 64;
-  // warp = sample quad of the round (samples 4 warp .. 4 warp + 3 = the four K slots of panel `warp`), lane -> units j = 32 i + lane
-  float w3a[4], w3b[4], w3c[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    w3a[i] = W3[32 * i + lane]; w3b[i] = W3[kHidden + 32 * i + lane]; w3c[i] = W3[2 * kHidden + 32 * i + lane];
-  }
-  const uint32_t row_off = (uint32_t)warp * kPanelBytes + (uint32_t)lane * 16;      // + i * 512: operand row j = 32 i + lane
-  float accb[4] = {0.f, 0.f, 0.f, 0.f};
-  float* sB2 = reinterpret_cast<float*>(smem + oW3d);        // [128] db2 partials of the CTA (the W3 slot of k_shade_dw2_tc is free here)
-  if (tid < kHidden) sB2[tid] = 0.f;
-
-  uint4 pm[4];                 // masks of my four samples, chunk i
-  float ph[4][4];              // H1[s0 + t][32 i + lane]
-  float4 po[3], pg[3];         // rgb / grad_rgb of my four samples (12 floats each)
-  auto prefetch = [&](int64_t rd) {
-    const bool on = rd < r_end;
-    const int64_t tile = rd >> 2;
-    const int r_in = (int)(rd & 3) * 32 + warp * 4;                 // first of my four rows inside the tile
-    const int64_t row0 = rd * kK + warp * 4;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      pm[i] = make_uint4(0, 0, 0, 0);
-      if (on) pm[i] = __ldg(reinterpret_cast<const uint4*>(h2_mask + tile * 512 + i * 128 + r_in));
-      // H1 transposed by the forward: [tile][sample quad][unit][4 samples] -> my operand row is one 16-byte load
-      float4 h4 = make_float4(0, 0, 0, 0);
-      if (on) h4 = __ldg(reinterpret_cast<const float4*>(h1 + tile * (int64_t)(kRows * kHidden) + (int64_t)(r_in >> 2) * (kHidden * 4) + (32 * i + lane) * 4));
-      ph[i][0] = h4.x; ph[i][1] = h4.y; ph[i][2] = h4.z; ph[i][3] = h4.w;
-    }
-    if (on && row0 + 4 <= n_pts) {
-      const float4* o = reinterpret_cast<const float4*>(rgb + row0 * 3);
-      const float4* g = reinterpret_cast<const float4*>(g_rgb + row0 * 3);
-      po[0] = __ldg(o); po[1] = __ldg(o + 1); po[2] = __ldg(o + 2);
-      pg[0] = __ldg(g); pg[1] = __ldg(g + 1); pg[2] = __ldg(g + 2);
-    } else {
-      float fo[12], fg[12];
-#pragma unroll
-      for (int e = 0; e < 12; ++e) {
-        const bool ok = on && row0 * 3 + e < n_pts * 3;
-        fo[e] = ok ? rgb[row0 * 3 + e] : 0.f;
-        fg[e] = ok ? g_rgb[row0 * 3 + e] : 0.f;
-      }
-      po[0] = make_float4(fo[0], fo[1], fo[2], fo[3]); po[1] = make_float4(fo[4], fo[5], fo[6], fo[7]); po[2] = make_float4(fo[8], fo[9], fo[10], fo[11]);
-      pg[0] = make_float4(fg[0], fg[1], fg[2], fg[3]); pg[1] = make_float4(fg[4], fg[5], fg[6], fg[7]); pg[2] = make_float4(fg[8], fg[9], fg[10], fg[11]);
-    }
-  };
-  auto fold = [&](bool first) {
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-      float v[16], sum[16];
-      tmem_ld16(my_tmem + cAcc + c * 16, v);
-      if (!first) {
-        tmem_ld16(my_tmem + cSum + c * 16, sum);
-#pragma unroll
-        for (int e = 0; e < 16; ++e) v[e] = __fadd_rn(sum[e], v[e]);
-      }
-      tmem_st16(my_tmem + cSum + c * 16, v);
-    }
-    tmem_st_wait();
-  };
-  if (r_begin < r_end) prefetch(r_begin);
-  bool pending = false;
-  int n_folded = 0;
-  for (int64_t rd = r_begin; rd < r_end; ++rd) {
-    const int i_rd = (int)(rd - r_begin);
-    // dz3 of my four samples (sigmoid' folded in), in the summation order of the other kernels
-    float d0[4], d1[4], d2[4];
-    {
-      const float fo[12] = {po[0].x, po[0].y, po[0].z, po[0].w, po[1].x, po[1].y, po[1].z, po[1].w, po[2].x, po[2].y, po[2].z, po[2].w};
-      const float fg[12] = {pg[0].x, pg[0].y, pg[0].z, pg[0].w, pg[1].x, pg[1].y, pg[1].z, pg[1].w, pg[2].x, pg[2].y, pg[2].z, pg[2].w};
-#pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        d0[t] = fg[3 * t] * (fo[3 * t] * (1.f - fo[3 * t]));
-        d1[t] = fg[3 * t + 1] * (fo[3 * t + 1] * (1.f - fo[3 * t + 1]));
-        d2[t] = fg[3 * t + 2] * (fo[3 * t + 2] * (1.f - fo[3 * t + 2]));
-      }
-    }
-    if ((i_rd % kFlush) == 0 && warp == 1 && rd + kFlush < r_end && elect_one())     // next tile of H1 -> L2
-      l2_prefetch(h1 + (rd + kFlush) * (int64_t)(kK * kHidden), (uint32_t)kRows * kHidden * 4);
-    if (pending) {                          // tensor pipe must have finished reading the staging buffer
-      mbar_wait(bar_addr, phase);
-      phase ^= 1;
-    }
-    if (i_rd > 0 && (i_rd % kFlush) == 0) { // the chain of the previous kFlush rounds is complete: fold it, restart the accumulator
-      tc_fence_after();
-      fold(n_folded == 0);
-      ++n_folded;
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const uint32_t mw[4] = {pm[i].x, pm[i].y, pm[i].z, pm[i].w};
-      uint4 zh, hh;
-      float4 zl, hl;
-      uint32_t* zhp = &zh.x; uint32_t* hhp = &hh.x; float* zlp = &zl.x; float* hlp = &hl.x;
-#pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        const float z = ((mw[t] >> lane) & 1u) ? fmaf(d2[t], w3c[i], fmaf(d1[t], w3b[i], d0[t] * w3a[i])) : 0.f;
-        accb[i] += z;                                       // db2[j] = sum over samples of dZ2[s][j]: rebuilt here anyway
-        zhp[t] = tf32_hi_bits(z);
-        zlp[t] = z - __uint_as_float(zhp[t]);
-        hhp[t] = tf32_hi_bits(ph[i][t]);
-        hlp[t] = ph[i][t] - __uint_as_float(hhp[t]);
-      }
-      const uint32_t off = row_off + (uint32_t)i * 512;
-      *reinterpret_cast<uint4*>(smem + off) = zh;
-      *reinterpret_cast<float4*>(smem + kOpBytes + off) = zl;
-      *reinterpret_cast<uint4*>(smem + 2 * kOpBytes + off) = hh;
-      *reinterpret_cast<float4*>(smem + 3 * kOpBytes + off) = hl;
-    }
-    fence_async_smem();
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0 && elect_one()) {   // one elected lane of a CONVERGED warp: plain UTCHMMA issue (see elect_one)
-      tc_fence_after();
-      const bool fresh = (i_rd % kFlush) == 0;
-#pragma unroll
-      for (int ks = 0; ks < (int)(kK / 8); ++ks) {
-        mma_ss(tmem + cAcc, dAhi + ks * kStepK, dBhi + ks * kStepK, (!fresh || ks > 0) ? 1u : 0u);
-        if (kThree) {
-          mma_ss(tmem + cAcc, dAlo + ks * kStepK, dBhi + ks * kStepK, 1);
-          mma_ss(tmem + cAcc, dAhi + ks * kStepK, dBlo + ks * kStepK, 1);
+        for (int e = 0; e < 4; ++e) {
+          const float dh = dz3[0] * sW3[c + e] + dz3[1] * sW3[kHidden + c + e] + dz3[2] * sW3[2 * kHidden + c + e];
+          dv[e] = hv[e] > 0.f ? dh : 0.f;
         }
+        d = make_float4(dv[0], dv[1], dv[2], dv[3]);
       }
-      mma_commit(bar_addr);
+      *reinterpret_cast<float4*>(sA + sr * kStride + c) = d;
+      *reinterpret_cast<float4*>(sB + sr * kStride + c) = h1;
     }
-    pending = true;
-    // the next round's loads fly while the tensor pipe works on this one (a single register set: issuing them before the staging
-    // would double the live registers past the 128 a two-CTA-per-SM kernel may use)
-    prefetch(rd + 1);
-  }
-  if (pending) {
-    mbar_wait(bar_addr, phase);
-    tc_fence_after();
-    fold(n_folded == 0);
-#pragma unroll 1
-    for (int c = 0; c < 2; ++c) {
-      float v[32];
-      tmem_ld32(my_tmem + cSum + c * 32, v);
-      float* dst = gW2 + ((warp & 3) * 32 + lane) * kHidden + (warp >> 2) * 64 + c * 32;
+    __syncthreads();
+    float acc[kNT][4];
 #pragma unroll
-      for (int e = 0; e < 32; ++e) atomicAdd(dst + e, v[e]);
+    for (int j = 0; j < kNT; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
+#pragma unroll
+    for (int s = 0; s < dw::kK / 8; ++s) {
+      // A[m][k] = dZ2[sample 8 s + k][unit 16 w + m]
+      const float av[4] = {sA[(8 * s + t) * kStride + 16 * warp + g], sA[(8 * s + t) * kStride + 16 * warp + g + 8],
+                           sA[(8 * s + t + 4) * kStride + 16 * warp + g], sA[(8 * s + t + 4) * kStride + 16 * warp + g + 8]};
+      uint32_t ah[4], al[4];
+      split4(av, ah, al);
+#pragma unroll
+      for (int j = 0; j < kNT; ++j) {
+        uint32_t bh[2], bl[2];
+        tile_frag(sB, s, j, g, t, bh, bl);
+        mma3<kThree>(acc[j], ah, al, make_uint4(bh[0], bh[1], bl[0], bl[1]));
+      }
     }
+#pragma unroll
+    for (int j = 0; j < kNT; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) sum[j][e] += acc[j][e];
   }
 #pragma unroll
-  for (int i = 0; i < 4; ++i) atomicAdd(sB2 + 32 * i + lane, accb[i]);      // the eight sample-quad warps hold partials of the same units
-  tc_fence_before();
-  __syncthreads();
-  if (tid < kHidden && gb2) atomicAdd(gb2 + tid, sB2[tid]);
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 256;" ::"r"(tmem) : "memory");
+  for (int j = 0; j < kNT; ++j) {
+    const int c = 8 * j + 2 * t, m = 16 * warp + g;
+    atomicAdd(grad_W2 + m * kHidden + c, sum[j][0]);
+    atomicAdd(grad_W2 + m * kHidden + c + 1, sum[j][1]);
+    atomicAdd(grad_W2 + (m + 8) * kHidden + c, sum[j][2]);
+    atomicAdd(grad_W2 + (m + 8) * kHidden + c + 1, sum[j][3]);
+  }
 }
 
 }  // namespace tc
@@ -1871,73 +637,92 @@ __global__ void __launch_bounds__(dw::kThreadsDW, dw::kCtasPerSM) k_shade_dw2_ma
 
 using namespace ubn;
 
+namespace {
+
+template <typename K>
+int set_smem(K kernel, uint32_t bytes) {
+  return finish(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+}
+
+unsigned unit_grid(int64_t n_pts, int warps) {
+  const int64_t n_units = (n_pts + tc::kUnit - 1) / tc::kUnit;
+  return (unsigned)std::min<int64_t>(kNumSMs, (n_units + warps - 1) / warps);
+}
+
+template <bool kSave, bool kThree, int kWarps, bool kPanel>
+int launch_fwd(const float* feat, const float* vb, const int64_t* ray_id, const float* W1k, const float* W2, const float* b2,
+               const float* W3, const float* b3, int64_t n, float* rgb, float* h1, float* h2, uint32_t* m1, cudaStream_t st) {
+  auto k = tc::k_shade_fwd_tc<kSave, kThree, kWarps, kPanel>;
+  if (int e = set_smem(k, tc::kSmemFwd)) return e;
+  k<<<unit_grid(n, kWarps), 32 * kWarps, tc::kSmemFwd, st>>>(feat, vb, ray_id, W1k, W2, b2, W3, b3, n, rgb, h1, h2, m1);
+  UBN_LAUNCH_CHECK();
+  return 0;
+}
+
+template <bool kSave, bool kThree, int kWarps>
+int launch_fwd_p(bool panel, const float* feat, const float* vb, const int64_t* ray_id, const float* W1k, const float* W2,
+                 const float* b2, const float* W3, const float* b3, int64_t n, float* rgb, float* h1, float* h2, uint32_t* m1,
+                 cudaStream_t st) {
+  return panel ? launch_fwd<kSave, kThree, kWarps, true>(feat, vb, ray_id, W1k, W2, b2, W3, b3, n, rgb, h1, h2, m1, st)
+               : launch_fwd<kSave, kThree, kWarps, false>(feat, vb, ray_id, W1k, W2, b2, W3, b3, n, rgb, h1, h2, nullptr, st);
+}
+
+template <bool kThree, int kWarps, bool kPanel, bool kMask1, bool kDz1Out>
+int launch_bwd(const float* feat, const int64_t* ray_id, const float* W1k, const float* W2, const float* W3, const float* rgb,
+               const float* h1, const float* h2, const float* grad_rgb, int64_t n, float* grad_feat, float* grad_vb, float* gW1k,
+               float* gb2, float* gW3, float* gb3, uint32_t* m2, const uint32_t* m1, float* dz1, cudaStream_t st) {
+  auto k = tc::k_shade_bwd_tc<kThree, kWarps, kPanel, kMask1, kDz1Out>;
+  const uint32_t bytes = tc::bk::smem_bytes(kWarps);
+  if (int e = set_smem(k, bytes)) return e;
+  k<<<unit_grid(n, kWarps), 32 * kWarps, bytes, st>>>(feat, ray_id, W1k, W2, W3, rgb, h1, h2, grad_rgb, n, grad_feat, grad_vb, gW1k,
+                                                      gb2, gW3, gb3, m2, m1, dz1);
+  UBN_LAUNCH_CHECK();
+  return 0;
+}
+
+template <bool kThree, bool kPanel, bool kMask2>
+int launch_dw2(const float* W3, const float* rgb, const float* h1, const float* h2, const uint32_t* m2, const float* grad_rgb,
+               int64_t n, float* gW2, cudaStream_t st) {
+  auto k = tc::k_shade_dw2_tc<kThree, kPanel, kMask2>;
+  if (int e = set_smem(k, tc::dw::kSmem)) return e;
+  const int64_t n_chunks = (n + tc::dw::kK - 1) / tc::dw::kK;
+  const unsigned grid = (unsigned)std::min<int64_t>(kNumSMs, n_chunks);
+  k<<<grid, tc::dw::kThreads, tc::dw::kSmem, st>>>(W3, rgb, h1, h2, m2, grad_rgb, n, gW2);
+  UBN_LAUNCH_CHECK();
+  return 0;
+}
+
+}  // namespace
+
 extern "C" int ubn_rgbnet_fwd_tc(const float* feat, const float* view_bias, const int64_t* ray_id, const float* W1k,
                                  const float* W2, const float* b2, const float* W3, const float* b3, int64_t n_pts,
                                  float* rgb, float* h1_save, float* h2_save, uint32_t* h1_mask, int single_pass, void* stream) {
   if (n_pts <= 0) return 0;
   const bool save = h1_save != nullptr && h2_save != nullptr;
-  const int64_t n_tiles = (n_pts + tc::kRows - 1) / tc::kRows;
-  const unsigned grid = (unsigned)std::min<int64_t>(kNumSMs, n_tiles);
+  const bool one = (single_pass & 1) != 0, four = (single_pass & 2) != 0, panel = save && (single_pass & 4) != 0;
   cudaStream_t st = as_stream(stream);
-  // single_pass bit 0: one TF32 pass per product; bit 1: the 4-warp form (A/B; default = 8 warps, two column halves per row)
-#define UBN_TC_LAUNCH_H(SAVE, THREE, H, P)                                                                                \
-  do {                                                                                                                  \
-    cudaError_t e = cudaFuncSetAttribute(tc::k_shade_fwd_tc<SAVE, THREE, H, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                         (int)tc::kSmemBytes);                                                          \
-    if (e != cudaSuccess) return finish(e);                                                                             \
-    tc::k_shade_fwd_tc<SAVE, THREE, H, P><<<grid, tc::kRows * H, tc::kSmemBytes, st>>>(feat, view_bias, ray_id, W1k, W2, b2, W3, \
-                                                                                        b3, n_pts, rgb, h1_save, h2_save,    \
-                                                                                        (SAVE && P) ? h1_mask : nullptr);    \
-  } while (0)
-#define UBN_TC_LAUNCH(SAVE, THREE, P)                                \
-  do {                                                               \
-    if (four_warps) UBN_TC_LAUNCH_H(SAVE, THREE, 1, P);              \
-    else UBN_TC_LAUNCH_H(SAVE, THREE, 2, P);                         \
-  } while (0)
-  const bool four_warps = (single_pass & 2) != 0, panel = (single_pass & 4) != 0;   // bit 2: panel-layout saves (see the kernel)
-  single_pass &= 1;
-  if (save && panel) {
-    if (single_pass) UBN_TC_LAUNCH(true, false, true); else UBN_TC_LAUNCH(true, true, true);
-  } else if (save) {
-    if (single_pass) UBN_TC_LAUNCH(true, false, false); else UBN_TC_LAUNCH(true, true, false);
-  } else {
-    if (single_pass) UBN_TC_LAUNCH(false, false, false); else UBN_TC_LAUNCH(false, true, false);
+#define UBN_FWD(SAVE, THREE, W) \
+  return launch_fwd_p<SAVE, THREE, W>(panel, feat, view_bias, ray_id, W1k, W2, b2, W3, b3, n_pts, rgb, h1_save, h2_save, h1_mask, st)
+  if (save) {
+    if (one) { if (four) UBN_FWD(true, false, 4); else UBN_FWD(true, false, 8); }
+    if (four) UBN_FWD(true, true, 4); else UBN_FWD(true, true, 8);
   }
-#undef UBN_TC_LAUNCH
-#undef UBN_TC_LAUNCH_H
-  UBN_LAUNCH_CHECK();
-  return 0;
+  if (one) { if (four) UBN_FWD(false, false, 4); else UBN_FWD(false, false, 8); }
+  if (four) UBN_FWD(false, true, 4); else UBN_FWD(false, true, 8);
+#undef UBN_FWD
 }
-
 
 extern "C" int ubn_rgbnet_bwd_tc_data(const float* W2, const float* W3, const float* rgb, const float* h1_save,
                                       const float* h2_save, const float* grad_rgb, int64_t n_pts, float* dz1_out,
                                       float* grad_W2, void* stream) {
   if (n_pts <= 0) return 0;
   cudaStream_t st = as_stream(stream);
-  {   // dH1 / dZ1 (TS-MMA chain)
-    const int64_t n_tiles = (n_pts + tc::kRows - 1) / tc::kRows;
-    const unsigned grid = (unsigned)std::min<int64_t>(kNumSMs, n_tiles);
-    cudaError_t e = cudaFuncSetAttribute(tc::k_shade_bwd_tc<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)tc::bw::kSmemBytesB);
-    if (e != cudaSuccess) return finish(e);
-    tc::k_shade_bwd_tc<false><<<grid, tc::kRows, tc::bw::kSmemBytesB, st>>>(W2, W3, rgb, h1_save, h2_save, grad_rgb, n_pts,
-                                                                            dz1_out, grad_W2);
-    UBN_LAUNCH_CHECK();
-  }
-  {   // dW2 (split-K GEMM over all samples)
-    const int64_t n_rounds = (n_pts + tc::dw::kK - 1) / tc::dw::kK;
-    const unsigned grid = (unsigned)std::min<int64_t>((int64_t)kNumSMs * tc::dw::kCtasPerSM, n_rounds);
-    cudaError_t e = cudaFuncSetAttribute(tc::k_shade_dw2_tc<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)tc::dw::kSmemBytesD);
-    if (e != cudaSuccess) return finish(e);
-    tc::k_shade_dw2_tc<true, false><<<grid, tc::dw::kThreadsDW, tc::dw::kSmemBytesD, st>>>(W3, rgb, h1_save, h2_save, grad_rgb, n_pts,
-                                                                                   grad_W2);
-    UBN_LAUNCH_CHECK();
-  }
-  return 0;
+  if (int e = launch_bwd<true, 8, false, false, true>(nullptr, nullptr, nullptr, W2, W3, rgb, h1_save, h2_save, grad_rgb, n_pts,
+                                                     nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                                     dz1_out, st))
+    return e;
+  return launch_dw2<true, false, false>(W3, rgb, h1_save, h2_save, nullptr, grad_rgb, n_pts, grad_W2, st);
 }
-
 
 extern "C" int ubn_rgbnet_bwd_tc_fused(const float* feat, const int64_t* ray_id, const float* W1k, const float* W2, const float* W3,
                                        const float* rgb, const float* h1_save, const float* h2_save, const float* grad_rgb,
@@ -1946,63 +731,27 @@ extern "C" int ubn_rgbnet_bwd_tc_fused(const float* feat, const int64_t* ray_id,
                                        const uint32_t* h1_mask, int single_pass, void* stream) {
   if (n_pts <= 0) return 0;
   cudaStream_t st = as_stream(stream);
-  {   // dX + every sample reduction except dW2
-    const int64_t n_tiles = (n_pts + tc::kRows - 1) / tc::kRows;
-    const unsigned grid = (unsigned)std::min<int64_t>(kNumSMs, n_tiles);
-#define UBN_BF(T)                                                                                                              \
-    do {                                                                                                                       \
-      cudaError_t e = cudaFuncSetAttribute(tc::k_shade_bwd_fused<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,              \
-                                           (int)tc::bf::kSmemBytesF);                                                          \
-      if (e != cudaSuccess) return finish(e);                                                                                  \
-      tc::k_shade_bwd_fused<T><<<grid, tc::kRows, tc::bf::kSmemBytesF, st>>>(feat, ray_id, W1k, W2, W3, rgb, h1_save, h2_save, grad_rgb, \
-                                                                             n_pts, grad_feat, grad_view_bias, grad_W1k, grad_b2,       \
-                                                                             grad_W3, grad_b3);                                         \
-    } while (0)
-#define UBN_BFW(T, P, M1)                                                                                                      \
-    do {                                                                                                                       \
-      cudaError_t e = cudaFuncSetAttribute(tc::k_shade_bwd_fused_ws<T, P, M1>, cudaFuncAttributeMaxDynamicSharedMemorySize,    \
-                                           (int)tc::bf2::kSmemBytesF2);                                                        \
-      if (e != cudaSuccess) return finish(e);                                                                                  \
-      tc::k_shade_bwd_fused_ws<T, P, M1><<<grid, 2 * tc::kRows, tc::bf2::kSmemBytesF2, st>>>(                                  \
-          feat, ray_id, W1k, W2, W3, rgb, h1_save, h2_save, grad_rgb, n_pts, grad_feat, grad_view_bias, grad_W1k, grad_b2, grad_W3,   \
-          grad_b3, (P) ? h2_mask_scratch : nullptr, h1_mask);                                                                  \
-    } while (0)
-    const bool one_pass = (single_pass & 1) != 0, plain = (single_pass & 2) != 0, panel = (single_pass & 4) != 0;
-    if (plain && panel) return finish(cudaErrorInvalidValue);       // the 4-warp A/B kernel reads row-major saves only
-    if (plain)      { if (one_pass) UBN_BF(false); else UBN_BF(true); }
-    else if (panel && h1_mask && h2_mask_scratch) { if (one_pass) UBN_BFW(false, true, true); else UBN_BFW(true, true, true); }
-    else if (panel)            { if (one_pass) UBN_BFW(false, true, false); else UBN_BFW(true, true, false); }
-    else                       { if (one_pass) UBN_BFW(false, false, false); else UBN_BFW(true, false, false); }
-#undef UBN_BFW
-#undef UBN_BF
-    UBN_LAUNCH_CHECK();
-  }
-  {   // dW2 (split-K GEMM over all samples)
-    const int64_t n_rounds = (n_pts + tc::dw::kK - 1) / tc::dw::kK;
-    const unsigned grid = (unsigned)std::min<int64_t>((int64_t)kNumSMs * tc::dw::kCtasPerSM, n_rounds);
-#define UBN_DW(T, P)                                                                                                           \
-    do {                                                                                                                       \
-      cudaError_t e = cudaFuncSetAttribute(tc::k_shade_dw2_tc<T, P>, cudaFuncAttributeMaxDynamicSharedMemorySize,              \
-                                           (int)tc::dw::kSmemBytesD);                                                          \
-      if (e != cudaSuccess) return finish(e);                                                                                  \
-      tc::k_shade_dw2_tc<T, P><<<grid, tc::dw::kThreadsDW, tc::dw::kSmemBytesD, st>>>(W3, rgb, h1_save, h2_save, grad_rgb, n_pts, grad_W2); \
-    } while (0)
-#define UBN_DWM(T)                                                                                                             \
-    do {                                                                                                                       \
-      cudaError_t e = cudaFuncSetAttribute(tc::k_shade_dw2_mask_tc<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,            \
-                                           (int)tc::dw::kSmemBytesD);                                                          \
-      if (e != cudaSuccess) return finish(e);                                                                                  \
-      tc::k_shade_dw2_mask_tc<T><<<grid, tc::dw::kThreadsDW, tc::dw::kSmemBytesD, st>>>(W3, rgb, h1_save, h2_mask_scratch, grad_rgb, n_pts, \
-                                                                                      grad_W2, grad_b2);                       \
-    } while (0)
-    // panel saves + warp-specialised first launch + a mask scratch: dZ2 rebuilt from the ReLU masks (H2 is not read again)
-    const bool from_masks = (single_pass & 4) && !(single_pass & 2) && h2_mask_scratch != nullptr && h1_mask != nullptr;
-    if (from_masks)           { if (single_pass & 1) UBN_DWM(false); else UBN_DWM(true); }
-    else if (single_pass & 4) { if (single_pass & 1) UBN_DW(false, true); else UBN_DW(true, true); }
-    else                      { if (single_pass & 1) UBN_DW(false, false); else UBN_DW(true, false); }
-#undef UBN_DWM
+  const bool one = (single_pass & 1) != 0, four = (single_pass & 2) != 0, panel = (single_pass & 4) != 0;
+  const bool mask1 = panel && h1_mask != nullptr, mask2 = panel && h2_mask_scratch != nullptr;
+  uint32_t* m2 = mask2 ? h2_mask_scratch : nullptr;
+  int e = 0;
+#define UBN_BWD(THREE, W, P, M1)                                                                                              \
+  e = launch_bwd<THREE, W, P, M1, false>(feat, ray_id, W1k, W2, W3, rgb, h1_save, h2_save, grad_rgb, n_pts, grad_feat,        \
+                                         grad_view_bias, grad_W1k, grad_b2, grad_W3, grad_b3, m2, h1_mask, nullptr, st)
+#define UBN_BWD_W(THREE, P, M1) \
+  do { if (four) UBN_BWD(THREE, 4, P, M1); else UBN_BWD(THREE, 8, P, M1); } while (0)
+#define UBN_BWD_T(P, M1) \
+  do { if (one) UBN_BWD_W(false, P, M1); else UBN_BWD_W(true, P, M1); } while (0)
+  if (mask1) UBN_BWD_T(true, true);
+  else if (panel) UBN_BWD_T(true, false);
+  else UBN_BWD_T(false, false);
+#undef UBN_BWD_T
+#undef UBN_BWD_W
+#undef UBN_BWD
+  if (e) return e;
+#define UBN_DW(THREE, P, M2) return launch_dw2<THREE, P, M2>(W3, rgb, h1_save, h2_save, m2, grad_rgb, n_pts, grad_W2, st)
+  if (mask2) { if (one) UBN_DW(false, true, true); else UBN_DW(true, true, true); }
+  if (panel) { if (one) UBN_DW(false, true, false); else UBN_DW(true, true, false); }
+  if (one) UBN_DW(false, false, false); else UBN_DW(true, false, false);
 #undef UBN_DW
-    UBN_LAUNCH_CHECK();
-  }
-  return 0;
 }

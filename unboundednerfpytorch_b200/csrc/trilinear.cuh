@@ -52,9 +52,8 @@ __device__ __forceinline__ float src_index(float coord, int size) {
   return __fmul_rn(__fmul_rn(__fadd_rn(coord, 1.f), 0.5f), (float)(size - 1));
 }
 
-// Mean over the P slabs exactly as torch-CUDA evaluates `out.mean(0)` on the grid_sample output (FourierGrid_grid.py:72), probed
-// on B200 (scripts/probe_mean_order.py: 0 mismatches in 4 M elements for P = 3..11; the sequential and the pairwise-tree orders
-// mismatch in ~58 %): ATen's reduction keeps four interleaved accumulators a[i & 3] += x_i, combines them ((a0 + a1) + a2) + a3
+// Mean over the P slabs exactly as torch-CUDA evaluates `out.mean(0)` on the grid_sample output (FourierGrid_grid.py:72), as
+// probed with scripts/probe_mean_order.py (the sequential and the pairwise-tree orders do not match): ATen's reduction keeps four interleaved accumulators a[i & 3] += x_i, combines them ((a0 + a1) + a2) + a3
 // and multiplies by the fp32 reciprocal of P.  Matching it makes raw_density -- and with it alpha, the weights and every
 // threshold decision downstream -- bit-identical to the reference's GPU path (alpha = 1 - (1+e)^-interval is ill-conditioned:
 // one ulp of density can move a dense-mode alpha by 1e-3 of its value).

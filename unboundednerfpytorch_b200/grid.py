@@ -1,4 +1,4 @@
-"""Voxel-grid modules with the reference's class / method surface, backed by the sm_100a kernels.
+"""Voxel-grid modules with the reference's class / method surface, backed by the sm_90a kernels.
 
 * ``DenseGrid``   -- FourierGrid/grid.py:41-84  (trilinear read = F.grid_sample there, grid.py:57)
 * ``FourierGrid`` -- FourierGrid/FourierGrid_grid.py:42-101 (P = 1+2F slabs sampled at gamma_n(x), mean)

@@ -28,8 +28,8 @@ def render_rays(model, rays_o, rays_d, viewdirs, render_kwargs, chunk=8192, keys
     rk = dict(render_kwargs)
     rk.setdefault('render_depth', True)
     # render_kwargs['coherent_rays']=True routes DenseGrid feature reads of image-ordered chunks through the TMA-staged brick
-    # kernel (csrc/render_tma.cu).  Opt-in: on the garden frame it measured 311.6 ms/frame against 271.7 ms for the
-    # lane-per-sample gather (profiles/README.md, round 2), so the gather stays the default.
+    # kernel (csrc/render_tma.cu).  Opt-in: the lane-per-sample gather stays the default (the TMA kernel was slower on a full
+    # garden frame when it was last compared; not re-measured on the H100).
     rk.setdefault('coherent_rays', False)
     outs = {k: [] for k in keys}
     for ro, rd, vd in zip(rays_o.split(chunk, 0), rays_d.split(chunk, 0), viewdirs.split(chunk, 0)):

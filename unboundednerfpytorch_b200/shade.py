@@ -13,14 +13,13 @@ import os
 from . import _cabi, ops
 from ._cabi import c_i64, c_int, check, ptr, stream_of
 
-# engine: 'tc3' = tcgen05 3xTF32 (fp32-grade, the default and the only mode the 1e-5 parity tests accept), 'tc1' = tcgen05 with a
+# engine: 'tc3' = tensor-core (mma.sync) 3xTF32 (fp32-grade, the default and the only mode the 1e-5 parity tests accept), 'tc1' = tensor cores with a
 # single TF32 pass per product in the forward AND (with BWD_MODE 'fused') the backward -- the opt-in reduced-precision training
 # mode, ~1e-3 relative error, gated by the PSNR test in tests/test_gpu_models.py --, 'simt' = fp32 FFMA
 MODE = os.environ.get('UBN_RGBNET_MODE', 'tc3')
-# backward engine: 'fused' = tcgen05 3xTF32, dZ2 -> dH1 -> dZ1 -> dX chained through tensor memory + all sample reductions in one
-# warp-specialised kernel (4 row warps drive the tensor cores, 4 column warps reduce over samples), dW2 in a second launch; no
-# intermediate in HBM; 'fused4' = the same without warp specialisation (A/B); 'tc3' = the previous three-launch form (dZ1 round trip + CUDA-core kernel for
-# the small gradients; kept for A/B); 'simt' = fp32 FFMA
+# backward engine: 'fused' = tensor-core 3xTF32, dZ2 -> dH1 -> dZ1 -> dX chained through registers + all sample reductions in one
+# kernel of 8 warps, dW2 in a second launch; no intermediate in HBM; 'fused4' = the same with 4 warps per CTA (A/B); 'tc3' = the
+# three-launch form (dZ1 round trip + CUDA-core kernel for the small gradients; kept for A/B); 'simt' = fp32 FFMA
 BWD_MODE = os.environ.get('UBN_RGBNET_BWD_MODE', 'fused')
 # ReLU masks instead of activation re-reads in the fused backward (default on): the forward leaves the masks of H1 (16 B per sample)
 # so that launch 1 gates dH1 without loading the H1 rows; launch 1 ballots the masks of H2 so that the dW2 launch rebuilds dZ2 (and
@@ -40,8 +39,8 @@ class _ShadeFn(torch.autograd.Function):
         # mirrors requires_grad of the inputs even under torch.no_grad() -- render / eval forwards must not allocate and stream
         # the two [M,128] activation saves
         need_grad = bool(need_grad) and any(ctx.needs_input_grad)
-        # panel-layout saves ([tile][32 column quads][128 rows][4], ceil(M/128)*128 rows): coalesced for the row-per-thread kernels
-        # on both sides; only the tcgen05 forward writes it and only the warp-specialised backward (+ dW2) reads it
+        # panel-layout saves ([tile][32 column quads][128 rows][4], ceil(M/128)*128 rows): every 8-sample x 16-byte piece of a
+        # tensor-core fragment is one contiguous 128-byte line; only the tensor-core forward writes it and only the fused backward reads it
         panel = need_grad and MODE in ('tc3', 'tc1', 'tc3w4') and BWD_MODE == 'fused'
         rows = -(-M // 128) * 128 if panel else M
         h1 = torch.empty(rows, 128, dtype=torch.float32, device=dev) if need_grad else None
@@ -78,7 +77,7 @@ class _ShadeFn(torch.autograd.Function):
         g_vb, gW1k, gW2, gb2, gW3, gb3 = z(ctx.n_rays, 128), z(128, 12), z(128, 128), z(128), z(3, 128), z(3)
         with ops._Guard(feat) as lib:
             bwd_mode = ctx.bwd_mode                      # as chosen in forward (the save layout depends on it)
-            if bwd_mode in ('fused', 'fused4'):          # 'fused4': the same kernel without warp specialisation (A/B)
+            if bwd_mode in ('fused', 'fused4'):          # 'fused4': the same kernels with 4 warps per CTA (A/B)
                 # panel saves: launch 1 leaves the ReLU masks of H2 (2 KB per 128-sample tile) in this scratch and the dW2 launch
                 # rebuilds dZ2 from them instead of reading the 512 B/sample of H2 again
                 masks = torch.empty(-(-M // 128) * 512, dtype=torch.int32, device=dev) if (ctx.panel and ctx.m1 is not None) else None
