@@ -360,6 +360,55 @@ int ubn_march_density_bwd(const float* rays_o, const float* rays_d, const float*
                           const float* g_weight, const float* g_alpha, const float* g_density,
                           const float* g_last, float* grad_density_grid, void* stream);
 
+/* ---- fused NDC ray march for the forward-facing model DirectMPIGO.forward (FourierGrid/dmpigo.py:224-340):
+ *      sample_ndc_pts_on_rays + bbox drop + mask cache + (density + act_shift) + Raw2Alpha(shift 0) + Alphas2Weights + both
+ *      thresholds + k0 query.  Same three-launch forward (pass A, ubn_exclusive_scan_i32, pass B) and two-launch backward as the
+ *      contracted march above, the same per-sample records and flag bits (UBN_FLAG_INNER is never set). ------------------- */
+typedef struct UbnNdcMarchCfg {
+  /* sample i of S: p = o + d * (i / (S-1)) exactly as render_utils_kernel.cu:260-263; S = int((mpi_depth-1)/stepsize)+1
+   * (dmpigo.py:239); samples with p outside [xyz_min, xyz_max] (strict comparisons) are dropped (dmpigo.py:242-243) */
+  float xyz_min[3];
+  float xyz_max[3];
+  int32_t n_samples;
+  float interval;               /* stepsize * voxel_size_ratio (dmpigo.py:265) */
+  float fast_color_thres;       /* <= 0: no thresholding */
+  int32_t use_maskcache;        /* dmpigo.py:268-272 */
+  int32_t mask_sz[3];
+  float mask_scale[3];
+  float mask_shift[3];
+} UbnNdcMarchCfg;
+
+/* Pass A: density = density_grid(p) + act_shift_grid(p) (dmpigo.py:275; one fp32 add), alpha = Raw2Alpha(density, 0, interval)
+ * (:276), the exact sequential transmittance scan and both thresholds (:277-292).  density_grid: single-slab C = 1 grid;
+ * act_shift_grid: the [1,1,1,1,mpi_depth] DenseGrid of dmpigo.py:47-57 (any C = 1 single-slab grid).  Outputs as
+ * ubn_march_density_fwd; `density` receives the biased density. */
+int ubn_march_ndc_density_fwd(const float* rays_o, const float* rays_d, const float* density_grid,
+                              const UbnGridDesc* density_desc, const float* act_shift_grid, const UbnGridDesc* act_shift_desc,
+                              const uint8_t* mask_world, const UbnNdcMarchCfg* cfg, int64_t n_rays, float* density,
+                              float* alpha, float* weight, float* T, uint8_t* flags, float* alphainv_last, int32_t* n_keep,
+                              void* stream);
+
+/* Pass B: for every survivor, in (ray, step) order at offsets[ray] + rank, the k0 read (dmpigo.py:295, F.grid_sample arithmetic,
+ * bit-identical) and the compacted records alpha, weight, ray_id, step_id (:321-327).  k0: single-slab channels-last grid with
+ * C = 3 (rgbnet_dim = 0) or C = 9 (LLFF, rgbnet_dim = 9); out_alpha / out_weight may be NULL. */
+int ubn_march_ndc_feature_fwd(const float* rays_o, const float* rays_d, const float* k0_grid, const UbnGridDesc* k0_desc,
+                              const UbnNdcMarchCfg* cfg, int64_t n_rays, const uint8_t* flags, const int64_t* offsets,
+                              const float* alpha, const float* weight, float* k0_feat, float* out_alpha, float* out_weight,
+                              int64_t* ray_id, int64_t* step_id, void* stream);
+
+/* Backward of pass B: grad_k0 += adjoint of the k0 read applied to grad_feat[M,C] (grid_sampler_3d_backward wrt the grid). */
+int ubn_march_ndc_feature_bwd(const float* rays_o, const float* rays_d, const UbnGridDesc* k0_desc, const UbnNdcMarchCfg* cfg,
+                              int64_t n_rays, const uint8_t* flags, const int64_t* offsets, const float* grad_feat,
+                              float* grad_k0, void* stream);
+
+/* Backward of pass A: exact reverse scan (alpha2weight_backward) -> raw2alpha_backward -> scatter into the density-grid gradient.
+ * act_shift gets no gradient (requires_grad = False, dmpigo.py:50). */
+int ubn_march_ndc_density_bwd(const float* rays_o, const float* rays_d, const UbnGridDesc* density_desc,
+                              const UbnNdcMarchCfg* cfg, int64_t n_rays, const float* density, const float* alpha,
+                              const float* weight, const float* T, const uint8_t* flags, const float* alphainv_last,
+                              const int64_t* offsets, const float* g_weight, const float* g_alpha, const float* g_last,
+                              float* grad_density_grid, void* stream);
+
 /* ---- rgbnet: rgb = sigmoid(rgbnet(cat[k0_feat, viewdirs_emb[ray_id]])) (FourierGrid_model.py:231-242,631-637;
  *      dcvgo.py:103-114,337-342) for the 3-layer, width-128, 12-feature configuration every shipped config uses.
  * The per-ray part of layer 1 is hoisted by the host: view_bias[n_rays,128] = emb(viewdirs) . W1[:,12:]^T + b1, so the

@@ -34,6 +34,11 @@ class UbnMarchCfg(ctypes.Structure):
                 ('use_maskcache', c_i32), ('mask_sz', c_i32 * 3), ('mask_scale', c_f * 3), ('mask_shift', c_f * 3)]
 
 
+class UbnNdcMarchCfg(ctypes.Structure):
+    _fields_ = [('xyz_min', c_f * 3), ('xyz_max', c_f * 3), ('n_samples', c_i32), ('interval', c_f), ('fast_color_thres', c_f),
+                ('use_maskcache', c_i32), ('mask_sz', c_i32 * 3), ('mask_scale', c_f * 3), ('mask_shift', c_f * 3)]
+
+
 ABI_VERSION = 3          # UBN_ABI_VERSION of include/ubnerf_b200.h this binding was written against
 FLAG_QUERIED, FLAG_LISTED, FLAG_SCANNED, FLAG_KEEP, FLAG_INNER = 1, 2, 4, 8, 16
 
@@ -100,6 +105,14 @@ _SIGNATURES = {
                               c_p, c_p, c_p, c_p, c_p],
     'ubn_march_density_bwd': [c_p, c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnMarchCfg), c_i64,
                               c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
+    'ubn_march_ndc_density_fwd': [c_p, c_p, c_p, ctypes.POINTER(UbnGridDesc), c_p, ctypes.POINTER(UbnGridDesc), c_p,
+                                  ctypes.POINTER(UbnNdcMarchCfg), c_i64, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
+    'ubn_march_ndc_feature_fwd': [c_p, c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnNdcMarchCfg), c_i64,
+                                  c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
+    'ubn_march_ndc_feature_bwd': [c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnNdcMarchCfg), c_i64,
+                                  c_p, c_p, c_p, c_p, c_p],
+    'ubn_march_ndc_density_bwd': [c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnNdcMarchCfg), c_i64,
+                                  c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
 }
 _RESTYPE = {'ubn_last_error_string': ctypes.c_char_p, 'ubn_launch_count': c_i64, 'ubn_reset_launch_count': None}
 

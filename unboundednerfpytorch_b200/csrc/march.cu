@@ -29,8 +29,9 @@ __device__ __forceinline__ float grid_density(const GridView& g, float x, float 
 // ------------------------------------------------------------------------------------------------
 // pass A forward
 // ------------------------------------------------------------------------------------------------
-// kP > 0: compile-time slab count + contiguous single-channel grid -> grid_density_fast (march_common.cuh); kP = 0: generic layout
-template <int kP>
+// kP > 0: compile-time slab count + contiguous single-channel grid -> grid_density_fast (march_common.cuh); kP = 0: generic layout.
+// Smp: the sampling policy (ContractedSampler / NdcSampler, march_common.cuh).
+template <class Smp, int kP>
 __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_fwd(
     const float* __restrict__ rays_o, const float* __restrict__ rays_d, const float* __restrict__ t_table,
     GridView g, const uint8_t* __restrict__ mask_world, MarchParams p, int64_t n_rays,
@@ -40,7 +41,7 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_fwd(
   const int lane = threadIdx.x & 31;
   const int64_t ray = (int64_t)blockIdx.x * kMarchWarps + (threadIdx.x >> 5);
   if (ray >= n_rays) return;
-  const Ray r = load_ray(rays_o + 3 * ray, rays_d + 3 * ray, p);
+  const Ray r = Smp::load(rays_o + 3 * ray, rays_d + 3 * ray, p);
   const int S = p.S;
 
   float T_cum = 1.f;      // warp-uniform
@@ -53,16 +54,17 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_fwd(
     const int s = base + lane;
     const bool valid = s < S;
     float x = 0, y = 0, z = 0;
-    bool inner = false;
-    if (valid) inner = sample_point(r, t_table[s], p, x, y, z);
+    bool inner = false, in_domain = false;
+    if (valid) in_domain = Smp::point(r, t_table, s, p, x, y, z, inner);
 
-    bool queried = valid;
+    bool queried = valid && in_domain;
     if (p.use_cumdist) {
       // dist[s] = || pts[s+1] - pts[s] || (torch .norm), s <= S-2; mask[s+1] |= cumdist(dist)[s]
       float dist = 0.f;
       if (s + 1 < S) {
         float x1, y1, z1;
-        sample_point(r, t_table[s + 1], p, x1, y1, z1);
+        bool inner1;
+        Smp::point(r, t_table, s + 1, p, x1, y1, z1, inner1);
         const float ex = __fsub_rn(x1, x), ey = __fsub_rn(y1, y), ez = __fsub_rn(z1, z);
         dist = norm3_torch(ex, ey, ez);
       }
@@ -94,6 +96,7 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_fwd(
     float dens = 0.f, alpha = 0.f;
     if (queried) {
       dens = kP > 0 ? grid_density_fast<(kP > 0 ? kP : 1)>(g, x, y, z) : grid_density(g, x, y, z);
+      dens = Smp::density(p, dens, x, y, z);
       const float e = expf(dens + p.shift);
       alpha = 1 - powf(1 + e, -p.interval);
     }
@@ -244,7 +247,7 @@ constexpr int kMaxChunks = 128;   // S <= 4096
 // samples that stay in the cell -- a large share of the steps in slab 0 and the lowest sin / cos slabs at half-voxel spacing -- are added in
 // registers, and a cell leaves as four pair reductions only when the ray moves on.  The scatter is bound by the count of L2
 // reduction requests (profiled: the L2 reduction path saturates while issue stays low), so fewer requests is the only lever.
-template <int kP, bool kRuns>
+template <class Smp, int kP, bool kRuns>
 __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_bwd(
     const float* __restrict__ rays_o, const float* __restrict__ rays_d, const float* __restrict__ t_table,
     GridView g /* data = grad grid */, MarchParams p, int64_t n_rays, const float* __restrict__ density,
@@ -258,7 +261,7 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_bwd(
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int64_t ray = (int64_t)blockIdx.x * kMarchWarps + w;
   if (ray >= n_rays) return;
-  const Ray r = load_ray(rays_o + 3 * ray, rays_d + 3 * ray, p);
+  const Ray r = Smp::load(rays_o + 3 * ray, rays_d + 3 * ray, p);
   const int S = p.S;
   const int n_chunks = (S + 31) / 32;
   const int L = n_chunks;                                  // kRuns: consecutive samples per lane in phase 2 (= ceil(S / 32))
@@ -330,7 +333,8 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_bwd(
     if (gd == 0.f) continue;
     // scatter into the density grid gradient (adjoint of grid_density)
     float x, y, z;
-    sample_point(r, t_table[s], p, x, y, z);
+    bool inner;
+    Smp::point(r, t_table, s, p, x, y, z, inner);
     const float nx = norm_coord(x, g.mn[0], g.len[0]);
     const float ny = norm_coord(y, g.mn[1], g.len[1]);
     const float nz = norm_coord(z, g.mn[2], g.len[2]);
@@ -398,7 +402,8 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_bwd(
       const float gd = s_gd[s + lane];
       if (gd == 0.f) continue;
       float x, y, z;
-      sample_point(r, t_table[s], p, x, y, z);
+      bool inner;
+      Smp::point(r, t_table, s, p, x, y, z, inner);
       const float nx = norm_coord(x, g.mn[0], g.len[0]);
       const float ny = norm_coord(y, g.mn[1], g.len[1]);
       const float nz = norm_coord(z, g.mn[2], g.len[2]);
@@ -445,6 +450,59 @@ static bool feature_grid_ok(const GridView& g) {
          ((uintptr_t)g.data & 15) == 0 && (g.sp % 4) == 0;
 }
 
+template <class Smp>
+static int launch_density_fwd(const float* rays_o, const float* rays_d, const float* t_table, const GridView& g,
+                              const uint8_t* mask_world, const MarchParams& p, int64_t n_rays, float* density, float* alpha,
+                              float* weight, float* T, uint8_t* flags, float* alphainv_last, int32_t* n_keep, cudaStream_t st) {
+#define UBN_DFWD(P)                                                                                              \
+  k_march_density_fwd<Smp, P><<<blocks_for(n_rays, kMarchWarps), 32 * kMarchWarps, 0, st>>>(                   \
+      rays_o, rays_d, t_table, g, mask_world, p, n_rays, density, alpha, weight, T, flags, alphainv_last, n_keep)
+  switch (density_fast_slabs(g)) {
+    case 1: UBN_DFWD(1); break;
+    case 3: UBN_DFWD(3); break;
+    case 5: UBN_DFWD(5); break;
+    case 7: UBN_DFWD(7); break;
+    case 9: UBN_DFWD(9); break;
+    default: UBN_DFWD(0); break;
+  }
+#undef UBN_DFWD
+  UBN_LAUNCH_CHECK();
+  return 0;
+}
+
+template <class Smp>
+static int launch_density_bwd(const float* rays_o, const float* rays_d, const float* t_table, const GridView& g,
+                              const MarchParams& p, int64_t n_rays, const float* density, const float* alpha, const float* weight,
+                              const float* T, const uint8_t* flags, const float* alphainv_last, const int64_t* offsets,
+                              const float* g_weight, const float* g_alpha, const float* g_density, const float* g_last,
+                              float* grad_density_grid, cudaStream_t st) {
+  // run-merging scatter (two-phase kernel) by default; ubn_set_density_scatter(0) selects the per-sample scatter (A/B, tests)
+  const size_t smem_runs = sizeof(float) * kMarchWarps * (size_t)(p.S + 33);
+  const bool runs = get_density_scatter() == 1 && smem_runs <= 40 * 1024;
+#define UBN_DBWD(P)                                                                                                  \
+  do {                                                                                                               \
+    if (runs && (P) > 0)                                                                                             \
+      k_march_density_bwd<Smp, P, true><<<blocks_for(n_rays, kMarchWarps), 32 * kMarchWarps, smem_runs, st>>>(     \
+          rays_o, rays_d, t_table, g, p, n_rays, density, alpha, weight, T, flags, alphainv_last, offsets, g_weight,  \
+          g_alpha, g_density, g_last, grad_density_grid);                                                            \
+    else                                                                                                             \
+      k_march_density_bwd<Smp, P, false><<<blocks_for(n_rays, kMarchWarps), 32 * kMarchWarps, 0, st>>>(            \
+          rays_o, rays_d, t_table, g, p, n_rays, density, alpha, weight, T, flags, alphainv_last, offsets, g_weight,  \
+          g_alpha, g_density, g_last, grad_density_grid);                                                            \
+  } while (0)
+  switch (density_fast_slabs(g)) {
+    case 1: UBN_DBWD(1); break;
+    case 3: UBN_DBWD(3); break;
+    case 5: UBN_DBWD(5); break;
+    case 7: UBN_DBWD(7); break;
+    case 9: UBN_DBWD(9); break;
+    default: UBN_DBWD(0); break;
+  }
+#undef UBN_DBWD
+  UBN_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace ubn
 
 using namespace ubn;
@@ -474,20 +532,8 @@ int ubn_march_density_fwd(const float* rays_o, const float* rays_d, const float*
   if (g.C != 1) return finish(cudaErrorInvalidValue);
   const MarchParams p = make_params(cfg);
   if (p.use_mask && !mask_world) return finish(cudaErrorInvalidValue);
-#define UBN_DFWD(P)                                                                                              \
-  k_march_density_fwd<P><<<blocks_for(n_rays, kMarchWarps), 32 * kMarchWarps, 0, as_stream(stream)>>>(           \
-      rays_o, rays_d, t_table, g, mask_world, p, n_rays, density, alpha, weight, T, flags, alphainv_last, n_keep)
-  switch (density_fast_slabs(g)) {
-    case 1: UBN_DFWD(1); break;
-    case 3: UBN_DFWD(3); break;
-    case 5: UBN_DFWD(5); break;
-    case 7: UBN_DFWD(7); break;
-    case 9: UBN_DFWD(9); break;
-    default: UBN_DFWD(0); break;
-  }
-#undef UBN_DFWD
-  UBN_LAUNCH_CHECK();
-  return 0;
+  return launch_density_fwd<ContractedSampler>(rays_o, rays_d, t_table, g, mask_world, p, n_rays, density, alpha, weight, T,
+                                               flags, alphainv_last, n_keep, as_stream(stream));
 }
 
 int ubn_march_feature_fwd(const float* rays_o, const float* rays_d, const float* t_table, const float* k0_grid,
@@ -545,31 +591,39 @@ int ubn_march_density_bwd(const float* rays_o, const float* rays_d, const float*
   if (g.C != 1) return finish(cudaErrorInvalidValue);
   const MarchParams p = make_params(cfg);
   if (p.S > 32 * kMaxChunks) return finish(cudaErrorInvalidValue);
-  // run-merging scatter (two-phase kernel) by default; ubn_set_density_scatter(0) selects the per-sample scatter (A/B, tests)
-  const size_t smem_runs = sizeof(float) * kMarchWarps * (size_t)(p.S + 33);
-  const bool runs = get_density_scatter() == 1 && smem_runs <= 40 * 1024;
-#define UBN_DBWD(P)                                                                                                  \
-  do {                                                                                                               \
-    if (runs && (P) > 0)                                                                                             \
-      k_march_density_bwd<P, true><<<blocks_for(n_rays, kMarchWarps), 32 * kMarchWarps, smem_runs, as_stream(stream)>>>( \
-          rays_o, rays_d, t_table, g, p, n_rays, density, alpha, weight, T, flags, alphainv_last, offsets, g_weight,  \
-          g_alpha, g_density, g_last, grad_density_grid);                                                            \
-    else                                                                                                             \
-      k_march_density_bwd<P, false><<<blocks_for(n_rays, kMarchWarps), 32 * kMarchWarps, 0, as_stream(stream)>>>(    \
-          rays_o, rays_d, t_table, g, p, n_rays, density, alpha, weight, T, flags, alphainv_last, offsets, g_weight,  \
-          g_alpha, g_density, g_last, grad_density_grid);                                                            \
-  } while (0)
-  switch (density_fast_slabs(g)) {
-    case 1: UBN_DBWD(1); break;
-    case 3: UBN_DBWD(3); break;
-    case 5: UBN_DBWD(5); break;
-    case 7: UBN_DBWD(7); break;
-    case 9: UBN_DBWD(9); break;
-    default: UBN_DBWD(0); break;
-  }
-#undef UBN_DBWD
-  UBN_LAUNCH_CHECK();
-  return 0;
+  return launch_density_bwd<ContractedSampler>(rays_o, rays_d, t_table, g, p, n_rays, density, alpha, weight, T, flags,
+                                               alphainv_last, offsets, g_weight, g_alpha, g_density, g_last, grad_density_grid,
+                                               as_stream(stream));
+}
+
+int ubn_march_ndc_density_fwd(const float* rays_o, const float* rays_d, const float* density_grid,
+                              const UbnGridDesc* density_desc, const float* act_shift_grid, const UbnGridDesc* act_shift_desc,
+                              const uint8_t* mask_world, const UbnNdcMarchCfg* cfg, int64_t n_rays, float* density,
+                              float* alpha, float* weight, float* T, uint8_t* flags, float* alphainv_last, int32_t* n_keep,
+                              void* stream) {
+  if (n_rays <= 0) return 0;
+  const GridView g = make_view(density_grid, density_desc);
+  const GridView sg = make_view(act_shift_grid, act_shift_desc);
+  if (g.C != 1 || g.P != 1 || sg.C != 1 || sg.P != 1 || cfg->n_samples < 2) return finish(cudaErrorInvalidValue);
+  const MarchParams p = make_ndc_params(cfg, sg);
+  if (p.use_mask && !mask_world) return finish(cudaErrorInvalidValue);
+  return launch_density_fwd<NdcSampler>(rays_o, rays_d, nullptr, g, mask_world, p, n_rays, density, alpha, weight, T, flags,
+                                         alphainv_last, n_keep, as_stream(stream));
+}
+
+int ubn_march_ndc_density_bwd(const float* rays_o, const float* rays_d, const UbnGridDesc* density_desc,
+                              const UbnNdcMarchCfg* cfg, int64_t n_rays, const float* density, const float* alpha,
+                              const float* weight, const float* T, const uint8_t* flags, const float* alphainv_last,
+                              const int64_t* offsets, const float* g_weight, const float* g_alpha, const float* g_last,
+                              float* grad_density_grid, void* stream) {
+  if (n_rays <= 0) return 0;
+  const GridView g = make_view(grad_density_grid, density_desc);
+  if (g.C != 1 || g.P != 1 || cfg->n_samples < 2) return finish(cudaErrorInvalidValue);
+  GridView none{};
+  const MarchParams p = make_ndc_params(cfg, none);
+  if (p.S > 32 * kMaxChunks) return finish(cudaErrorInvalidValue);
+  return launch_density_bwd<NdcSampler>(rays_o, rays_d, nullptr, g, p, n_rays, density, alpha, weight, T, flags, alphainv_last,
+                                         offsets, g_weight, g_alpha, nullptr, g_last, grad_density_grid, as_stream(stream));
 }
 
 }  // extern "C"

@@ -15,10 +15,12 @@ struct MarchParams {
   int use_mask;
   int msz[3];
   float mscale[3], mshift[3];
+  float bmin[3], bmax[3];         // NDC march: samples outside this box (strict comparisons) are dropped
+  GridView shift_grid;            // NDC march: the act_shift DenseGrid, added to the raw density
 };
 
 inline MarchParams make_params(const UbnMarchCfg* c) {
-  MarchParams p;
+  MarchParams p{};
   p.cx = c->scene_center[0]; p.cy = c->scene_center[1]; p.cz = c->scene_center[2];
   p.rx = c->scene_radius[0]; p.ry = c->scene_radius[1]; p.rz = c->scene_radius[2];
   p.B = c->contract_B; p.A = c->contract_A;
@@ -28,6 +30,21 @@ inline MarchParams make_params(const UbnMarchCfg* c) {
   p.use_cumdist = c->use_cumdist; p.cumdist_thres = c->cumdist_thres;
   p.use_mask = c->use_maskcache;
   for (int a = 0; a < 3; ++a) { p.msz[a] = c->mask_sz[a]; p.mscale[a] = c->mask_scale[a]; p.mshift[a] = c->mask_shift[a]; }
+  return p;
+}
+
+// DirectMPIGO (dmpigo.py:224-340): no contraction, no cumdist, Raw2Alpha with shift 0 (the per-plane bias is in the density)
+inline MarchParams make_ndc_params(const UbnNdcMarchCfg* c, const GridView& shift_grid) {
+  MarchParams p{};
+  p.S = c->n_samples;
+  p.shift = 0.f; p.interval = c->interval; p.thres = c->fast_color_thres;
+  p.use_cumdist = 0;
+  p.use_mask = c->use_maskcache;
+  for (int a = 0; a < 3; ++a) {
+    p.msz[a] = c->mask_sz[a]; p.mscale[a] = c->mask_scale[a]; p.mshift[a] = c->mask_shift[a];
+    p.bmin[a] = c->xyz_min[a]; p.bmax[a] = c->xyz_max[a];
+  }
+  p.shift_grid = shift_grid;
   return p;
 }
 
@@ -76,6 +93,41 @@ __device__ __forceinline__ bool sample_point(const Ray& r, float t, const MarchP
   }
   return inner;
 }
+
+// Sampling policies of the fused march kernels (march.cu, march_ndc.cu).  A policy says where sample s of a ray lies, whether the
+// model samples there at all, and what is added to the density-grid value before Raw2Alpha.  The scan, flags, compaction and
+// backward scan code is written once against this interface.
+//   point(r, t_table, s, p, x, y, z, inner) -> false when the sample is outside the model's domain; `inner` -> UBN_FLAG_INNER
+//   density(p, d, x, y, z)                  -> the raw density that Raw2Alpha(shift = p.shift) activates
+struct ContractedSampler {      // FourierGrid_model.py:509-552, dcvgo.py:228-262: contracted point at t_table[s]
+  __device__ static Ray load(const float* o, const float* d, const MarchParams& p) { return load_ray(o, d, p); }
+  __device__ static bool point(const Ray& r, const float* t_table, int s, const MarchParams& p, float& x, float& y, float& z,
+                               bool& inner) {
+    inner = sample_point(r, t_table[s], p, x, y, z);
+    return true;
+  }
+  __device__ static float density(const MarchParams&, float d, float, float, float) { return d; }
+};
+
+struct NdcSampler {             // dmpigo.py:224-249, 275: NDC point inside the strict bbox; density + act_shift(p)
+  __device__ static Ray load(const float* o, const float* d, const MarchParams&) {
+    Ray r;
+    r.ox = o[0]; r.oy = o[1]; r.oz = o[2];
+    r.dx = d[0]; r.dy = d[1]; r.dz = d[2];
+    return r;
+  }
+  __device__ static bool point(const Ray& r, const float*, int s, const MarchParams& p, float& x, float& y, float& z,
+                               bool& inner) {
+    ndc_point(r.ox, r.oy, r.oz, r.dx, r.dy, r.dz, s, p.S, x, y, z);
+    inner = false;
+    return !((p.bmin[0] > x) | (p.bmin[1] > y) | (p.bmin[2] > z) | (p.bmax[0] < x) | (p.bmax[1] < y) | (p.bmax[2] < z));
+  }
+  // act_shift is a [1,1,1,1,D] grid: X = Y = 1, so the pre-clamped cell does not apply; the general trilinear read is
+  // F.grid_sample's arithmetic for any shape.  One fp32 add, as torch's `density(p) + act_shift(p)`.
+  __device__ static float density(const MarchParams& p, float d, float x, float y, float z) {
+    return __fadd_rn(d, grid_density_at(p.shift_grid, x, y, z));
+  }
+};
 
 struct CellR {
   int v;            // base voxel index  (x0*Y + y0)*Z + z0, pre-clamped

@@ -230,10 +230,9 @@ __global__ void k_sample_ndc(const float* __restrict__ rays_o, const float* __re
   if (idx >= n_rays * n_samples) return;
   const int64_t r = idx / n_samples;
   const int i_step = (int)(idx % n_samples);
-  const float dist = ((float)i_step) / (n_samples - 1);
-  const float px = rays_o[3 * r] + rays_d[3 * r] * dist;
-  const float py = rays_o[3 * r + 1] + rays_d[3 * r + 1] * dist;
-  const float pz = rays_o[3 * r + 2] + rays_d[3 * r + 2] * dist;
+  float px, py, pz;
+  ndc_point(rays_o[3 * r], rays_o[3 * r + 1], rays_o[3 * r + 2], rays_d[3 * r], rays_d[3 * r + 1], rays_d[3 * r + 2], i_step,
+            n_samples, px, py, pz);
   rays_pts[3 * idx] = px;
   rays_pts[3 * idx + 1] = py;
   rays_pts[3 * idx + 2] = pz;

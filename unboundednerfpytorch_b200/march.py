@@ -1,6 +1,8 @@
 """Fused ray march (autograd.Function) over the C ABI: the hot path of FourierGridModel.forward
-(FourierGrid_model.py:554-621) and DirectContractedVoxGO.forward (dcvgo.py:264-331) up to and including
-the feature-grid read, in 3 launches forward (pass A, scan, pass B) and 2 backward.
+(FourierGrid_model.py:554-621) and DirectContractedVoxGO.forward (dcvgo.py:264-331) -- ``March`` -- and of
+DirectMPIGO.forward (dmpigo.py:251-295) -- ``NdcMarch`` -- up to and including the feature-grid read, in 3 launches
+forward (pass A, scan, pass B) and 2 backward.  Both share the dense pass-A records, the compaction and the
+gradient-buffer plumbing below.
 """
 import functools
 import os
@@ -9,7 +11,7 @@ import numpy as np
 import torch
 
 from . import _cabi, ops
-from ._cabi import UbnMarchCfg, c_i64, check, ptr, stream_of
+from ._cabi import UbnMarchCfg, UbnNdcMarchCfg, c_i64, check, ptr, stream_of
 from .grid import grid_desc
 
 
@@ -75,6 +77,41 @@ def make_cfg(scene_center, scene_radius, bg_len, contracted_norm, n_samples, act
     return c
 
 
+def _pass_a_buffers(N, S, dev):
+    """Dense per-sample records of pass A: density, alpha, weight, T [N*S], flags [N*S], alphainv_last [N], n_keep [N]."""
+    f32 = dict(dtype=torch.float32, device=dev)
+    return (torch.empty(N * S, **f32), torch.empty(N * S, **f32), torch.empty(N * S, **f32), torch.empty(N * S, **f32),
+            torch.empty(N * S, dtype=torch.uint8, device=dev), torch.empty(N, **f32), torch.empty(N, dtype=torch.int32, device=dev))
+
+
+def _compact(lib, nkeep, N, S, dense_known, st):
+    """offsets[N+1] = exclusive scan of the per-ray survivor counts, and M = offsets[N]: known without a host sync when nothing
+    can be masked out, else the march's one device-to-host read."""
+    offsets = torch.empty(N + 1, dtype=torch.int64, device=nkeep.device)
+    scratch = torch.empty(N // 1024 + 4, dtype=torch.int64, device=nkeep.device)
+    check(lib.ubn_exclusive_scan_i32(ptr(nkeep), c_i64(N), ptr(offsets), ptr(scratch), st))
+    M = N * S if dense_known else int(offsets[N].item())
+    return offsets, M
+
+
+def _grad_target(param, meta, want, dev):
+    """(gradient buffer to scatter into, the parameter's persistent buffer or None).  Persistent gradient buffers
+    (dist.PeerTail / grid.attach_grad_buffer): the scatter adds straight into a buffer the training loop owns (peer-mapped for
+    the multi-GPU tail, zero at the start of a step) instead of a fresh zero-filled allocation per step."""
+    if not want:
+        return None, None
+    buf = getattr(param, '_ubn_grad_buffer', None)
+    return (buf if buf is not None else torch.empty_strided(*meta, dtype=torch.float32, device=dev).zero_()), buf
+
+
+def _hand_over(param, grad, buf):
+    """With a persistent buffer the parameter's .grad is pointed at it and autograd gets no gradient to accumulate."""
+    if buf is not None:
+        param.grad = buf
+        return None
+    return grad
+
+
 class March(torch.autograd.Function):
     """(density_grid, k0_grid, rays) -> compacted per-survivor records.
 
@@ -90,24 +127,14 @@ class March(torch.autograd.Function):
         rays_d = rays_d.contiguous().float()
         N, S = rays_o.shape[0], cfg.n_samples
         f32 = dict(dtype=torch.float32, device=dev)
-        dens = torch.empty(N * S, **f32)
-        alpha = torch.empty(N * S, **f32)
-        weight = torch.empty(N * S, **f32)
-        T = torch.empty(N * S, **f32)
-        flags = torch.empty(N * S, dtype=torch.uint8, device=dev)
-        last = torch.empty(N, **f32)
-        nkeep = torch.empty(N, dtype=torch.int32, device=dev)
-        offsets = torch.empty(N + 1, dtype=torch.int64, device=dev)
-        scratch = torch.empty(N // 1024 + 4, dtype=torch.int64, device=dev)
+        dens, alpha, weight, T, flags, last, nkeep = _pass_a_buffers(N, S, dev)
         with ops._Guard(rays_o) as lib:
             st = stream_of(rays_o)
             with _cabi.timed('march_density_fwd'):
                 check(lib.ubn_march_density_fwd(ptr(rays_o), ptr(rays_d), ptr(t_table), ptr(density_grid), ddesc,
                                                 ptr(mask_world), cfg, c_i64(N), ptr(dens), ptr(alpha), ptr(weight), ptr(T),
                                                 ptr(flags), ptr(last), ptr(nkeep), st))
-            check(lib.ubn_exclusive_scan_i32(ptr(nkeep), c_i64(N), ptr(offsets), ptr(scratch), st))
-            # compacted size: known without a host sync when nothing can be masked out
-            M = N * S if dense_known else int(offsets[N].item())
+            offsets, M = _compact(lib, nkeep, N, S, dense_known, st)
             C = k0_grid.shape[1]
             feat = torch.empty(M, C, **f32)
             o_dens = torch.empty(M, **f32)
@@ -133,10 +160,7 @@ class March(torch.autograd.Function):
         ctx.cfg, ctx.ddesc, ctx.kdesc = cfg, ddesc, kdesc
         ctx.dmeta = (density_grid.shape, density_grid.stride())
         ctx.kmeta = (k0_grid.shape, k0_grid.stride())
-        # persistent gradient buffers (dist.PeerTail / grid.attach_grad_buffer): the scatter adds straight into a buffer the
-        # training loop owns (peer-mapped for the multi-GPU tail, zero at the start of a step) instead of a fresh zero-filled
-        # 1.5 GB allocation per step; the parameter's .grad is pointed at it and autograd gets no gradient to accumulate
-        ctx.dparam, ctx.kparam = density_grid, k0_grid
+        ctx.dparam, ctx.kparam = density_grid, k0_grid      # for their persistent gradient buffers (_grad_target)
         ctx.mark_non_differentiable(ray_id, step_id, o_t, o_inner)
         return o_weight, last, o_alpha, o_dens, feat, ray_id, step_id, o_t, o_inner
 
@@ -148,16 +172,11 @@ class March(torch.autograd.Function):
         N = rays_o.shape[0]
         cont = lambda g: g.contiguous() if g is not None else None
         g_weight, g_last, g_alpha, g_dens, g_feat = map(cont, (g_weight, g_last, g_alpha, g_dens, g_feat))
-        grad_d = grad_k = None
         with ops._Guard(rays_o) as lib:
             want_k = ctx.needs_input_grad[1] and g_feat is not None
             want_d = ctx.needs_input_grad[0]
-            buf_d = getattr(ctx.dparam, '_ubn_grad_buffer', None) if want_d else None
-            buf_k = getattr(ctx.kparam, '_ubn_grad_buffer', None) if want_k else None
-            if want_d:
-                grad_d = buf_d if buf_d is not None else torch.empty_strided(*ctx.dmeta, dtype=torch.float32, device=dev).zero_()
-            if want_k:
-                grad_k = buf_k if buf_k is not None else torch.empty_strided(*ctx.kmeta, dtype=torch.float32, device=dev).zero_()
+            grad_d, buf_d = _grad_target(ctx.dparam, ctx.dmeta, want_d, dev)
+            grad_k, buf_k = _grad_target(ctx.kparam, ctx.kmeta, want_k, dev)
             if want_k:
                 with _cabi.timed('march_feature_bwd'):
                     check(lib.ubn_march_feature_bwd(ptr(rays_o), ptr(rays_d), ptr(t_table), ctx.kdesc, ctx.cfg, c_i64(N),
@@ -168,8 +187,93 @@ class March(torch.autograd.Function):
                                                     ptr(dens), ptr(alpha), ptr(weight), ptr(T), ptr(flags), ptr(last),
                                                     ptr(offsets), ptr(g_weight), ptr(g_alpha), ptr(g_dens), ptr(g_last),
                                                     ptr(grad_d), stream_of(rays_o)))
-        if buf_d is not None:
-            ctx.dparam.grad, grad_d = buf_d, None
-        if buf_k is not None:
-            ctx.kparam.grad, grad_k = buf_k, None
+        grad_d = _hand_over(ctx.dparam, grad_d, buf_d)
+        grad_k = _hand_over(ctx.kparam, grad_k, buf_k)
         return grad_d, grad_k, None, None, None, None, None, None, None, None, None
+
+
+def make_ndc_cfg(xyz_min, xyz_max, n_samples, interval, fast_color_thres, mask, mask_scale, mask_shift):
+    c = UbnNdcMarchCfg()
+    for a in range(3):
+        c.xyz_min[a] = float(xyz_min[a])
+        c.xyz_max[a] = float(xyz_max[a])
+        c.mask_sz[a] = int(mask.shape[a])
+        c.mask_scale[a] = float(mask_scale[a])
+        c.mask_shift[a] = float(mask_shift[a])
+    c.n_samples = int(n_samples)
+    c.interval = float(interval)
+    c.fast_color_thres = float(fast_color_thres)
+    c.use_maskcache = 1
+    return c
+
+
+def ndc_supported(k0_grid):
+    """Grids the fused NDC feature read covers: single-slab channels-last k0 with 3 or 9 channels, >= 2 voxels per axis."""
+    return (k0_grid.is_cuda and k0_grid.dim() == 5 and k0_grid.shape[0] == 1 and k0_grid.shape[1] in (3, 9)
+            and k0_grid.stride(1) == 1 and min(k0_grid.shape[2:]) >= 2 and k0_grid[0, 0].numel() < 2 ** 31)
+
+
+class NdcMarch(torch.autograd.Function):
+    """DirectMPIGO's march: (density_grid, k0_grid, rays) -> compacted per-survivor records.
+
+    Returns (weights[M], alphainv_last[N], raw_alpha[M], k0_feat[M,C], ray_id[M] i64, step_id[M] i64).  Differentiable wrt
+    density_grid and k0_grid; act_shift_grid is a constant (requires_grad=False in the reference, dmpigo.py:50)."""
+
+    @staticmethod
+    def forward(ctx, density_grid, k0_grid, act_shift_grid, rays_o, rays_d, mask_world, cfg, ddesc, kdesc, sdesc):
+        dev = rays_o.device
+        rays_o = rays_o.contiguous().float()
+        rays_d = rays_d.contiguous().float()
+        N, S = rays_o.shape[0], cfg.n_samples
+        f32 = dict(dtype=torch.float32, device=dev)
+        dens, alpha, weight, T, flags, last, nkeep = _pass_a_buffers(N, S, dev)
+        with ops._Guard(rays_o) as lib:
+            st = stream_of(rays_o)
+            with _cabi.timed('march_ndc_density_fwd'):
+                check(lib.ubn_march_ndc_density_fwd(ptr(rays_o), ptr(rays_d), ptr(density_grid), ddesc, ptr(act_shift_grid), sdesc,
+                                                    ptr(mask_world), cfg, c_i64(N), ptr(dens), ptr(alpha), ptr(weight), ptr(T),
+                                                    ptr(flags), ptr(last), ptr(nkeep), st))
+            offsets, M = _compact(lib, nkeep, N, S, False, st)
+            feat = torch.empty(M, k0_grid.shape[1], **f32)
+            o_alpha = torch.empty(M, **f32)
+            o_weight = torch.empty(M, **f32)
+            ray_id = torch.empty(M, dtype=torch.int64, device=dev)
+            step_id = torch.empty(M, dtype=torch.int64, device=dev)
+            with _cabi.timed('march_ndc_feature_fwd'):
+                check(lib.ubn_march_ndc_feature_fwd(ptr(rays_o), ptr(rays_d), ptr(k0_grid), kdesc, cfg, c_i64(N), ptr(flags),
+                                                    ptr(offsets), ptr(alpha), ptr(weight), ptr(feat), ptr(o_alpha), ptr(o_weight),
+                                                    ptr(ray_id), ptr(step_id), st))
+        ctx.save_for_backward(rays_o, rays_d, dens, alpha, weight, T, flags, last, offsets)
+        ctx.cfg, ctx.ddesc, ctx.kdesc = cfg, ddesc, kdesc
+        ctx.dmeta = (density_grid.shape, density_grid.stride())
+        ctx.kmeta = (k0_grid.shape, k0_grid.stride())
+        ctx.dparam, ctx.kparam = density_grid, k0_grid
+        ctx.mark_non_differentiable(ray_id, step_id)
+        return o_weight, last, o_alpha, feat, ray_id, step_id
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_weight, g_last, g_alpha, g_feat, *unused):
+        rays_o, rays_d, dens, alpha, weight, T, flags, last, offsets = ctx.saved_tensors
+        dev = rays_o.device
+        N = rays_o.shape[0]
+        cont = lambda g: g.contiguous() if g is not None else None
+        g_weight, g_last, g_alpha, g_feat = map(cont, (g_weight, g_last, g_alpha, g_feat))
+        with ops._Guard(rays_o) as lib:
+            st = stream_of(rays_o)
+            want_k = ctx.needs_input_grad[1] and g_feat is not None
+            want_d = ctx.needs_input_grad[0]
+            grad_d, buf_d = _grad_target(ctx.dparam, ctx.dmeta, want_d, dev)
+            grad_k, buf_k = _grad_target(ctx.kparam, ctx.kmeta, want_k, dev)
+            if want_k:
+                with _cabi.timed('march_ndc_feature_bwd'):
+                    check(lib.ubn_march_ndc_feature_bwd(ptr(rays_o), ptr(rays_d), ctx.kdesc, ctx.cfg, c_i64(N), ptr(flags),
+                                                        ptr(offsets), ptr(g_feat), ptr(grad_k), st))
+            if want_d:
+                with _cabi.timed('march_ndc_density_bwd'):
+                    check(lib.ubn_march_ndc_density_bwd(ptr(rays_o), ptr(rays_d), ctx.ddesc, ctx.cfg, c_i64(N), ptr(dens),
+                                                        ptr(alpha), ptr(weight), ptr(T), ptr(flags), ptr(last), ptr(offsets),
+                                                        ptr(g_weight), ptr(g_alpha), ptr(g_last), ptr(grad_d), st))
+        grad_d = _hand_over(ctx.dparam, grad_d, buf_d)
+        grad_k = _hand_over(ctx.kparam, grad_k, buf_k)
+        return grad_d, grad_k, None, None, None, None, None, None, None, None

@@ -1,7 +1,9 @@
-"""Unbounded-scene voxel-grid radiance-field models with the reference's constructor / forward surface:
+"""Voxel-grid radiance-field models with the reference's constructor / forward surface:
 
 * ``FourierGridModel``       -- FourierGrid/FourierGrid_model.py:134-681
 * ``DirectContractedVoxGO``  -- FourierGrid/dcvgo.py:28-384
+* ``DirectVoxGO``            -- FourierGrid/dvgo.py:26-425 (bounded scenes)
+* ``DirectMPIGO``            -- FourierGrid/dmpigo.py:18-340 (forward-facing scenes in NDC space)
 
 Same constructor keywords, ``get_kwargs()`` keys, state-dict names (``density.grid``, ``k0.grid``,
 ``rgbnet.{0,2.0,3}.{weight,bias}``, ``mask_cache.mask`` ...), ``forward(rays_o, rays_d, viewdirs,
@@ -704,4 +706,238 @@ class DirectVoxGO(nn.Module):
         if render_kwargs.get('render_depth', False):
             with torch.no_grad():
                 ret['depth'] = segment_sum(weights * step_id, ray_id, N)
+        return ret
+
+
+# ======================================================================================================
+class DirectMPIGO(nn.Module):
+    """Forward-facing model in NDC space (FourierGrid/dmpigo.py:18-340): a DenseGrid density with a frozen per-plane bias
+    ``act_shift`` ([1,1,1,1,mpi_depth] DenseGrid), a DenseGrid k0 (3 channels, or rgbnet_dim features + rgbnet), a mask cache,
+    NDC samples o + d * i/(S-1) inside the bbox.  ``forward`` runs the fused NDC march (march.NdcMarch); ``forward_ops``
+    composes the drop-in ops in the reference's order."""
+
+    def __init__(self, xyz_min, xyz_max, num_voxels=0, mpi_depth=0, mask_cache_path=None, mask_cache_thres=1e-3,
+                 mask_cache_world_size=None, fast_color_thres=0, density_type='DenseGrid', k0_type='DenseGrid',
+                 density_config={}, k0_config={}, rgbnet_dim=0, rgbnet_depth=3, rgbnet_width=128, viewbase_pe=0, **kwargs):
+        super().__init__()
+        if density_type != 'DenseGrid' or k0_type != 'DenseGrid':
+            raise NotImplementedError('only DenseGrid is on the hot path (TensoRFGrid is out of scope)')
+        self.register_buffer('xyz_min', torch.as_tensor(np.asarray(xyz_min), dtype=torch.float32).clone())
+        self.register_buffer('xyz_max', torch.as_tensor(np.asarray(xyz_max), dtype=torch.float32).clone())
+        self.fast_color_thres = fast_color_thres
+        self._set_grid_resolution(num_voxels, mpi_depth)
+        self.density_type, self.density_config = density_type, density_config
+        self.density = G.DenseGrid(channels=1, world_size=self.world_size, xyz_min=self.xyz_min, xyz_max=self.xyz_max)
+        # initial bias: every plane contributes the same alpha to a ray crossing all of them (dmpigo.py:45-57)
+        self.act_shift = G.DenseGrid(channels=1, world_size=[1, 1, mpi_depth], xyz_min=xyz_min, xyz_max=xyz_max)
+        self.act_shift.grid.requires_grad = False
+        with torch.no_grad():
+            g = np.full([mpi_depth], 1. / mpi_depth - 1e-6)
+            p = [1 - g[0]]
+            for i in range(1, len(g)):
+                p.append((1 - g[:i + 1].sum()) / (1 - g[:i].sum()))
+            for i in range(len(p)):
+                self.act_shift.grid[..., i].fill_(np.log(p[i] ** (-1 / self.voxel_size_ratio) - 1))
+        self.rgbnet_kwargs = dict(rgbnet_dim=rgbnet_dim, rgbnet_depth=rgbnet_depth, rgbnet_width=rgbnet_width,
+                                  viewbase_pe=viewbase_pe)
+        self.k0_type, self.k0_config = k0_type, k0_config
+        if rgbnet_dim <= 0:
+            self.k0_dim, self.rgbnet = 3, None
+            self.k0 = G.DenseGrid(channels=3, world_size=self.world_size, xyz_min=self.xyz_min, xyz_max=self.xyz_max)
+        else:
+            self.k0_dim = rgbnet_dim
+            self.k0 = G.DenseGrid(channels=rgbnet_dim, world_size=self.world_size, xyz_min=self.xyz_min, xyz_max=self.xyz_max)
+            self.register_buffer('viewfreq', torch.FloatTensor([(2 ** i) for i in range(viewbase_pe)]))
+            self.rgbnet = _make_rgbnet(3 + 3 * viewbase_pe * 2 + rgbnet_dim, rgbnet_width, rgbnet_depth)
+        self.mask_cache_path, self.mask_cache_thres = mask_cache_path, mask_cache_thres
+        if mask_cache_world_size is None:
+            mask_cache_world_size = self.world_size
+        if mask_cache_path:
+            raise NotImplementedError('coarse-checkpoint mask cache needs a device at construction; build MaskGrid(path=...) '
+                                      'and assign model.mask_cache instead')
+        self.mask_cache = G.MaskGrid(path=None, mask=torch.ones([int(v) for v in mask_cache_world_size], dtype=torch.bool),
+                                     xyz_min=self.xyz_min, xyz_max=self.xyz_max)
+        self._host_cache = None
+        self._mask_host = None
+
+    def _set_grid_resolution(self, num_voxels, mpi_depth):
+        """dmpigo.py:120-130: X, Y from the voxel budget per plane (fp32 sqrt, truncated to long), Z = mpi_depth."""
+        self.num_voxels = num_voxels
+        self.mpi_depth = mpi_depth
+        mn, mx = self.xyz_min.cpu(), self.xyz_max.cpu()
+        r = (num_voxels / self.mpi_depth / (mx - mn)[:2].prod()).sqrt()
+        self.world_size = torch.zeros(3, dtype=torch.long)
+        self.world_size[:2] = (mx - mn)[:2] * r
+        self.world_size[2] = self.mpi_depth
+        self.voxel_size_ratio = 256. / mpi_depth
+
+    def get_kwargs(self):
+        return {
+            'xyz_min': self.xyz_min.cpu().numpy(), 'xyz_max': self.xyz_max.cpu().numpy(), 'num_voxels': self.num_voxels,
+            'mpi_depth': self.mpi_depth, 'voxel_size_ratio': self.voxel_size_ratio, 'mask_cache_path': self.mask_cache_path,
+            'mask_cache_thres': self.mask_cache_thres, 'mask_cache_world_size': list(self.mask_cache.mask.shape),
+            'fast_color_thres': self.fast_color_thres, 'density_type': self.density_type, 'k0_type': self.k0_type,
+            'density_config': self.density_config, 'k0_config': self.k0_config, **self.rgbnet_kwargs,
+        }
+
+    # ---- host-side caches (bbox and mask-cache geometry go to the kernels by value) ----------------------------------------
+    def _apply(self, fn, *a, **k):
+        self._host_cache = self._mask_host = None
+        return super()._apply(fn, *a, **k)
+
+    def _load_from_state_dict(self, *a, **k):
+        self._host_cache = self._mask_host = None
+        return super()._load_from_state_dict(*a, **k)
+
+    def _host(self):
+        if self._host_cache is None:
+            self._host_cache = (self.xyz_min.detach().cpu().tolist(), self.xyz_max.detach().cpu().tolist())
+        return self._host_cache
+
+    def _mask_geometry(self):
+        if self._mask_host is None or self._mask_host[0] is not self.mask_cache:
+            self._mask_host = (self.mask_cache, self.mask_cache.xyz2ijk_scale.cpu().tolist(),
+                               self.mask_cache.xyz2ijk_shift.cpu().tolist())
+        return self._mask_host[1], self._mask_host[2]
+
+    # ---- grid maintenance -----------------------------------------------------------------------------------------------
+    @torch.no_grad()
+    def scale_volume_grid(self, num_voxels, mpi_depth):
+        """dmpigo.py:150-172.  The mask rebuild activates density + act_shift.grid (the per-sample path adds act_shift too)."""
+        self._set_grid_resolution(num_voxels, mpi_depth)
+        self.density.scale_volume_grid(self.world_size)
+        self.k0.scale_volume_grid(self.world_size)
+        if np.prod(self.world_size.tolist()) <= 256 ** 3:
+            dev = self.density.grid.device
+            ws = [int(v) for v in self.world_size]
+            axes = [torch.linspace(float(self.xyz_min[a]), float(self.xyz_max[a]), ws[a], device=dev) for a in range(3)]
+            xyz = torch.stack(torch.meshgrid(*axes, indexing='ij'), -1)
+            dens = (self.density.get_dense_grid() + self.act_shift.grid).contiguous()
+            alpha = F.max_pool3d(self.activate_density(dens), kernel_size=3, padding=1, stride=1)[0, 0]
+            self.mask_cache = G.MaskGrid(path=None, mask=self.mask_cache(xyz) & (alpha > self.fast_color_thres),
+                                         xyz_min=self.xyz_min, xyz_max=self.xyz_max).to(dev)
+
+    @torch.no_grad()
+    def update_occupancy_cache(self):
+        """dmpigo.py:174-187: mask &= max_pool3d(Raw2Alpha(density(lattice), shift 0)) > fast_color_thres -- WITHOUT act_shift,
+        as the reference does (two launches: ops.lattice_alpha, ops.maxpool3_gt_and_)."""
+        from . import ops
+        mn, mx = self.density._bounds()
+        lo, hi = self._host()
+        alpha = ops.lattice_alpha(self.density.grid.data, mn, mx, 0, lo, hi, self.mask_cache.mask.shape, 0.0,
+                                  float(self.voxel_size_ratio))
+        ops.maxpool3_gt_and_(self.mask_cache.mask, alpha, self.fast_color_thres)
+
+    @torch.no_grad()
+    def update_occupancy_cache_lt_nviews(self, rays_o_tr, rays_d_tr, imsz, render_kwargs, maskout_lt_nviews):
+        """dmpigo.py:189-207: mask &= (number of training views whose samples reach a voxel's trilinear support with total weight
+        > 1) >= maskout_lt_nviews.  Per view, the grid-sample adjoint of ones over the view's in-box NDC samples."""
+        dev = self.density.grid.device
+        mn, mx = self.density._bounds()
+        count = torch.zeros_like(self.density.get_dense_grid(), dtype=torch.long)
+        for rays_o_, rays_d_ in zip(rays_o_tr.split(imsz), rays_d_tr.split(imsz)):
+            ones = torch.zeros_like(self.density.get_dense_grid()).requires_grad_(True)
+            with torch.enable_grad():
+                for rays_o, rays_d in zip(rays_o_.split(8192), rays_d_.split(8192)):
+                    ray_pts = self.sample_ray(rays_o=rays_o.to(dev), rays_d=rays_d.to(dev), **render_kwargs)[0]
+                    G.grid_sample(ones, ray_pts, mn, mx, 0).sum().backward()
+            count += (ones.grad > 1)
+        self.mask_cache.mask &= (count >= maskout_lt_nviews)[0, 0]
+
+    def density_total_variation_add_grad(self, weight, dense_mode):
+        wxy, wxy_, wz, _ = self._tv_weights(weight, dense_mode)
+        self.density.total_variation_add_grad(wxy, wxy_, wz, dense_mode)
+
+    def k0_total_variation_add_grad(self, weight, dense_mode):
+        wxy, wxy_, wz, _ = self._tv_weights(weight, dense_mode)
+        self.k0.total_variation_add_grad(wxy, wxy_, wz, dense_mode)
+
+    def _tv_weights(self, weight, dense_mode):
+        """dmpigo.py:209-217: (wxy, wxy, wz) with wxy = weight * max(world_size[:2]) / 128 (an fp32 tensor expression there)
+        and wz = weight * mpi_depth / 128."""
+        wxy = float(weight * self.world_size[:2].max() / 128)
+        wz = weight * self.mpi_depth / 128
+        return (wxy, wxy, wz, dense_mode)
+
+    def tv_terms(self, weight_density=0., weight_k0=0., dense_mode=True):
+        """{grid parameter: (wx, wy, wz, dense_mode)} for dist.reduce_tv_step (same weights as the two methods above)."""
+        return {grid.grid: self._tv_weights(weight, dense_mode)
+                for grid, weight in ((self.density, weight_density), (self.k0, weight_k0)) if weight > 0}
+
+    # ---- rendering ------------------------------------------------------------------------------------------------------
+    def activate_density(self, density, interval=None):
+        interval = interval if interval is not None else self.voxel_size_ratio
+        shape = density.shape
+        return Raw2Alpha.apply(density.flatten().contiguous(), 0., interval).reshape(shape)
+
+    def _n_samples(self, stepsize):
+        return int((self.mpi_depth - 1) / stepsize) + 1
+
+    def sample_ray(self, rays_o, rays_d, near, far, stepsize, **render_kwargs):
+        """dmpigo.py:224-249 -> (ray_pts [M,3], ray_id [M], step_id [M], N_samples) of the in-box NDC samples."""
+        from . import ops
+        assert near == 0 and far == 1
+        N_samples = self._n_samples(stepsize)
+        ray_pts, mask_outbbox = ops.sample_ndc_pts_on_rays(rays_o.contiguous(), rays_d.contiguous(), self.xyz_min, self.xyz_max,
+                                                           N_samples)
+        mask_inbbox = ~mask_outbbox
+        dev = rays_o.device
+        ray_id = torch.arange(mask_inbbox.shape[0], device=dev).view(-1, 1).expand_as(mask_inbbox)[mask_inbbox]
+        step_id = torch.arange(mask_inbbox.shape[1], device=dev).view(1, -1).expand_as(mask_inbbox)[mask_inbbox]
+        return ray_pts[mask_inbbox], ray_id, step_id, N_samples
+
+    _shade = _ContractedBase._shade        # sigmoid(k0), or the rgbnet on cat[k0, view embedding] (cuBLAS for LLFF's width 64)
+
+    def _fused_ok(self):
+        return march.ndc_supported(self.k0.grid) and self.density.grid.is_cuda
+
+    def forward(self, rays_o, rays_d, viewdirs, global_step=None, **render_kwargs):
+        assert len(rays_o.shape) == 2 and rays_o.shape[-1] == 3, 'Only suuport point queries in [N, 3] format'
+        if not self._fused_ok():
+            return self.forward_ops(rays_o, rays_d, viewdirs, global_step=global_step, **render_kwargs)
+        assert render_kwargs['near'] == 0 and render_kwargs['far'] == 1
+        N = len(rays_o)
+        N_samples = self._n_samples(render_kwargs['stepsize'])
+        lo, hi = self._host()
+        mscale, mshift = self._mask_geometry()
+        cfg = march.make_ndc_cfg(lo, hi, N_samples, render_kwargs['stepsize'] * self.voxel_size_ratio, self.fast_color_thres,
+                                 self.mask_cache.mask, mscale, mshift)
+        descs = [G.grid_desc(g.grid, *g._bounds(), 0) for g in (self.density, self.k0, self.act_shift)]
+        weights, alphainv_last, alpha, k0, ray_id, step_id = march.NdcMarch.apply(
+            self.density.grid, self.k0.grid, self.act_shift.grid, rays_o, rays_d, self.mask_cache.mask, cfg, *descs)
+        rgb = self._shade(k0, viewdirs, ray_id)
+        return self._finish(N, weights, alphainv_last, alpha, rgb, ray_id, step_id, N_samples, global_step, render_kwargs)
+
+    def forward_ops(self, rays_o, rays_d, viewdirs, global_step=None, **render_kwargs):
+        """Op-by-op composition in the reference's order (dmpigo.py:251-340)."""
+        N = len(rays_o)
+        ray_pts, ray_id, step_id, N_samples = self.sample_ray(rays_o=rays_o, rays_d=rays_d, **render_kwargs)
+        interval = render_kwargs['stepsize'] * self.voxel_size_ratio
+        mask = self.mask_cache(ray_pts)
+        ray_pts, ray_id, step_id = ray_pts[mask], ray_id[mask], step_id[mask]
+        density = self.density(ray_pts) + self.act_shift(ray_pts)
+        alpha = self.activate_density(density, interval)
+        if self.fast_color_thres > 0:
+            mask = (alpha > self.fast_color_thres)
+            ray_pts, ray_id, step_id, alpha = ray_pts[mask], ray_id[mask], step_id[mask], alpha[mask]
+        weights, alphainv_last = Alphas2Weights.apply(alpha.contiguous(), ray_id.contiguous(), N)
+        if self.fast_color_thres > 0:
+            mask = (weights > self.fast_color_thres)
+            ray_pts, ray_id, step_id, alpha, weights = ray_pts[mask], ray_id[mask], step_id[mask], alpha[mask], weights[mask]
+        k0 = self.k0(ray_pts)
+        rgb = self._shade(k0, viewdirs, ray_id)
+        return self._finish(N, weights, alphainv_last, alpha, rgb, ray_id, step_id, N_samples, global_step, render_kwargs)
+
+    def _finish(self, N, weights, alphainv_last, alpha, rgb, ray_id, step_id, N_samples, global_step, render_kwargs):
+        rgb_marched = composite_rgb(weights, rgb, ray_id, N)
+        if render_kwargs.get('rand_bkgd', False) and global_step is not None:
+            rgb_marched = rgb_marched + alphainv_last.unsqueeze(-1) * torch.rand_like(rgb_marched)
+        else:
+            rgb_marched = rgb_marched + alphainv_last.unsqueeze(-1) * render_kwargs['bg']
+        s = (step_id + 0.5) / N_samples
+        ret = {'alphainv_last': alphainv_last, 'weights': weights, 'rgb_marched': rgb_marched, 'raw_alpha': alpha,
+               'raw_rgb': rgb, 'ray_id': ray_id, 'n_max': N_samples, 's': s}
+        if render_kwargs.get('render_depth', False):
+            with torch.no_grad():
+                ret['depth'] = segment_sum(weights * s, ray_id, N)
         return ret
