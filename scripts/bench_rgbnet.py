@@ -1,0 +1,165 @@
+"""The rgbnet alone (shade.shade forward + backward, csrc/shade_tc.cu) at the truck training shape: M = 4,194,304 samples, 8192
+rays with sorted ray_id (512 consecutive samples per ray), seeded inputs.  Prints one JSON line:
+
+* ms             -- CUDA events around the forward launch (``rgbnet_fwd``) and around the two backward launches
+                    (``rgbnet_bwd``), mean over --iters steps after --warmup;
+* kernels_ms     -- with --profile DIR: per-kernel mean times from a torch.profiler run of its own (trace written to DIR);
+* rates          -- per kernel (or the backward pair from the events): HMMA-equivalent TFLOP/s, counting every issued
+                    mma.m16n8k8 TF32 as 16 * 8 * 8 * 2 FLOP (3xTF32 issues three per product), and algorithmic HBM GB/s
+                    (the bytes each kernel must read and write, computed from the shapes below), with the share of the H100 SXM
+                    data-sheet peaks (495 TFLOP/s dense TF32, 3.35 TB/s);
+* max_err        -- every gradient (k0, W1, b1, W2, b2, W3, b3) at the timed size against an fp64 evaluation, as a fraction of
+                    the largest element of the fp64 gradient (samples whose fp64 pre-activations come within 1e-5 of zero are
+                    dropped for this check, as in tests/test_gpu_models.py);
+* gpu / power_limit_w -- where it ran, read in the same run.
+
+    python scripts/bench_rgbnet.py [--iters 20] [--warmup 3] [--profile DIR] [--no-check]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+TF32_PEAK = 495e12          # H100 SXM data sheet, dense
+HBM_PEAK = 3.35e12
+MMA_FLOP = 16 * 8 * 8 * 2
+# issued mma.m16n8k8 per sample in the default 3xTF32 build (read off the SASS of the kernels)
+HMMA_PER_SAMPLE = {'k_shade_fwd_tc': 864 / 16,      # layer 1 (2 k-steps) + layer 2 (16 k-steps), 16 column tiles, 3 passes
+                   'k_shade_bwd_tc': 1120 / 16,     # dH1 768 + dX 96 + dW1k/view bias 96 + dW3 96 + E 64, per 16-sample unit
+                   'k_shade_dw2_tc': 1536 / 32}     # 8 warps x 4 k-steps x 16 column tiles x 3 passes per 32-sample chunk
+# bytes each kernel must move per sample (fp32 unless noted)
+BYTES_PER_SAMPLE = {'k_shade_fwd_tc': 48 + 8 + 12 + 512 + 512 + 16,          # feat, ray_id, rgb, H1 + H2 saves, H1 masks
+                    'k_shade_bwd_tc': 512 + 48 + 12 + 12 + 8 + 16 + 48 + 16,  # H2, feat, rgb, grad_rgb, ray_id, H1 masks; grad_feat, H2 masks
+                    'k_shade_dw2_tc': 512 + 16 + 12 + 12}                     # H1, H2 masks, rgb, grad_rgb
+
+
+def _gpu_info():
+    name = torch.cuda.get_device_name(0)
+    try:
+        out = subprocess.run(['nvidia-smi', '--query-gpu=power.limit', '--format=csv,noheader,nounits', '-i', '0'],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        power = float(out.splitlines()[0])
+    except Exception:
+        power = None
+    return name, power
+
+
+def _inputs(M, n_rays, seed=0):
+    from unboundednerfpytorch_b200 import models
+    torch.manual_seed(seed)
+    net = models._make_rgbnet(39, 128, 3).cuda()
+    g = torch.Generator().manual_seed(seed)
+    k0 = torch.randn(M, 12, generator=g).cuda()
+    emb = torch.randn(n_rays, 27, generator=g).cuda()
+    ray_id = torch.arange(n_rays).repeat_interleave(M // n_rays).cuda()
+    gr = torch.randn(M, 3, generator=g).cuda()
+    return net, k0, emb, ray_id, gr
+
+
+def _step(shade, net, k0, emb, ray_id, gr):
+    net.zero_grad(set_to_none=True)
+    k0.grad = None
+    out = shade.shade(net, k0, emb, ray_id)
+    out.backward(gr)
+
+
+def _rates(name, ms, M):
+    flop = HMMA_PER_SAMPLE[name] * MMA_FLOP * M
+    byt = BYTES_PER_SAMPLE[name] * M
+    return dict(ms=round(ms, 3), tflops_hmma_equiv=round(flop / ms / 1e9, 1), share_of_tf32_datasheet=round(flop / ms / 1e9 / (TF32_PEAK / 1e12), 3),
+                hbm_gbs=round(byt / ms / 1e6, 1), share_of_hbm_datasheet=round(byt / ms * 1e3 / HBM_PEAK, 3))
+
+
+def _check(shade, net, k0, emb, ray_id, gr, chunk=200_000):
+    """max |grad - grad_fp64| / max |grad_fp64| for k0 and every parameter, at the full size, ReLU-ambiguous samples dropped"""
+    from unboundednerfpytorch_b200 import models
+    W1, b1, W2, b2 = (p.double() for p in (net[0].weight, net[0].bias, net[2][0].weight, net[2][0].bias))
+    ok = torch.empty(k0.shape[0], dtype=torch.bool, device=k0.device)
+    with torch.no_grad():
+        for lo in range(0, k0.shape[0], chunk):
+            sl = slice(lo, lo + chunk)
+            z1 = torch.cat([k0[sl], emb[ray_id[sl]]], -1).double() @ W1.t() + b1
+            z2 = torch.relu(z1) @ W2.t() + b2
+            ok[sl] = torch.minimum(z1.abs().amin(1), z2.abs().amin(1)) > 1e-5
+    k0, ray_id, gr = k0[ok].clone().requires_grad_(True), ray_id[ok].contiguous(), gr[ok].contiguous()
+    net64 = models._make_rgbnet(39, 128, 3).cuda().double()
+    net64.load_state_dict({k: v.double() for k, v in net.state_dict().items()})
+    k64 = k0.detach().double().requires_grad_(True)
+    for lo in range(0, k0.shape[0], chunk):
+        sl = slice(lo, lo + chunk)
+        out64 = torch.sigmoid(net64(torch.cat([k64[sl], emb[ray_id[sl]].double()], -1)))
+        (out64 * gr[sl].double()).sum().backward()
+    want = [k64.grad] + [p.grad for p in net64.parameters()]
+    _step(shade, net, k0, emb, ray_id, gr)
+    got = [k0.grad] + [p.grad for p in net.parameters()]
+    err = {}
+    for a, b, nm in zip(got, want, ['k0', 'W1', 'b1', 'W2', 'b2', 'W3', 'b3']):
+        err[nm] = float((a.double() - b).abs().max() / b.abs().max())
+    return err, int(k0.shape[0])
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--samples', type=int, default=4_194_304)
+    ap.add_argument('--rays', type=int, default=8192)
+    ap.add_argument('--iters', type=int, default=20)
+    ap.add_argument('--warmup', type=int, default=3)
+    ap.add_argument('--profile', default=None, help='also run a torch.profiler pass and write its trace under this directory')
+    ap.add_argument('--no-check', action='store_true')
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        sys.exit('bench_rgbnet.py needs a GPU')
+    from unboundednerfpytorch_b200 import _cabi, shade
+    name, power = _gpu_info()
+    M = args.samples
+    net, k0, emb, ray_id, gr = _inputs(M, args.rays)
+    k0.requires_grad_(True)
+    res = dict(metric='rgbnet forward + backward, truck shape', gpu=name, power_limit_w=power, samples=M, rays=args.rays,
+               mode=shade.MODE, bwd_mode=shade.BWD_MODE)
+    for _ in range(args.warmup):
+        _step(shade, net, k0, emb, ray_id, gr)
+    torch.cuda.synchronize()
+    _cabi.TIMER = _cabi.KernelTimer()
+    for _ in range(args.iters):
+        _step(shade, net, k0, emb, ray_id, gr)
+    summ = _cabi.TIMER.summary()
+    _cabi.TIMER = None
+    res['ms'] = {k: round(v[0], 3) for k, v in summ.items()}
+    res['rates'] = {'k_shade_fwd_tc': _rates('k_shade_fwd_tc', summ['rgbnet_fwd'][0], M)}
+    bwd = summ['rgbnet_bwd'][0]
+    pair_flop = (HMMA_PER_SAMPLE['k_shade_bwd_tc'] + HMMA_PER_SAMPLE['k_shade_dw2_tc']) * MMA_FLOP * M
+    res['rates']['backward_pair'] = dict(ms=round(bwd, 3), tflops_hmma_equiv=round(pair_flop / bwd / 1e9, 1),
+                                         share_of_tf32_datasheet=round(pair_flop / bwd / 1e9 / (TF32_PEAK / 1e12), 3))
+    if args.profile:
+        from torch.profiler import ProfilerActivity, profile
+        os.makedirs(args.profile, exist_ok=True)
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(args.iters):
+                _step(shade, net, k0, emb, ray_id, gr)
+            torch.cuda.synchronize()
+        prof.export_chrome_trace(os.path.join(args.profile, 'bench_rgbnet.pt.trace.json'))
+        kms = {}
+        for ev in prof.key_averages():
+            for kname in HMMA_PER_SAMPLE:
+                if kname in ev.key:
+                    t = getattr(ev, 'device_time_total', None) or getattr(ev, 'cuda_time_total', 0.0)
+                    kms[kname] = kms.get(kname, 0.0) + t / 1e3 / args.iters
+        res['kernels_ms'] = {k: round(v, 3) for k, v in kms.items()}
+        for k, v in kms.items():
+            res['rates'][k] = _rates(k, v, M)
+    if not args.no_check:
+        err, n = _check(shade, net, k0.detach(), emb, ray_id, gr)
+        res['max_err_of_scale'] = {k: float(f'{v:.3g}') for k, v in err.items()}
+        res['check_samples'] = n
+        res['check_ok'] = all(v <= 1e-5 for v in err.values())
+    print(json.dumps(res))
+
+
+if __name__ == '__main__':
+    main()

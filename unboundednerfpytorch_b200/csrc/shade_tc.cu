@@ -15,7 +15,9 @@
 //
 // Sample reductions of the backward (dW1k, dW3, db2, grad_view_bias) run on the tensor cores too: their contraction
 // index is the sample, which the accumulator layout spreads over g, so the warp turns the 16 x 128 operand through a
-// private shared-memory tile and reads it back as B fragments (sample = k).
+// private shared-memory tile and reads it back as B fragments (sample = k).  Their per-unit results go into running sums
+// that each warp owns, so the backward has no shared-memory atomics (sm_90 has no native shared fp32 add: those would be
+// compare-and-swap loops).
 #include <algorithm>
 
 #include "common.cuh"
@@ -226,19 +228,62 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_fwd_tc(
 //   dz3 = g_rgb * rgb (1 - rgb);  dZ2 = (dz3 . W3) * [H2 > 0];  dH1 = dZ2 . W2;  dZ1 = dH1 * [H1 > 0]
 //   kDz1Out: write dZ1 [n,128] row-major and stop (ubn_rgbnet_bwd_small finishes on the CUDA cores); otherwise also
 //   dX = dZ1 . W1k and every sample reduction except dW2:  dW1k^T = X^T . dZ1,  grad_view_bias[ray] += sum dZ1 of the
-//   ray (segment indicators as extra A rows),  dW3 = dz3^T . H2,  db2 = sum_i W3[i] * (dz3_i^T . [H2 > 0]),  db3 = sum dz3.
+//   ray (segment indicators as extra A rows),  dW3 = dz3^T . H2,  E = dz3^T . [H2 > 0] (db2 = sum_i W3[i] * E[i]),  db3 = sum dz3.
+//
+// Each warp walks one contiguous, balanced range of 16-sample units.  The sample reductions restart their MMA accumulator every
+// unit and add it with plain fp32 adds into running sums that the warp owns (its private slice of shared memory, db3 in a
+// register), so no two warps ever touch the same word until the one cross-warp sum at the end of the CTA.  Because the range is
+// contiguous and ray_id is sorted, the dZ1 sum of the ray that is still open at the end of a unit is carried (one more row of
+// the warp's slice) into the next unit and written to grad_view_bias once, when its ray ends.
 namespace bk {
+constexpr uint32_t kFragW2f = kNT * kNT * 32 * 8;          // 64 KB: fp32 B fragments, split into hi / lo at the MMA
+constexpr uint32_t kFragW1Tf = 2 * kNT * 32 * 8;
 constexpr uint32_t oW2 = 0;                                // dH1 = dZ2 . W2: B[k][n] = W2[k][n]
-constexpr uint32_t oW1T = oW2 + kFragW2;                   // dX = dZ1 . W1k: B[k][n] = W1k[k][n]
-constexpr uint32_t oW3 = oW1T + kFragW1T;
-constexpr uint32_t oAccW1 = oW3 + 3 * kHidden * 4;         // [12][128] dW1k^T partials
-constexpr uint32_t oAccW3 = oAccW1 + kFeat * kHidden * 4;  // [3][128]
-constexpr uint32_t oAccB2 = oAccW3 + 3 * kHidden * 4;      // [128]
-constexpr uint32_t oAccB3 = oAccB2 + kHidden * 4;          // [4]
-constexpr uint32_t oTile = oAccB3 + 16;                    // per warp [16][kStride]
+constexpr uint32_t oW1T = oW2 + kFragW2f;                  // dX = dZ1 . W1k: B[k][n] = W1k[k][n]
+constexpr uint32_t oW3 = oW1T + kFragW1Tf;
+constexpr uint32_t oWarp = oW3 + 3 * kHidden * 4;
+// per warp: operand tile [16][kStride], the running sums dW1k^T [12][kStride], dW3 [3][kStride], E [3][kStride], and the
+// open ray's dZ1 sum [kStride]
 constexpr uint32_t kTileBytes = kUnit * kStride * 4;
-constexpr uint32_t smem_bytes(int warps) { return oTile + warps * kTileBytes; }
+constexpr int kSumRows = kFeat + 3 + 3;
+constexpr uint32_t kWarpBytes = kTileBytes + (kSumRows + 1) * kStride * 4;
+constexpr uint32_t smem_bytes(int warps) { return oWarp + warps * kWarpBytes; }
 }  // namespace bk
+
+// lane (g, t) of (n-tile j, k-step s) gets the fp32 pair {B[8s+2t][8j+g], B[8s+2t+1][8j+g]}, B[k][n] = W[k * ld + n]
+__device__ void stage_frags_f32(const float* __restrict__ W, int ld, int K, int N, int n_ksteps, int n_ntiles, uint2* dst, int tid,
+                                int nthreads) {
+  for (int i = tid; i < n_ntiles * n_ksteps * 32; i += nthreads) {
+    const int lane = i & 31, s = (i >> 5) % n_ksteps, j = (i >> 5) / n_ksteps;
+    const int n = 8 * j + (lane >> 2), k = 8 * s + 2 * (lane & 3);
+    const float w0 = (k < K && n < N) ? W[k * ld + n] : 0.f, w1 = (k + 1 < K && n < N) ? W[(k + 1) * ld + n] : 0.f;
+    dst[i] = make_uint2(__float_as_uint(w0), __float_as_uint(w1));
+  }
+}
+
+// mma3 with the B fragment given as fp32: the same hi / lo split (and the same three products in the same order) as stage_frags
+template <bool kThree>
+__device__ __forceinline__ void mma3f(float (&d)[4], const uint32_t (&ah)[4], const uint32_t (&al)[4], uint2 b) {
+  const uint32_t h0 = b.x & 0xFFFFE000u, h1 = b.y & 0xFFFFE000u;
+  if (kThree) {
+    mma_tf32(d, al, h0, h1);
+    mma_tf32(d, ah, __float_as_uint(__uint_as_float(b.x) - __uint_as_float(h0)),
+             __float_as_uint(__uint_as_float(b.y) - __uint_as_float(h1)));
+  }
+  mma_tf32(d, ah, h0, h1);
+}
+
+template <int KS, int NT, bool kThree>
+__device__ __forceinline__ void warp_gemm_f(float (&acc)[NT][4], const float (&x)[KS][4], const uint2* __restrict__ frag, int lane) {
+#pragma unroll
+  for (int s = 0; s < KS; ++s) {
+    const float av[4] = {x[s][0], x[s][2], x[s][1], x[s][3]};
+    uint32_t ah[4], al[4];
+    split4(av, ah, al);
+#pragma unroll
+    for (int j = 0; j < NT; ++j) mma3f<kThree>(acc[j], ah, al, frag[(j * KS + s) * 32 + lane]);
+  }
+}
 
 // B fragment of the warp tile S[16][kStride] (sample = k): k-step s, column tile j -> S[8 s + t][8 j + g], S[8 s + t + 4][..]
 __device__ __forceinline__ void tile_frag(const float* S, int s, int j, int g, int t, uint32_t (&hi)[2], uint32_t (&lo)[2]) {
@@ -259,6 +304,26 @@ __device__ __forceinline__ void tile_store(float* S, const float (&v)[kNT][4], i
   }
 }
 
+__device__ __forceinline__ void sum_add2(float* p, float a, float b) {
+  float2 v = *reinterpret_cast<float2*>(p);
+  v.x += a;
+  v.y += b;
+  *reinterpret_cast<float2*>(p) = v;
+}
+
+__device__ __forceinline__ void red_add2(float* p, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
+}
+
+// grad_view_bias[ray] += V for the columns 8 j + 2 t, + 1 (j < 16) of a g-row of lanes
+__device__ __forceinline__ void emit_ray(float* grad_view_bias, int64_t ray, const float* V, int t) {
+#pragma unroll
+  for (int j = 0; j < kNT; ++j) {
+    const float2 v = *reinterpret_cast<const float2*>(V + 8 * j + 2 * t);
+    red_add2(grad_view_bias + ray * kHidden + 8 * j + 2 * t, v.x, v.y);
+  }
+}
+
 template <bool kThree, int kWarps, bool kPanel, bool kMask1, bool kDz1Out>
 __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc(
     const float* __restrict__ feat, const int64_t* __restrict__ ray_id, const float* __restrict__ W1k,
@@ -270,22 +335,28 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc(
   extern __shared__ __align__(16) uint8_t smem[];
   constexpr int kThreads = 32 * kWarps;
   const int tid = threadIdx.x, lane = tid & 31, g = lane >> 2, t = lane & 3, warp = tid >> 5;
-  const uint4* fW2 = reinterpret_cast<const uint4*>(smem + bk::oW2);
-  const uint4* fW1T = reinterpret_cast<const uint4*>(smem + bk::oW1T);
+  const uint2* fW2 = reinterpret_cast<const uint2*>(smem + bk::oW2);
+  const uint2* fW1T = reinterpret_cast<const uint2*>(smem + bk::oW1T);
   float* sW3 = reinterpret_cast<float*>(smem + bk::oW3);
-  float* accW1 = reinterpret_cast<float*>(smem + bk::oAccW1);
-  float* accW3 = reinterpret_cast<float*>(smem + bk::oAccW3);
-  float* accB2 = reinterpret_cast<float*>(smem + bk::oAccB2);
-  float* accB3 = reinterpret_cast<float*>(smem + bk::oAccB3);
-  float* S = reinterpret_cast<float*>(smem + bk::oTile + warp * bk::kTileBytes);
-  stage_frags(W2, kHidden, false, kHidden, kHidden, kNT, kNT, reinterpret_cast<uint4*>(smem + bk::oW2), tid, kThreads);
-  if (!kDz1Out) stage_frags(W1k, kFeat, false, kHidden, kFeat, kNT, 2, reinterpret_cast<uint4*>(smem + bk::oW1T), tid, kThreads);
+  float* S = reinterpret_cast<float*>(smem + bk::oWarp + warp * bk::kWarpBytes);
+  float* sumW1 = S + kUnit * kStride;                     // dW1k^T [feature][unit]
+  float* sumW3 = sumW1 + kFeat * kStride;
+  float* sumE = sumW3 + 3 * kStride;
+  float* vbc = sumE + 3 * kStride;                        // lanes g == 4: the open ray's sum of dZ1 so far
+  stage_frags_f32(W2, kHidden, kHidden, kHidden, kNT, kNT, reinterpret_cast<uint2*>(smem + bk::oW2), tid, kThreads);
+  if (!kDz1Out) stage_frags_f32(W1k, kFeat, kHidden, kFeat, kNT, 2, reinterpret_cast<uint2*>(smem + bk::oW1T), tid, kThreads);
   for (int i = tid; i < 3 * kHidden; i += kThreads) sW3[i] = W3[i];
-  for (int i = tid; i < (kFeat + 3 + 1) * kHidden + 4; i += kThreads) accW1[i] = 0.f;   // accW1 .. accB3 are contiguous
+  if (!kDz1Out)
+    for (int i = lane; i < bk::kSumRows * kStride; i += 32) sumW1[i] = 0.f;
   __syncthreads();
 
+  float db3 = 0.f;                                        // lane i < 3: this warp's sum of dz3_i
+  int64_t open_ray = -1;                                  // warp-uniform: the ray whose dZ1 sum vbc carries (-1: none)
+
   const int64_t n_units = (n_pts + kUnit - 1) / kUnit;
-  for (int64_t u = (int64_t)blockIdx.x * kWarps + warp; u < n_units; u += (int64_t)gridDim.x * kWarps) {
+  const int64_t n_warps = (int64_t)gridDim.x * kWarps, wid = (int64_t)blockIdx.x * kWarps + warp;
+  const int64_t u_end = n_units * (wid + 1) / n_warps;
+  for (int64_t u = n_units * wid / n_warps; u < u_end; ++u) {
     const int64_t r0 = u * kUnit;
     const int64_t row[2] = {r0 + g, r0 + g + 8};
     const bool live[2] = {row[0] < n_pts, row[1] < n_pts};
@@ -329,8 +400,7 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc(
     }
     if (!kDz1Out) {
       __syncwarp();
-      // dW3 = dz3^T . H2 and E = dz3^T . [H2 > 0] (db2 = sum_i W3[i] * E[i]): A rows 0..2 = dz3^T, sample = k
-      uint32_t ah[4], al[4];
+      // dW3 = dz3^T . H2 and E = dz3^T . [H2 > 0]: A rows 0..2 = dz3^T, sample = k
       {
         // a0 = A[g][t], a1 = A[g + 8][t], a2 = A[g][t + 4], a3 = A[g + 8][t + 4]; A[i][k] = dz3 of sample k (rows >= 3: 0)
         // dz3 of sample k lives in lane (g = k % 8, any t) as dz3[k / 8][.]
@@ -348,32 +418,36 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc(
           }
           av[s][0] = a[0]; av[s][1] = a[1]; av[s][2] = a[2]; av[s][3] = a[3];
         }
-        float dW3a[kNT][4], Ea[kNT][4];
+        uint32_t ah[2][4], al[2][4];
 #pragma unroll
-        for (int j = 0; j < kNT; ++j) dW3a[j][0] = dW3a[j][1] = dW3a[j][2] = dW3a[j][3] = Ea[j][0] = Ea[j][1] = Ea[j][2] = Ea[j][3] = 0.f;
+        for (int s = 0; s < 2; ++s) split4(av[s], ah[s], al[s]);
 #pragma unroll
-        for (int s = 0; s < 2; ++s) {
-          split4(av[s], ah, al);
+        for (int jh = 0; jh < 2; ++jh) {                     // two halves of the column tiles: 64 accumulators live, not 128
+          constexpr int kH = kNT / 2;
+          float dW3a[kH][4], Ea[kH][4];
 #pragma unroll
-          for (int j = 0; j < kNT; ++j) {
-            uint32_t bh[2], bl[2];
-            tile_frag(S, s, j, g, t, bh, bl);
-            mma3<kThree>(dW3a[j], ah, al, make_uint4(bh[0], bh[1], bl[0], bl[1]));
-            const uint32_t one = 0x3f800000u;
-            const uint32_t mb0 = __uint_as_float(bh[0]) + __uint_as_float(bl[0]) > 0.f ? one : 0u;
-            const uint32_t mb1 = __uint_as_float(bh[1]) + __uint_as_float(bl[1]) > 0.f ? one : 0u;
-            if (kThree) mma_tf32(Ea[j], al, mb0, mb1);
-            mma_tf32(Ea[j], ah, mb0, mb1);
+          for (int jj = 0; jj < kH; ++jj) dW3a[jj][0] = dW3a[jj][1] = dW3a[jj][2] = dW3a[jj][3] = Ea[jj][0] = Ea[jj][1] = Ea[jj][2] = Ea[jj][3] = 0.f;
+#pragma unroll
+          for (int s = 0; s < 2; ++s) {
+#pragma unroll
+            for (int jj = 0; jj < kH; ++jj) {
+              uint32_t bh[2], bl[2];
+              tile_frag(S, s, kH * jh + jj, g, t, bh, bl);
+              mma3<kThree>(dW3a[jj], ah[s], al[s], make_uint4(bh[0], bh[1], bl[0], bl[1]));
+              const uint32_t one = 0x3f800000u;
+              const uint32_t mb0 = __uint_as_float(bh[0]) + __uint_as_float(bl[0]) > 0.f ? one : 0u;
+              const uint32_t mb1 = __uint_as_float(bh[1]) + __uint_as_float(bl[1]) > 0.f ? one : 0u;
+              if (kThree) mma_tf32(Ea[jj], al[s], mb0, mb1);
+              mma_tf32(Ea[jj], ah[s], mb0, mb1);
+            }
           }
-        }
-        if (g < 3) {
+          if (g < 3) {
 #pragma unroll
-          for (int j = 0; j < kNT; ++j) {
-            const int c = 8 * j + 2 * t;
-            atomicAdd(accW3 + g * kHidden + c, dW3a[j][0]);
-            atomicAdd(accW3 + g * kHidden + c + 1, dW3a[j][1]);
-            atomicAdd(accB2 + c, sW3[g * kHidden + c] * Ea[j][0]);
-            atomicAdd(accB2 + c + 1, sW3[g * kHidden + c + 1] * Ea[j][1]);
+            for (int jj = 0; jj < kH; ++jj) {
+              const int c = 8 * (kH * jh + jj) + 2 * t;
+              sum_add2(sumW3 + g * kStride + c, dW3a[jj][0], dW3a[jj][1]);
+              sum_add2(sumE + g * kStride + c, Ea[jj][0], Ea[jj][1]);
+            }
           }
         }
 #pragma unroll
@@ -382,7 +456,7 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc(
           s3 += __shfl_xor_sync(0xffffffffu, s3, 4);
           s3 += __shfl_xor_sync(0xffffffffu, s3, 8);
           s3 += __shfl_xor_sync(0xffffffffu, s3, 16);
-          if (lane == i) atomicAdd(accB3 + i, s3);
+          if (lane == i) db3 += s3;
         }
       }
       __syncwarp();
@@ -391,7 +465,7 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc(
     float d1[kNT][4];
 #pragma unroll
     for (int j = 0; j < kNT; ++j) d1[j][0] = d1[j][1] = d1[j][2] = d1[j][3] = 0.f;
-    warp_gemm<kNT, kNT, kThree>(d1, d2, fW2, lane);
+    warp_gemm_f<kNT, kNT, kThree>(d1, d2, fW2, lane);
     // dZ1 = dH1 * [H1 > 0]
     if (kMask1) {
 #pragma unroll
@@ -429,7 +503,7 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc(
     // dX = dZ1 . W1k
     {
       float dx[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-      warp_gemm<kNT, 2, kThree>(dx, d1, fW1T, lane);
+      warp_gemm_f<kNT, 2, kThree>(dx, d1, fW1T, lane);
 #pragma unroll
       for (int j = 0; j < 2; ++j)
 #pragma unroll
@@ -443,7 +517,8 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc(
     const int64_t my_ray = (lane < kUnit && r0 + lane < n_pts) ? ray_id[r0 + lane] : -1;
     const int64_t prev_ray = __shfl_up_sync(0xffffffffu, my_ray, 1);
     const uint32_t starts = __ballot_sync(0xffffffffu, lane < kUnit && my_ray >= 0 && (lane == 0 || prev_ray != my_ray));
-    const bool segs_fit = __popc(starts) <= 4;
+    const int nseg = __popc(starts);                          // >= 1: sample r0 is live
+    const bool segs_fit = nseg <= 4;
     {
       float acc[kNT][4];
 #pragma unroll
@@ -477,73 +552,123 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc(
 #pragma unroll
       for (int j = 0; j < kNT; ++j) {
         const int c = 8 * j + 2 * t;
-        atomicAdd(accW1 + g * kHidden + c, acc[j][0]);
-        atomicAdd(accW1 + g * kHidden + c + 1, acc[j][1]);
-        if (g < 4) {
-          atomicAdd(accW1 + (g + 8) * kHidden + c, acc[j][2]);
-          atomicAdd(accW1 + (g + 8) * kHidden + c + 1, acc[j][3]);
-        }
+        sum_add2(sumW1 + g * kStride + c, acc[j][0], acc[j][1]);
+        if (g < 4) sum_add2(sumW1 + (g + 8) * kStride + c, acc[j][2], acc[j][3]);
       }
-      // ray of segment q = the ray of its first sample (every lane shuffles: warp-uniform)
-      int64_t seg_ray[4];
-      {
-        uint32_t m = starts;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int src = m ? __ffs(m) - 1 : 0;
-          seg_ray[q] = __shfl_sync(0xffffffffu, my_ray, src);
-          if (!m) seg_ray[q] = -1;
-          m &= m - 1;
-        }
-      }
-      if (segs_fit && g >= 4) {
-        const int64_t ray = seg_ray[g - 4];
-        if (ray >= 0) {
+      // rays of the unit's first and last segment, and (lanes g = 4 + q) of segment q
+      const int64_t first_ray = __shfl_sync(0xffffffffu, my_ray, __ffs(starts) - 1);
+      const int64_t last_ray = __shfl_sync(0xffffffffu, my_ray, 31 - __clz(starts));
+      uint32_t above = starts;                                // drop the first g - 4 starts
+      for (int q = 0; q < g - 4; ++q) above &= above - 1;
+      const int64_t seg_ray = __shfl_sync(0xffffffffu, my_ray, above ? __ffs(above) - 1 : 0);
+      if (segs_fit) {
+        const bool cont = first_ray == open_ray;
+        if (g == 4) {
+          if (!cont && open_ray >= 0) emit_ray(grad_view_bias, open_ray, vbc, t);    // the carried ray ended with the last unit
 #pragma unroll
           for (int j = 0; j < kNT; ++j) {
-            atomicAdd(grad_view_bias + ray * kHidden + 8 * j + 2 * t, acc[j][2]);
-            atomicAdd(grad_view_bias + ray * kHidden + 8 * j + 2 * t + 1, acc[j][3]);
+            float* v = vbc + 8 * j + 2 * t;
+            const float2 o = cont ? *reinterpret_cast<const float2*>(v) : make_float2(0.f, 0.f);
+            *reinterpret_cast<float2*>(v) = make_float2(o.x + acc[j][2], o.y + acc[j][3]);
+          }
+          if (nseg > 1) emit_ray(grad_view_bias, first_ray, vbc, t);                 // segment 0 ends inside this unit
+        }
+        if (nseg > 1) {
+          if (g > 4 && g - 4 < nseg - 1) {                   // inner segments
+#pragma unroll
+            for (int j = 0; j < kNT; ++j) red_add2(grad_view_bias + seg_ray * kHidden + 8 * j + 2 * t, acc[j][2], acc[j][3]);
+          }
+          __syncwarp();                                       // lanes g == 4 have read vbc
+          if (g == 3 + nseg) {                                // the last segment stays open
+#pragma unroll
+            for (int j = 0; j < kNT; ++j) *reinterpret_cast<float2*>(vbc + 8 * j + 2 * t) = make_float2(acc[j][2], acc[j][3]);
           }
         }
+        open_ray = last_ray;
       }
     }
     if (!segs_fit) {                                          // more than 4 rays in 16 samples: per-sample adds
+      if (open_ray >= 0 && g == 4) emit_ray(grad_view_bias, open_ray, vbc, t);
+      open_ray = -1;
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         if (!live[r]) continue;
         const int64_t ray = ray_id[row[r]];
 #pragma unroll
-        for (int j = 0; j < kNT; ++j) {
-          atomicAdd(grad_view_bias + ray * kHidden + 8 * j + 2 * t, d1[j][2 * r]);
-          atomicAdd(grad_view_bias + ray * kHidden + 8 * j + 2 * t + 1, d1[j][2 * r + 1]);
-        }
+        for (int j = 0; j < kNT; ++j) red_add2(grad_view_bias + ray * kHidden + 8 * j + 2 * t, d1[j][2 * r], d1[j][2 * r + 1]);
       }
     }
     __syncwarp();
   }
   if (kDz1Out) return;
+  if (open_ray >= 0 && g == 4) emit_ray(grad_view_bias, open_ray, vbc, t);
+  if (lane < 3) atomicAdd(grad_b3 + lane, db3);
   __syncthreads();
-  for (int i = tid; i < kFeat * kHidden; i += kThreads) {        // accW1 is dW1k^T: [feature][unit]
+  // the warps' running sums, added in warp order, go to global once per CTA
+  const float* sums = reinterpret_cast<const float*>(smem + bk::oWarp + bk::kTileBytes);
+  auto warp_sum = [&](int r, int c) {
+    float v = 0.f;
+#pragma unroll
+    for (int w = 0; w < kWarps; ++w) v += sums[w * (bk::kWarpBytes / 4) + r * kStride + c];
+    return v;
+  };
+  for (int i = tid; i < kFeat * kHidden; i += kThreads) {        // row f of the sums is column f of dW1k
     const int f = i / kHidden, c = i % kHidden;
-    atomicAdd(grad_W1k + c * kFeat + f, accW1[i]);
+    atomicAdd(grad_W1k + c * kFeat + f, warp_sum(f, c));
   }
-  for (int i = tid; i < 3 * kHidden; i += kThreads) atomicAdd(grad_W3 + i, accW3[i]);
-  for (int i = tid; i < kHidden; i += kThreads) atomicAdd(grad_b2 + i, accB2[i]);
-  if (tid < 3) atomicAdd(grad_b3 + tid, accB3[tid]);
+  for (int i = tid; i < 3 * kHidden; i += kThreads) atomicAdd(grad_W3 + i, warp_sum(kFeat + i / kHidden, i % kHidden));
+  for (int c = tid; c < kHidden; c += kThreads) {
+    float v = 0.f;
+#pragma unroll
+    for (int i = 0; i < 3; ++i) v += sW3[i * kHidden + c] * warp_sum(kFeat + 3 + i, c);
+    atomicAdd(grad_b2 + c, v);
+  }
 }
 
 // ---- backward, launch 2: dW2 += dZ2^T . H1 -------------------------------------------------------------------------------
-// A split-K GEMM over samples: each CTA takes 32-sample chunks, stages dZ2 (rebuilt from dz3, W3 and H2 or its ReLU masks) and
-// H1 as [32][kStride] tiles, and warp w accumulates output rows 16 w .. 16 w + 15.  The MMA accumulator restarts every chunk
-// and is added into an fp32 running sum, so the tensor core never carries a long accumulation chain.
+// A split-K GEMM over samples: each CTA takes 32-sample chunks, stages dZ2 (rebuilt from dz3, W3 and H2 or its ReLU masks) as a
+// [32][kStride] fp32 tile and H1 as a [32][kStrideB] tile of ready-split {hi, lo} pairs (split once per element, not once per
+// warp), and warp w accumulates output rows 16 w .. 16 w + 15.  The tiles are double-buffered and each thread loads the next
+// chunk's rows into registers before the MMAs of the current one, so the HBM reads overlap the tensor cores and one barrier
+// per chunk suffices.  The MMA accumulator restarts every chunk and is added into an fp32 running sum, so the tensor core
+// never carries a long accumulation chain.
 namespace dw {
 constexpr int kThreads = 256;
 constexpr int kK = 32;
+constexpr int kStrideB = kHidden + 4;                      // uint2 per element: conflict-free fragment reads
 constexpr uint32_t oW3 = 0;
-constexpr uint32_t oA = oW3 + 3 * kHidden * 4;
-constexpr uint32_t oB = oA + kK * kStride * 4;
-constexpr uint32_t kSmem = oB + kK * kStride * 4;
+constexpr uint32_t kBufA = kK * kStride * 4;
+constexpr uint32_t kBuf = kBufA + kK * kStrideB * 8;
+constexpr uint32_t oBuf = oW3 + 3 * kHidden * 4;
+constexpr uint32_t kSmem = oBuf + 2 * kBuf;
 }  // namespace dw
+
+// one thread's share of a chunk (sample row r, columns 32 q + 4 (tid & 7) .. + 3), straight from global memory
+struct Dw2Rows {
+  float4 h1[4], h2[4];
+  uint32_t m2[4];
+  float y[3], gy[3];
+};
+
+template <bool kPanel, bool kMask2>
+__device__ __forceinline__ void dw2_load(Dw2Rows& d, const float* __restrict__ rgb, const float* __restrict__ h1_save,
+                                         const float* __restrict__ h2_save, const uint32_t* __restrict__ h2_mask,
+                                         const float* __restrict__ grad_rgb, int64_t r, int64_t n_pts, int c0) {
+  const bool ok = r < n_pts;
+  const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    d.y[i] = ok ? rgb[r * 3 + i] : 0.f;
+    d.gy[i] = ok ? grad_rgb[r * 3 + i] : 0.f;
+  }
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int c = 32 * q + c0;
+    d.h1[q] = ok ? *reinterpret_cast<const float4*>(h1_save + save_idx<kPanel>(r, c)) : zero;
+    if (kMask2) d.m2[q] = ok ? h2_mask[mask_idx(r, q)] : 0u;
+    else d.h2[q] = ok ? *reinterpret_cast<const float4*>(h2_save + save_idx<kPanel>(r, c)) : zero;
+  }
+}
 
 template <bool kThree, bool kPanel, bool kMask2>
 __global__ void __launch_bounds__(dw::kThreads, 1) k_shade_dw2_tc(
@@ -553,53 +678,49 @@ __global__ void __launch_bounds__(dw::kThreads, 1) k_shade_dw2_tc(
   extern __shared__ __align__(16) uint8_t smem[];
   const int tid = threadIdx.x, lane = tid & 31, g = lane >> 2, t = lane & 3, warp = tid >> 5;
   float* sW3 = reinterpret_cast<float*>(smem + dw::oW3);
-  float* sA = reinterpret_cast<float*>(smem + dw::oA);    // dZ2 [sample][unit]
-  float* sB = reinterpret_cast<float*>(smem + dw::oB);    // H1  [sample][unit]
   for (int i = tid; i < 3 * kHidden; i += dw::kThreads) sW3[i] = W3[i];
   float sum[kNT][4];
 #pragma unroll
   for (int j = 0; j < kNT; ++j) sum[j][0] = sum[j][1] = sum[j][2] = sum[j][3] = 0.f;
-  const int sr = tid >> 3;                                 // staging: sample row, 4 float4 column groups per thread
+  const int sr = tid >> 3, c0 = 4 * (tid & 7);             // staging: sample row, 4 float4 column groups per thread
   const int64_t n_chunks = (n_pts + dw::kK - 1) / dw::kK;
-  for (int64_t ch = blockIdx.x; ch < n_chunks; ch += gridDim.x) {
-    __syncthreads();                                       // previous chunk's fragment reads done (and sW3 staged)
-    const int64_t r = ch * dw::kK + sr;
-    const bool ok = r < n_pts;
-    float dz3[3] = {0.f, 0.f, 0.f};
-    if (ok) {
+  Dw2Rows d;
+  int64_t ch = blockIdx.x;
+  if (ch < n_chunks) dw2_load<kPanel, kMask2>(d, rgb, h1_save, h2_save, h2_mask, grad_rgb, ch * dw::kK + sr, n_pts, c0);
+  __syncthreads();                                         // sW3 staged
+  for (int buf = 0; ch < n_chunks; ch += gridDim.x, buf ^= 1) {
+    float* sA = reinterpret_cast<float*>(smem + dw::oBuf + buf * dw::kBuf);                // dZ2 [sample][unit]
+    uint2* sB = reinterpret_cast<uint2*>(smem + dw::oBuf + buf * dw::kBuf + dw::kBufA);   // H1 {hi, lo} [sample][unit]
+    float dz3[3];
 #pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        const float y = rgb[r * 3 + i];
-        dz3[i] = grad_rgb[r * 3 + i] * y * (1.f - y);
-      }
-    }
+    for (int i = 0; i < 3; ++i) dz3[i] = d.gy[i] * d.y[i] * (1.f - d.y[i]);
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
-      const int c = 32 * q + 4 * (tid & 7);
-      float4 h1 = make_float4(0.f, 0.f, 0.f, 0.f), d = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (ok) {
-        h1 = *reinterpret_cast<const float4*>(h1_save + save_idx<kPanel>(r, c));
-        float hv[4];
-        if (kMask2) {
-          const uint32_t w = h2_mask[mask_idx(r, c >> 5)] >> (c & 31);
+      const int c = 32 * q + c0;
+      float hv[4];
+      if (kMask2) {
+        const uint32_t w = d.m2[q] >> c0;
 #pragma unroll
-          for (int e = 0; e < 4; ++e) hv[e] = ((w >> e) & 1u) ? 1.f : 0.f;
-        } else {
-          const float4 h2 = *reinterpret_cast<const float4*>(h2_save + save_idx<kPanel>(r, c));
-          hv[0] = h2.x; hv[1] = h2.y; hv[2] = h2.z; hv[3] = h2.w;
-        }
-        float dv[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float dh = dz3[0] * sW3[c + e] + dz3[1] * sW3[kHidden + c + e] + dz3[2] * sW3[2 * kHidden + c + e];
-          dv[e] = hv[e] > 0.f ? dh : 0.f;
-        }
-        d = make_float4(dv[0], dv[1], dv[2], dv[3]);
+        for (int e = 0; e < 4; ++e) hv[e] = ((w >> e) & 1u) ? 1.f : 0.f;
+      } else {
+        hv[0] = d.h2[q].x; hv[1] = d.h2[q].y; hv[2] = d.h2[q].z; hv[3] = d.h2[q].w;
       }
-      *reinterpret_cast<float4*>(sA + sr * kStride + c) = d;
-      *reinterpret_cast<float4*>(sB + sr * kStride + c) = h1;
+      float dv[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float dh = dz3[0] * sW3[c + e] + dz3[1] * sW3[kHidden + c + e] + dz3[2] * sW3[2 * kHidden + c + e];
+        dv[e] = hv[e] > 0.f ? dh : 0.f;
+      }
+      *reinterpret_cast<float4*>(sA + sr * kStride + c) = make_float4(dv[0], dv[1], dv[2], dv[3]);
+      const float hb[4] = {d.h1[q].x, d.h1[q].y, d.h1[q].z, d.h1[q].w};
+      uint32_t hi[4], lo[4];
+      split4(hb, hi, lo);
+      *reinterpret_cast<uint4*>(sB + sr * dw::kStrideB + c) = make_uint4(hi[0], lo[0], hi[1], lo[1]);
+      *reinterpret_cast<uint4*>(sB + sr * dw::kStrideB + c + 2) = make_uint4(hi[2], lo[2], hi[3], lo[3]);
     }
-    __syncthreads();
+    __syncthreads();                                       // this buffer is complete; the other one is no longer read
+    if (ch + gridDim.x < n_chunks)
+      dw2_load<kPanel, kMask2>(d, rgb, h1_save, h2_save, h2_mask, grad_rgb, (ch + gridDim.x) * dw::kK + sr, n_pts, c0);
     float acc[kNT][4];
 #pragma unroll
     for (int j = 0; j < kNT; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
@@ -612,9 +733,8 @@ __global__ void __launch_bounds__(dw::kThreads, 1) k_shade_dw2_tc(
       split4(av, ah, al);
 #pragma unroll
       for (int j = 0; j < kNT; ++j) {
-        uint32_t bh[2], bl[2];
-        tile_frag(sB, s, j, g, t, bh, bl);
-        mma3<kThree>(acc[j], ah, al, make_uint4(bh[0], bh[1], bl[0], bl[1]));
+        const uint2 b0 = sB[(8 * s + t) * dw::kStrideB + 8 * j + g], b1 = sB[(8 * s + t + 4) * dw::kStrideB + 8 * j + g];
+        mma3<kThree>(acc[j], ah, al, make_uint4(b0.x, b1.x, b0.y, b1.y));
       }
     }
 #pragma unroll
