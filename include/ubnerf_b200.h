@@ -262,6 +262,11 @@ int ubn_count_gt(const float* grad, float thres, int64_t n, float* count, void* 
  * linspace(-1, 1, size) per axis, cams [n_cams, 3] device array already in the slab's (embedded, flipped) coordinates. */
 int ubn_maskout_near_cam(float* slab, int64_t voxel_stride, int64_t X, int64_t Y, int64_t Z, const float* cams, int64_t n_cams,
                          float near_clip, float fill, void* stream);
+/* maskout_near_cam_vox of DirectVoxGO (dvgo.py:185-198): as above on the lattice linspace(lattice_min[a], lattice_max[a], size)
+ * (HOST float[3] arrays; the world bbox there), cams [n_cams, 3] device array in world coordinates. */
+int ubn_maskout_near_cam_lattice(float* slab, int64_t voxel_stride, int64_t X, int64_t Y, int64_t Z, const float* lattice_min,
+                                 const float* lattice_max, const float* cams, int64_t n_cams, float near_clip, float fill,
+                                 void* stream);
 
 /* ---- fused ray march: sample_ray + density query + Raw2Alpha + Alphas2Weights + thresholds + k0 query
  *      for FourierGridModel.forward (FourierGrid_model.py:509-621) and DirectContractedVoxGO.forward
@@ -405,6 +410,52 @@ int ubn_march_ndc_feature_bwd(const float* rays_o, const float* rays_d, const Ub
  * act_shift gets no gradient (requires_grad = False, dmpigo.py:50). */
 int ubn_march_ndc_density_bwd(const float* rays_o, const float* rays_d, const UbnGridDesc* density_desc,
                               const UbnNdcMarchCfg* cfg, int64_t n_rays, const float* density, const float* alpha,
+                              const float* weight, const float* T, const uint8_t* flags, const float* alphainv_last,
+                              const int64_t* offsets, const float* g_weight, const float* g_alpha, const float* g_last,
+                              float* grad_density_grid, void* stream);
+
+/* ---- fused box march for the bounded-scene model DirectVoxGO.forward (FourierGrid/dvgo.py:306-397): sample_pts_on_rays +
+ *      in-box drop + mask cache + density + Raw2Alpha + Alphas2Weights + both thresholds + k0 query.  Same three-launch forward
+ *      (pass A, ubn_exclusive_scan_i32, pass B) and two-launch backward as the contracted march, the same per-sample records and
+ *      flag bits (UBN_FLAG_INNER is never set).  Records are [n_rays * s_max]; ray r fills its first n_steps(r) of them only. ---- */
+typedef struct UbnBoxMarchCfg {
+  /* scene bbox: the AABB of render_utils_kernel.cu:12-79 (t_min / t_max) and the inclusive in-box test of :191-192 */
+  float xyz_min[3];
+  float xyz_max[3];
+  float near;                   /* t clamp (render_utils_kernel.cu:37-38); far is 1e9 as dvgo.py:321 sets it */
+  float stepdist;               /* stepsize * voxel_size (dvgo.py:324); sample i = start + dir * (stepdist * i) (:185-190) */
+  int32_t s_max;                /* record stride: a host bound on n_steps = max(ceil((t_max - t_min) * |d| / stepdist), 1) (:53).
+                                   A ray with more steps sets *overflow in pass A, it is never truncated silently. <= 4096 */
+  float act_shift;              /* Raw2Alpha shift (dvgo.py:60, 357) */
+  float interval;               /* stepsize * voxel_size_ratio (dvgo.py:347) */
+  float fast_color_thres;       /* <= 0: no thresholding (dvgo.py:358-375) */
+  int32_t use_maskcache;        /* dvgo.py:350-354: the lookup comes before the density query */
+  int32_t mask_sz[3];           /* MaskGrid geometry (grid.py:223-242): mask dims, xyz2ijk_scale, xyz2ijk_shift */
+  float mask_scale[3];
+  float mask_shift[3];
+} UbnBoxMarchCfg;
+
+/* Pass A: density = density_grid(p) (single-slab C = 1 grid), alpha = Raw2Alpha(density, act_shift, interval), the exact sequential
+ * transmittance scan and both thresholds; outputs as ubn_march_density_fwd.  overflow: device int32 the caller zeroes; set to 1 when
+ * some ray's n_steps exceeds s_max (that ray is clamped to s_max samples and the caller must treat the result as an error). */
+int ubn_march_box_density_fwd(const float* rays_o, const float* rays_d, const float* density_grid, const UbnGridDesc* density_desc,
+                              const uint8_t* mask_world, const UbnBoxMarchCfg* cfg, int64_t n_rays, float* density, float* alpha,
+                              float* weight, float* T, uint8_t* flags, float* alphainv_last, int32_t* n_keep, int32_t* overflow,
+                              void* stream);
+/* Pass B: for every survivor, in (ray, step) order at offsets[ray] + rank, the k0 read (F.grid_sample arithmetic, bit-identical)
+ * and the compacted records alpha, weight, ray_id, step_id (step_id = the ray's own step index).  k0: single-slab channels-last
+ * grid with C = 12 (16-byte aligned) or C = 3; k0_feat 16-byte aligned; out_alpha / out_weight may be NULL. */
+int ubn_march_box_feature_fwd(const float* rays_o, const float* rays_d, const float* k0_grid, const UbnGridDesc* k0_desc,
+                              const UbnBoxMarchCfg* cfg, int64_t n_rays, const uint8_t* flags, const int64_t* offsets,
+                              const float* alpha, const float* weight, float* k0_feat, float* out_alpha, float* out_weight,
+                              int64_t* ray_id, int64_t* step_id, void* stream);
+/* Backward of pass B: grad_k0 += adjoint of the k0 read applied to grad_feat[M,C]. */
+int ubn_march_box_feature_bwd(const float* rays_o, const float* rays_d, const UbnGridDesc* k0_desc, const UbnBoxMarchCfg* cfg,
+                              int64_t n_rays, const uint8_t* flags, const int64_t* offsets, const float* grad_feat,
+                              float* grad_k0, void* stream);
+/* Backward of pass A: exact reverse scan -> raw2alpha_backward -> scatter into the density-grid gradient. */
+int ubn_march_box_density_bwd(const float* rays_o, const float* rays_d, const UbnGridDesc* density_desc,
+                              const UbnBoxMarchCfg* cfg, int64_t n_rays, const float* density, const float* alpha,
                               const float* weight, const float* T, const uint8_t* flags, const float* alphainv_last,
                               const int64_t* offsets, const float* g_weight, const float* g_alpha, const float* g_last,
                               float* grad_density_grid, void* stream);

@@ -39,6 +39,12 @@ class UbnNdcMarchCfg(ctypes.Structure):
                 ('use_maskcache', c_i32), ('mask_sz', c_i32 * 3), ('mask_scale', c_f * 3), ('mask_shift', c_f * 3)]
 
 
+class UbnBoxMarchCfg(ctypes.Structure):
+    _fields_ = [('xyz_min', c_f * 3), ('xyz_max', c_f * 3), ('near', c_f), ('stepdist', c_f), ('s_max', c_i32), ('act_shift', c_f),
+                ('interval', c_f), ('fast_color_thres', c_f), ('use_maskcache', c_i32), ('mask_sz', c_i32 * 3),
+                ('mask_scale', c_f * 3), ('mask_shift', c_f * 3)]
+
+
 ABI_VERSION = 3          # UBN_ABI_VERSION of include/ubnerf_b200.h this binding was written against
 FLAG_QUERIED, FLAG_LISTED, FLAG_SCANNED, FLAG_KEEP, FLAG_INNER = 1, 2, 4, 8, 16
 
@@ -81,6 +87,7 @@ _SIGNATURES = {
     'ubn_view_scatter_ones': [c_p, c_p, c_i64, c_i64, c_f, c_f, c_f, ctypes.POINTER(UbnGridDesc), c_p, c_p],
     'ubn_count_gt': [c_p, c_f, c_i64, c_p, c_p],
     'ubn_maskout_near_cam': [c_p, c_i64, c_i64, c_i64, c_i64, c_p, c_i64, c_f, c_f, c_p],
+    'ubn_maskout_near_cam_lattice': [c_p, c_i64, c_i64, c_i64, c_i64, c_p, c_p, c_p, c_i64, c_f, c_f, c_p],
     'ubn_cumdist_thres': [c_p, c_f, c_i64, c_i64, c_p, c_p],
     'ubn_get_rays_of_a_view': [c_int, c_int, c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_int, c_p, c_p, c_p, c_p, c_p],
     'ubn_gather_rays': [c_p, c_p, c_int, c_p, c_i64, c_i64, c_p, c_p],
@@ -112,6 +119,14 @@ _SIGNATURES = {
     'ubn_march_ndc_feature_bwd': [c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnNdcMarchCfg), c_i64,
                                   c_p, c_p, c_p, c_p, c_p],
     'ubn_march_ndc_density_bwd': [c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnNdcMarchCfg), c_i64,
+                                  c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
+    'ubn_march_box_density_fwd': [c_p, c_p, c_p, ctypes.POINTER(UbnGridDesc), c_p, ctypes.POINTER(UbnBoxMarchCfg), c_i64,
+                                  c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
+    'ubn_march_box_feature_fwd': [c_p, c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnBoxMarchCfg), c_i64,
+                                  c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
+    'ubn_march_box_feature_bwd': [c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnBoxMarchCfg), c_i64,
+                                  c_p, c_p, c_p, c_p, c_p],
+    'ubn_march_box_density_bwd': [c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnBoxMarchCfg), c_i64,
                                   c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
 }
 _RESTYPE = {'ubn_last_error_string': ctypes.c_char_p, 'ubn_launch_count': c_i64, 'ubn_reset_launch_count': None}

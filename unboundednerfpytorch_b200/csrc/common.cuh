@@ -42,6 +42,69 @@ __device__ __forceinline__ void ndc_point(float ox, float oy, float oz, float dx
   z = fmaf(dz, dist, oz);
 }
 
+// ---- bounded-scene sampling (render_utils_kernel.cu:12-79,167-194) -----------------------------------------------------------
+// Shared by ubn_infer_* / ubn_sample_pts_* (ray_ops.cu) and the fused box march (BoxSampler, march_common.cuh), so both produce the
+// same bits.  The expressions are kept as the reference writes them: nvcc's default fma contraction then lands on the same operations.
+struct RayBox {
+  float t_min, t_max;
+};
+
+__device__ __forceinline__ RayBox ray_aabb(const float* __restrict__ o, const float* __restrict__ d,
+                                           const float* __restrict__ xyz_min,
+                                           const float* __restrict__ xyz_max, float near, float far) {
+  // zero direction components become 1e-6 (double literal narrowed to float), :23-25
+  const float vx = (d[0] == 0) ? (float)1e-6 : d[0];
+  const float vy = (d[1] == 0) ? (float)1e-6 : d[1];
+  const float vz = (d[2] == 0) ? (float)1e-6 : d[2];
+  const float ax = (xyz_max[0] - o[0]) / vx;
+  const float ay = (xyz_max[1] - o[1]) / vy;
+  const float az = (xyz_max[2] - o[2]) / vz;
+  const float bx = (xyz_min[0] - o[0]) / vx;
+  const float by = (xyz_min[1] - o[1]) / vy;
+  const float bz = (xyz_min[2] - o[2]) / vz;
+  RayBox r;
+  r.t_min = fmaxf(fminf(fmaxf(fmaxf(fminf(ax, bx), fminf(ay, by)), fminf(az, bz)), far), near);
+  r.t_max = fmaxf(fminf(fminf(fminf(fmaxf(ax, bx), fmaxf(ay, by)), fmaxf(az, bz)), far), near);
+  return r;
+}
+
+__device__ __forceinline__ float ray_norm(const float* __restrict__ d) {
+  return sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+}
+
+__device__ __forceinline__ int64_t ray_n_samples(const float* __restrict__ d, float t_min, float t_max,
+                                                 float stepdist) {
+  const float rnorm = ray_norm(d);
+  // max(ceil(float), 1.) is evaluated in double in the reference (:53)
+  return (int64_t)fmax((double)ceilf((t_max - t_min) * rnorm / stepdist), 1.);
+}
+
+// rays_start = o + d * t_min and rays_dir = d / |d|, each rounded to float as K3 writes them to memory (:72-77)
+__device__ __forceinline__ void ray_start_dir(const float* __restrict__ o, const float* __restrict__ d, float t_min, float* start,
+                                              float* dir) {
+  const float rnorm = ray_norm(d);
+  start[0] = o[0] + d[0] * t_min;
+  start[1] = o[1] + d[1] * t_min;
+  start[2] = o[2] + d[2] * t_min;
+  dir[0] = d[0] / rnorm;
+  dir[1] = d[1] / rnorm;
+  dir[2] = d[2] / rnorm;
+}
+
+// sample i of a bounded-scene ray: p = start + dir * (stepdist * i)   (:185-190)
+__device__ __forceinline__ void box_point(const float* start, const float* dir, float stepdist, int i, float& x, float& y,
+                                          float& z) {
+  const float dist = stepdist * i;
+  x = start[0] + dir[0] * dist;
+  y = start[1] + dir[1] * dist;
+  z = start[2] + dir[2] * dist;
+}
+
+// the reference's inclusive in-box test: a sample is dropped when (min > p) | (max < p) on any axis (:191-192)
+__device__ __forceinline__ bool outside_box(const float* mn, const float* mx, float x, float y, float z) {
+  return (mn[0] > x) | (mn[1] > y) | (mn[2] > z) | (mx[0] < x) | (mx[1] < y) | (mx[2] < z);
+}
+
 }  // namespace ubn
 
 #define UBN_LAUNCH_CHECK()                 \

@@ -121,15 +121,17 @@ __global__ void __launch_bounds__(256) k_count_gt(const float* __restrict__ grad
   if (i < n && grad[i] > thres) count[i] += 1.f;
 }
 
-// maskout_near_cam_vox: grid[idx] = fill where the nearest camera (in the slab's embedded coordinates) is within near_clip of the
-// lattice point linspace(-1, 1, size) -- distances as torch evaluates (g - c).pow(2).sum(-1).sqrt() on 3-vectors
-__global__ void __launch_bounds__(256) k_maskout_near_cam(float* __restrict__ slab, int64_t sv, int X, int Y, int Z,
+// maskout_near_cam_vox: grid[idx] = fill where the nearest camera is within near_clip of the lattice point linspace(lo, hi, size)
+// per axis -- [-1, 1] in a FourierGrid slab's embedded coordinates, [xyz_min, xyz_max] for DVGO's world lattice -- distances as
+// torch evaluates (g - c).pow(2).sum(-1).sqrt() on 3-vectors
+__global__ void __launch_bounds__(256) k_maskout_near_cam(float* __restrict__ slab, int64_t sv, int X, int Y, int Z, float lox,
+                                                          float loy, float loz, float hix, float hiy, float hiz,
                                                           const float* __restrict__ cams, int n_cams, float near_clip, float fill) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t n = (int64_t)X * Y * Z;
   if (idx >= n) return;
   const int k = (int)(idx % Z), j = (int)((idx / Z) % Y), i = (int)(idx / ((int64_t)Z * Y));
-  const float gx = linspace_at(-1.f, 1.f, X, i), gy = linspace_at(-1.f, 1.f, Y, j), gz = linspace_at(-1.f, 1.f, Z, k);
+  const float gx = linspace_at(lox, hix, X, i), gy = linspace_at(loy, hiy, Y, j), gz = linspace_at(loz, hiz, Z, k);
   float best = INFINITY;
   for (int c = 0; c < n_cams; ++c) {
     const float ex = __fsub_rn(gx, cams[3 * c]), ey = __fsub_rn(gy, cams[3 * c + 1]), ez = __fsub_rn(gz, cams[3 * c + 2]);
@@ -201,8 +203,20 @@ int ubn_maskout_near_cam(float* slab, int64_t voxel_stride, int64_t X, int64_t Y
                          float near_clip, float fill, void* stream) {
   const int64_t n = X * Y * Z;
   if (n <= 0 || n_cams <= 0) return 0;
-  k_maskout_near_cam<<<blocks_for(n, 256), 256, 0, as_stream(stream)>>>(slab, voxel_stride, (int)X, (int)Y, (int)Z, cams, (int)n_cams,
-                                                                        near_clip, fill);
+  k_maskout_near_cam<<<blocks_for(n, 256), 256, 0, as_stream(stream)>>>(slab, voxel_stride, (int)X, (int)Y, (int)Z, -1.f, -1.f, -1.f,
+                                                                        1.f, 1.f, 1.f, cams, (int)n_cams, near_clip, fill);
+  UBN_LAUNCH_CHECK();
+  return 0;
+}
+
+int ubn_maskout_near_cam_lattice(float* slab, int64_t voxel_stride, int64_t X, int64_t Y, int64_t Z, const float* lattice_min,
+                                 const float* lattice_max, const float* cams, int64_t n_cams, float near_clip, float fill,
+                                 void* stream) {
+  const int64_t n = X * Y * Z;
+  if (n <= 0 || n_cams <= 0) return 0;
+  k_maskout_near_cam<<<blocks_for(n, 256), 256, 0, as_stream(stream)>>>(slab, voxel_stride, (int)X, (int)Y, (int)Z, lattice_min[0],
+                                                                        lattice_min[1], lattice_min[2], lattice_max[0], lattice_max[1],
+                                                                        lattice_max[2], cams, (int)n_cams, near_clip, fill);
   UBN_LAUNCH_CHECK();
   return 0;
 }

@@ -19,6 +19,7 @@
 // are evaluated in the reference's sequential order (a warp-uniform loop over the lanes) so that the
 // index-like outputs (which samples are listed / scanned / kept) stay bit-exact.
 #include <algorithm>
+#include <type_traits>
 
 #include "march_common.cuh"
 
@@ -42,7 +43,8 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_fwd(
   const int64_t ray = (int64_t)blockIdx.x * kMarchWarps + (threadIdx.x >> 5);
   if (ray >= n_rays) return;
   const Ray r = Smp::load(rays_o + 3 * ray, rays_d + 3 * ray, p);
-  const int S = p.S;
+  const int S = p.S;      // record stride
+  const int n = r.n;      // samples of this ray (warp-uniform): S, or the box march's n_steps
 
   float T_cum = 1.f;      // warp-uniform
   bool done = false;      // warp-uniform: early stop reached
@@ -50,9 +52,9 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_fwd(
   bool carry_over = false;   // cumdist flag for the first sample of the next chunk
   int n_keep = 0;
 
-  for (int base = 0; base < S; base += 32) {
+  for (int base = 0; base < n; base += 32) {
     const int s = base + lane;
-    const bool valid = s < S;
+    const bool valid = s < n;
     float x = 0, y = 0, z = 0;
     bool inner = false, in_domain = false;
     if (valid) in_domain = Smp::point(r, t_table, s, p, x, y, z, inner);
@@ -262,16 +264,17 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_bwd(
   const int64_t ray = (int64_t)blockIdx.x * kMarchWarps + w;
   if (ray >= n_rays) return;
   const Ray r = Smp::load(rays_o + 3 * ray, rays_d + 3 * ray, p);
-  const int S = p.S;
-  const int n_chunks = (S + 31) / 32;
-  const int L = n_chunks;                                  // kRuns: consecutive samples per lane in phase 2 (= ceil(S / 32))
-  float* s_gd = s_gd_all + w * (S + 33);
+  const int S = p.S;                                       // record stride
+  const int n = r.n;                                       // samples of this ray (S, or the box march's n_steps)
+  const int n_chunks = (n + 31) / 32;
+  const int L = n_chunks;                                  // kRuns: consecutive samples per lane in phase 2 (= ceil(n / 32))
+  float* s_gd = s_gd_all + w * (S + 33);                   // index s + s / L < n + 32 <= S + 33
 
   // exclusive prefix of KEEP counts per chunk -> compact index of every kept sample
   int run = 0;
   for (int c = 0; c < n_chunks; ++c) {
     const int s = c * 32 + lane;
-    const bool keep = (s < S) && (flags[ray * S + s] & UBN_FLAG_KEEP);
+    const bool keep = (s < n) && (flags[ray * S + s] & UBN_FLAG_KEEP);
     const unsigned km = __ballot_sync(0xffffffffu, keep);
     if (lane == 0) s_cnt[w][c] = run;
     run += __popc(km);
@@ -282,7 +285,7 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_bwd(
   float back_cum = (g_last ? g_last[ray] : 0.f) * last[ray];   // warp-uniform
   for (int c = n_chunks - 1; c >= 0; --c) {
     const int s = c * 32 + lane;
-    const bool valid = s < S;
+    const bool valid = s < n;
     const int64_t i = ray * S + s;
     const uint8_t f = valid ? flags[i] : 0;
     const bool keep = f & UBN_FLAG_KEEP;
@@ -398,7 +401,7 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_bwd(
     const float m = (float)(1 << (k > 0 ? k - 1 : 0));
     for (int i = 0; i < L; ++i) {
       const int s = lane * L + i;
-      if (s >= S) break;
+      if (s >= n) break;
       const float gd = s_gd[s + lane];
       if (gd == 0.f) continue;
       float x, y, z;
@@ -457,13 +460,18 @@ static int launch_density_fwd(const float* rays_o, const float* rays_d, const fl
 #define UBN_DFWD(P)                                                                                              \
   k_march_density_fwd<Smp, P><<<blocks_for(n_rays, kMarchWarps), 32 * kMarchWarps, 0, st>>>(                   \
       rays_o, rays_d, t_table, g, mask_world, p, n_rays, density, alpha, weight, T, flags, alphainv_last, n_keep)
-  switch (density_fast_slabs(g)) {
-    case 1: UBN_DFWD(1); break;
-    case 3: UBN_DFWD(3); break;
-    case 5: UBN_DFWD(5); break;
-    case 7: UBN_DFWD(7); break;
-    case 9: UBN_DFWD(9); break;
-    default: UBN_DFWD(0); break;
+  if constexpr (std::is_same<Smp, BoxSampler>::value) {      // DVGO's density: one contiguous slab, the fast path only
+    if (density_fast_slabs(g) != 1) return finish(cudaErrorInvalidValue);
+    UBN_DFWD(1);
+  } else {
+    switch (density_fast_slabs(g)) {
+      case 1: UBN_DFWD(1); break;
+      case 3: UBN_DFWD(3); break;
+      case 5: UBN_DFWD(5); break;
+      case 7: UBN_DFWD(7); break;
+      case 9: UBN_DFWD(9); break;
+      default: UBN_DFWD(0); break;
+    }
   }
 #undef UBN_DFWD
   UBN_LAUNCH_CHECK();
@@ -490,13 +498,18 @@ static int launch_density_bwd(const float* rays_o, const float* rays_d, const fl
           rays_o, rays_d, t_table, g, p, n_rays, density, alpha, weight, T, flags, alphainv_last, offsets, g_weight,  \
           g_alpha, g_density, g_last, grad_density_grid);                                                            \
   } while (0)
-  switch (density_fast_slabs(g)) {
-    case 1: UBN_DBWD(1); break;
-    case 3: UBN_DBWD(3); break;
-    case 5: UBN_DBWD(5); break;
-    case 7: UBN_DBWD(7); break;
-    case 9: UBN_DBWD(9); break;
-    default: UBN_DBWD(0); break;
+  if constexpr (std::is_same<Smp, BoxSampler>::value) {
+    if (density_fast_slabs(g) != 1) return finish(cudaErrorInvalidValue);
+    UBN_DBWD(1);
+  } else {
+    switch (density_fast_slabs(g)) {
+      case 1: UBN_DBWD(1); break;
+      case 3: UBN_DBWD(3); break;
+      case 5: UBN_DBWD(5); break;
+      case 7: UBN_DBWD(7); break;
+      case 9: UBN_DBWD(9); break;
+      default: UBN_DBWD(0); break;
+    }
   }
 #undef UBN_DBWD
   UBN_LAUNCH_CHECK();
@@ -624,6 +637,35 @@ int ubn_march_ndc_density_bwd(const float* rays_o, const float* rays_d, const Ub
   if (p.S > 32 * kMaxChunks) return finish(cudaErrorInvalidValue);
   return launch_density_bwd<NdcSampler>(rays_o, rays_d, nullptr, g, p, n_rays, density, alpha, weight, T, flags, alphainv_last,
                                          offsets, g_weight, g_alpha, nullptr, g_last, grad_density_grid, as_stream(stream));
+}
+
+// S_max (cfg->s_max) is the record stride of pass A; the backward's chunk table holds 32 * kMaxChunks samples of a ray
+static bool box_cfg_ok(const UbnBoxMarchCfg* c) { return c->s_max >= 1 && c->s_max <= 32 * kMaxChunks && c->stepdist > 0.f; }
+
+int ubn_march_box_density_fwd(const float* rays_o, const float* rays_d, const float* density_grid, const UbnGridDesc* density_desc,
+                              const uint8_t* mask_world, const UbnBoxMarchCfg* cfg, int64_t n_rays, float* density, float* alpha,
+                              float* weight, float* T, uint8_t* flags, float* alphainv_last, int32_t* n_keep, int32_t* overflow,
+                              void* stream) {
+  if (n_rays <= 0) return 0;
+  const GridView g = make_view(density_grid, density_desc);
+  if (g.C != 1 || g.P != 1 || !box_cfg_ok(cfg) || !overflow) return finish(cudaErrorInvalidValue);
+  const MarchParams p = make_box_params(cfg, overflow);
+  if (p.use_mask && !mask_world) return finish(cudaErrorInvalidValue);
+  return launch_density_fwd<BoxSampler>(rays_o, rays_d, nullptr, g, mask_world, p, n_rays, density, alpha, weight, T, flags,
+                                        alphainv_last, n_keep, as_stream(stream));
+}
+
+int ubn_march_box_density_bwd(const float* rays_o, const float* rays_d, const UbnGridDesc* density_desc,
+                              const UbnBoxMarchCfg* cfg, int64_t n_rays, const float* density, const float* alpha,
+                              const float* weight, const float* T, const uint8_t* flags, const float* alphainv_last,
+                              const int64_t* offsets, const float* g_weight, const float* g_alpha, const float* g_last,
+                              float* grad_density_grid, void* stream) {
+  if (n_rays <= 0) return 0;
+  const GridView g = make_view(grad_density_grid, density_desc);
+  if (g.C != 1 || g.P != 1 || !box_cfg_ok(cfg)) return finish(cudaErrorInvalidValue);
+  const MarchParams p = make_box_params(cfg, nullptr);
+  return launch_density_bwd<BoxSampler>(rays_o, rays_d, nullptr, g, p, n_rays, density, alpha, weight, T, flags, alphainv_last,
+                                        offsets, g_weight, g_alpha, nullptr, g_last, grad_density_grid, as_stream(stream));
 }
 
 }  // extern "C"

@@ -17,6 +17,8 @@ struct MarchParams {
   float mscale[3], mshift[3];
   float bmin[3], bmax[3];         // NDC march: samples outside this box (strict comparisons) are dropped
   GridView shift_grid;            // NDC march: the act_shift DenseGrid, added to the raw density
+  float near, stepdist;           // box march: t_min clamp and the step length of a sample
+  int* overflow;                  // box march, pass A: set to 1 when a ray needs more than S steps (else NULL)
 };
 
 inline MarchParams make_params(const UbnMarchCfg* c) {
@@ -49,7 +51,8 @@ inline MarchParams make_ndc_params(const UbnNdcMarchCfg* c, const GridView& shif
 }
 
 struct Ray {
-  float ox, oy, oz, dx, dy, dz;   // normalised origin, unit direction
+  float ox, oy, oz, dx, dy, dz;   // normalised origin, unit direction (box march: rays_start, rays_dir)
+  int n;                          // samples of this ray: S, or the box march's own n_steps (<= S)
 };
 
 // ||v|| exactly as torch's CUDA reduction evaluates x.norm(dim=-1) on 3-vectors: the lanes of the reduced
@@ -71,6 +74,7 @@ __device__ __forceinline__ Ray load_ray(const float* __restrict__ o, const float
   r.dx = __fdiv_rn(d[0], n);
   r.dy = __fdiv_rn(d[1], n);
   r.dz = __fdiv_rn(d[2], n);
+  r.n = p.S;
   return r;
 }
 
@@ -110,10 +114,11 @@ struct ContractedSampler {      // FourierGrid_model.py:509-552, dcvgo.py:228-26
 };
 
 struct NdcSampler {             // dmpigo.py:224-249, 275: NDC point inside the strict bbox; density + act_shift(p)
-  __device__ static Ray load(const float* o, const float* d, const MarchParams&) {
+  __device__ static Ray load(const float* o, const float* d, const MarchParams& p) {
     Ray r;
     r.ox = o[0]; r.oy = o[1]; r.oz = o[2];
     r.dx = d[0]; r.dy = d[1]; r.dz = d[2];
+    r.n = p.S;
     return r;
   }
   __device__ static bool point(const Ray& r, const float*, int s, const MarchParams& p, float& x, float& y, float& z,
@@ -128,6 +133,48 @@ struct NdcSampler {             // dmpigo.py:224-249, 275: NDC point inside the 
     return __fadd_rn(d, grid_density_at(p.shift_grid, x, y, z));
   }
 };
+
+struct BoxSampler {             // dvgo.py:306-328, render_utils_kernel.cu:12-79,167-194: start + dir * (stepdist * s), s < n_steps
+  // t_min / t_max from the AABB (near clamp, far = 1e9 as sample_ray sets it), n_steps, start and dir with the very functions
+  // ubn_sample_pts_* use (common.cuh).  n_steps > S (the host's S_max) raises p.overflow and is clamped so no record is out of range.
+  __device__ static Ray load(const float* o, const float* d, const MarchParams& p) {
+    const RayBox b = ray_aabb(o, d, p.bmin, p.bmax, p.near, 1e9f);
+    const int64_t n = ray_n_samples(d, b.t_min, b.t_max, p.stepdist);
+    float start[3], dir[3];
+    ray_start_dir(o, d, b.t_min, start, dir);
+    Ray r;
+    r.ox = start[0]; r.oy = start[1]; r.oz = start[2];
+    r.dx = dir[0]; r.dy = dir[1]; r.dz = dir[2];
+    r.n = (int)min(n, (int64_t)p.S);
+    if (n > p.S && p.overflow) *p.overflow = 1;
+    return r;
+  }
+  __device__ static bool point(const Ray& r, const float*, int s, const MarchParams& p, float& x, float& y, float& z,
+                               bool& inner) {
+    const float start[3] = {r.ox, r.oy, r.oz}, dir[3] = {r.dx, r.dy, r.dz};
+    box_point(start, dir, p.stepdist, s, x, y, z);
+    inner = false;
+    return !outside_box(p.bmin, p.bmax, x, y, z);
+  }
+  __device__ static float density(const MarchParams&, float d, float, float, float) { return d; }
+};
+
+// DirectVoxGO (dvgo.py:330-397): no contraction, no cumdist; Raw2Alpha with the scalar act_shift; mask cache before the density
+inline MarchParams make_box_params(const UbnBoxMarchCfg* c, int* overflow) {
+  MarchParams p{};
+  p.S = c->s_max;
+  p.shift = c->act_shift; p.interval = c->interval; p.thres = c->fast_color_thres;
+  p.use_cumdist = 0;
+  p.use_mask = c->use_maskcache;
+  for (int a = 0; a < 3; ++a) {
+    p.msz[a] = c->mask_sz[a]; p.mscale[a] = c->mask_scale[a]; p.mshift[a] = c->mask_shift[a];
+    p.bmin[a] = c->xyz_min[a]; p.bmax[a] = c->xyz_max[a];
+  }
+  p.near = c->near;
+  p.stepdist = c->stepdist;
+  p.overflow = overflow;
+  return p;
+}
 
 struct CellR {
   int v;            // base voxel index  (x0*Y + y0)*Z + z0, pre-clamped

@@ -1,7 +1,7 @@
 """Fused ray march (autograd.Function) over the C ABI: the hot path of FourierGridModel.forward
 (FourierGrid_model.py:554-621) and DirectContractedVoxGO.forward (dcvgo.py:264-331) -- ``March`` -- and of
-DirectMPIGO.forward (dmpigo.py:251-295) -- ``NdcMarch`` -- up to and including the feature-grid read, in 3 launches
-forward (pass A, scan, pass B) and 2 backward.  Both share the dense pass-A records, the compaction and the
+DirectMPIGO.forward (dmpigo.py:251-295) -- ``NdcMarch`` -- and of DirectVoxGO.forward (dvgo.py:330-366) -- ``BoxMarch`` --
+up to and including the feature-grid read, in 3 launches forward (pass A, scan, pass B) and 2 backward.  All share the dense pass-A records, the compaction and the
 gradient-buffer plumbing below.
 """
 import functools
@@ -277,3 +277,119 @@ class NdcMarch(torch.autograd.Function):
         grad_d = _hand_over(ctx.dparam, grad_d, buf_d)
         grad_k = _hand_over(ctx.kparam, grad_k, buf_k)
         return grad_d, grad_k, None, None, None, None, None, None, None, None
+
+
+def box_s_max(xyz_min, xyz_max, stepdist):
+    """Record stride of the box march: a host bound on every ray's n_steps = max(ceil((t_max - t_min) * |d| / stepdist), 1).
+    (t_max - t_min) * |d| is the length of the ray's chord through the box (a zero direction component is replaced by 1e-6,
+    which only lengthens the direction the slabs see, so |d| under-measures that chord), and a chord through a box is at most
+    its diagonal.  The margin of 4 steps covers the fp32 rounding of t_min, t_max and the product.  A ray beyond it (a camera
+    ~1e7 box lengths away) is reported by pass A, never truncated."""
+    diag = float(np.linalg.norm(np.asarray(xyz_max, dtype=np.float64) - np.asarray(xyz_min, dtype=np.float64)))
+    return int(np.ceil(diag / float(np.float32(stepdist)))) + 4
+
+
+BOX_S_MAX_LIMIT = 4096     # the backward's per-ray chunk table
+
+
+def make_box_cfg(xyz_min, xyz_max, near, stepdist, act_shift, interval, fast_color_thres, mask, mask_scale, mask_shift):
+    c = _cabi.UbnBoxMarchCfg()
+    for a in range(3):
+        c.xyz_min[a] = float(xyz_min[a])
+        c.xyz_max[a] = float(xyz_max[a])
+    c.near = float(near)
+    c.stepdist = float(stepdist)
+    c.s_max = box_s_max(xyz_min, xyz_max, stepdist)
+    if c.s_max > BOX_S_MAX_LIMIT:
+        raise ValueError(f'the box march bounds a ray at {BOX_S_MAX_LIMIT} steps; this bbox / stepsize needs {c.s_max}')
+    c.act_shift = float(act_shift)
+    c.interval = float(interval)
+    c.fast_color_thres = float(fast_color_thres)
+    c.use_maskcache = 1 if mask is not None else 0
+    if mask is not None:
+        for a in range(3):
+            c.mask_sz[a] = int(mask.shape[a])
+            c.mask_scale[a] = float(mask_scale[a])
+            c.mask_shift[a] = float(mask_shift[a])
+    return c
+
+
+def box_supported(density_grid, k0_grid):
+    """Grids the fused box march covers: a contiguous single-slab density grid and a single-slab channels-last k0 with 3 or 12
+    channels (16-byte aligned records for 12), >= 2 voxels per axis, 32-bit voxel offsets."""
+    return (density_grid.is_cuda and k0_grid.is_cuda and density_grid.dim() == 5 and density_grid.shape[:2] == (1, 1)
+            and density_grid.is_contiguous() and min(density_grid.shape[2:]) >= 2 and density_grid.numel() < 2 ** 31
+            and k0_grid.dim() == 5 and k0_grid.shape[0] == 1 and k0_grid.shape[1] in (3, 12) and k0_grid.stride(1) == 1
+            and k0_grid.stride(4) == k0_grid.shape[1] and min(k0_grid.shape[2:]) >= 2 and k0_grid[0, 0].numel() < 2 ** 31
+            and (k0_grid.shape[1] != 12 or k0_grid.data_ptr() % 16 == 0))
+
+
+class BoxMarch(torch.autograd.Function):
+    """DirectVoxGO's march: (density_grid, k0_grid, rays) -> compacted per-survivor records sorted by (ray, step).
+
+    Returns (weights[M], alphainv_last[N], raw_alpha[M], k0_feat[M,C], ray_id[M] i64, step_id[M] i64); step_id is the ray's own
+    step index.  Differentiable wrt density_grid and k0_grid.  A ray needing more than cfg.s_max steps raises."""
+
+    @staticmethod
+    def forward(ctx, density_grid, k0_grid, rays_o, rays_d, mask_world, cfg, ddesc, kdesc):
+        dev = rays_o.device
+        rays_o = rays_o.contiguous().float()
+        rays_d = rays_d.contiguous().float()
+        N, S = rays_o.shape[0], cfg.s_max
+        f32 = dict(dtype=torch.float32, device=dev)
+        dens, alpha, weight, T, flags, last, nkeep = _pass_a_buffers(N, S, dev)
+        overflow = torch.zeros(1, dtype=torch.int32, device=dev)
+        with ops._Guard(rays_o) as lib:
+            st = stream_of(rays_o)
+            with _cabi.timed('march_box_density_fwd'):
+                check(lib.ubn_march_box_density_fwd(ptr(rays_o), ptr(rays_d), ptr(density_grid), ddesc, ptr(mask_world), cfg,
+                                                    c_i64(N), ptr(dens), ptr(alpha), ptr(weight), ptr(T), ptr(flags), ptr(last),
+                                                    ptr(nkeep), ptr(overflow), st))
+            offsets, _ = _compact(lib, nkeep, N, S, True, st)
+            # the march's one device-to-host read: the survivor count and the overflow word together
+            M, over = torch.stack([offsets[N], overflow[0].to(torch.int64)]).tolist() if N > 0 else (0, 0)
+            if over:
+                raise RuntimeError(f'box march: a ray needs more than s_max = {S} steps (bbox / stepsize / ray origin out of range)')
+            feat = torch.empty(M, k0_grid.shape[1], **f32)
+            o_alpha = torch.empty(M, **f32)
+            o_weight = torch.empty(M, **f32)
+            ray_id = torch.empty(M, dtype=torch.int64, device=dev)
+            step_id = torch.empty(M, dtype=torch.int64, device=dev)
+            with _cabi.timed('march_box_feature_fwd'):
+                check(lib.ubn_march_box_feature_fwd(ptr(rays_o), ptr(rays_d), ptr(k0_grid), kdesc, cfg, c_i64(N), ptr(flags),
+                                                    ptr(offsets), ptr(alpha), ptr(weight), ptr(feat), ptr(o_alpha), ptr(o_weight),
+                                                    ptr(ray_id), ptr(step_id), st))
+        ctx.save_for_backward(rays_o, rays_d, dens, alpha, weight, T, flags, last, offsets)
+        ctx.cfg, ctx.ddesc, ctx.kdesc = cfg, ddesc, kdesc
+        ctx.dmeta = (density_grid.shape, density_grid.stride())
+        ctx.kmeta = (k0_grid.shape, k0_grid.stride())
+        ctx.dparam, ctx.kparam = density_grid, k0_grid
+        ctx.mark_non_differentiable(ray_id, step_id)
+        return o_weight, last, o_alpha, feat, ray_id, step_id
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_weight, g_last, g_alpha, g_feat, *unused):
+        rays_o, rays_d, dens, alpha, weight, T, flags, last, offsets = ctx.saved_tensors
+        dev = rays_o.device
+        N = rays_o.shape[0]
+        cont = lambda g: g.contiguous() if g is not None else None
+        g_weight, g_last, g_alpha, g_feat = map(cont, (g_weight, g_last, g_alpha, g_feat))
+        with ops._Guard(rays_o) as lib:
+            st = stream_of(rays_o)
+            want_k = ctx.needs_input_grad[1] and g_feat is not None
+            want_d = ctx.needs_input_grad[0]
+            grad_d, buf_d = _grad_target(ctx.dparam, ctx.dmeta, want_d, dev)
+            grad_k, buf_k = _grad_target(ctx.kparam, ctx.kmeta, want_k, dev)
+            if want_k:
+                with _cabi.timed('march_box_feature_bwd'):
+                    check(lib.ubn_march_box_feature_bwd(ptr(rays_o), ptr(rays_d), ctx.kdesc, ctx.cfg, c_i64(N), ptr(flags),
+                                                        ptr(offsets), ptr(g_feat), ptr(grad_k), st))
+            if want_d:
+                with _cabi.timed('march_box_density_bwd'):
+                    check(lib.ubn_march_box_density_bwd(ptr(rays_o), ptr(rays_d), ctx.ddesc, ctx.cfg, c_i64(N), ptr(dens),
+                                                        ptr(alpha), ptr(weight), ptr(T), ptr(flags), ptr(last), ptr(offsets),
+                                                        ptr(g_weight), ptr(g_alpha), ptr(g_last), ptr(grad_d), st))
+        grad_d = _hand_over(ctx.dparam, grad_d, buf_d)
+        grad_k = _hand_over(ctx.kparam, grad_k, buf_k)
+        return grad_d, grad_k, None, None, None, None, None, None

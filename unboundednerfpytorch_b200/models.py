@@ -185,6 +185,51 @@ def _occupancy_update(model, density, mask_cache, interval):
     ops.maxpool3_gt_and_(mask_cache.mask, alpha, model.fast_color_thres)
 
 
+@torch.no_grad()
+def _scale_dense_model(model, num_voxels):
+    """scale_volume_grid of the DenseGrid models (dcvgo.py:196-212, dvgo.py:213-234): new resolution, both grids resampled, and
+    -- up to 256^3 voxels -- the mask cache rebuilt on the new lattice as mask(lattice) & (max_pool3d(alpha(density)) > thres)."""
+    model._set_grid_resolution(num_voxels)
+    model.density.scale_volume_grid(model.world_size)
+    model.k0.scale_volume_grid(model.world_size)
+    if np.prod(model.world_size.tolist()) <= 256 ** 3:
+        dev = model.density.grid.device
+        ws = [int(v) for v in model.world_size]
+        axes = [torch.linspace(float(model.xyz_min[a]), float(model.xyz_max[a]), ws[a], device=dev) for a in range(3)]
+        xyz = torch.stack(torch.meshgrid(*axes, indexing='ij'), -1)
+        alpha = F.max_pool3d(model.activate_density(model.density.get_dense_grid().contiguous()), kernel_size=3,
+                             padding=1, stride=1)[0, 0]
+        model.mask_cache = G.MaskGrid(path=None, mask=model.mask_cache(xyz) & (alpha > model.fast_color_thres),
+                                      xyz_min=model.xyz_min, xyz_max=model.xyz_max).to(dev)
+        model._mask_host = None
+
+
+@torch.no_grad()
+def _count_views(density, world_size, voxel_size, rays_o_tr, rays_d_tr, imsz, near, stepsize, downrate, irregular_shape):
+    """voxel_count_views (FourierGrid_model.py:390-420, dvgo.py:238-277): per-voxel number of training views that see it.  The
+    reference materialises the sample points of 10 000 rays at a time and runs DenseGrid(ones).sum().backward(); here one kernel
+    per view scatters the trilinear weights of every (ray, sample) straight into a per-view buffer, a second adds (buffer > 1) to
+    the count.  far is 1e9 as the reference sets it."""
+    from . import ops
+    far = 1e9
+    dev = density.grid.device
+    ws = [int(v) for v in world_size]
+    n_samples = int(np.linalg.norm(np.array(ws) + 1) / stepsize) + 1
+    step = float(stepsize * voxel_size)
+    mn, mx = density._bounds()
+    count = torch.zeros(1, 1, *ws, device=dev)
+    buf = torch.empty(*ws, device=dev)
+    for rays_o_, rays_d_ in zip(rays_o_tr.split(imsz), rays_d_tr.split(imsz)):
+        if not irregular_shape:
+            rays_o_, rays_d_ = rays_o_[::downrate, ::downrate], rays_d_[::downrate, ::downrate]
+        ro = rays_o_.to(dev).reshape(-1, 3).contiguous().float()
+        rd = rays_d_.to(dev).reshape(-1, 3).contiguous().float()
+        buf.zero_()
+        ops.view_scatter_ones(ro, rd, mn, mx, ws, n_samples, near, far, step, buf)
+        ops.count_gt_(count, buf, 1.0)
+    return count
+
+
 # ======================================================================================================
 class FourierGridModel(_ContractedBase):
     """FourierGrid/FourierGrid_model.py:134-681."""
@@ -312,27 +357,9 @@ class FourierGridModel(_ContractedBase):
             ops.maskout_near_cam_(self.density.grid.data[i][0], cam.reshape(-1, 3), near_clip, -100.0)
 
     def voxel_count_views(self, rays_o_tr, rays_d_tr, imsz, near, far, stepsize, downrate=1, irregular_shape=False):
-        """FourierGrid_model.py:390-420: per-voxel number of training views that see it.  The reference materialises the sample
-        points of 10 000 rays at a time and runs DenseGrid(ones).sum().backward(); here one kernel per view scatters the
-        trilinear weights of every (ray, sample) straight into a per-view buffer, a second adds (buffer > 1) to the count."""
-        from . import ops
-        far = 1e9
-        dev = self.density.grid.device
-        ws = [int(v) for v in self.world_size_density]
-        n_samples = int(np.linalg.norm(np.array(ws) + 1) / stepsize) + 1
-        step = float(stepsize * self.voxel_size_density)
-        mn, mx = self.density._bounds()
-        count = torch.zeros(1, 1, *ws, device=dev)
-        buf = torch.empty(*ws, device=dev)
-        for rays_o_, rays_d_ in zip(rays_o_tr.split(imsz), rays_d_tr.split(imsz)):
-            if not irregular_shape:
-                rays_o_, rays_d_ = rays_o_[::downrate, ::downrate], rays_d_[::downrate, ::downrate]
-            ro = rays_o_.to(dev).reshape(-1, 3).contiguous().float()
-            rd = rays_d_.to(dev).reshape(-1, 3).contiguous().float()
-            buf.zero_()
-            ops.view_scatter_ones(ro, rd, mn, mx, ws, n_samples, near, far, step, buf)
-            ops.count_gt_(count, buf, 1.0)
-        return count
+        """FourierGrid_model.py:390-420 (see _count_views)."""
+        return _count_views(self.density, self.world_size_density, self.voxel_size_density, rays_o_tr, rays_d_tr, imsz, near,
+                            stepsize, downrate, irregular_shape)
 
     def hit_coarse_geo(self, rays_o, rays_d, near, far, stepsize, **render_kwargs):
         """FourierGrid_model.py:495-507: does a ray hit the occupancy mask?"""
@@ -477,21 +504,8 @@ class DirectContractedVoxGO(_ContractedBase):
             'k0_config': self.k0_config, **self.rgbnet_kwargs,
         }
 
-    @torch.no_grad()
     def scale_volume_grid(self, num_voxels):
-        self._set_grid_resolution(num_voxels)
-        self.density.scale_volume_grid(self.world_size)
-        self.k0.scale_volume_grid(self.world_size)
-        if np.prod(self.world_size.tolist()) <= 256 ** 3:
-            dev = self.density.grid.device
-            ws = [int(v) for v in self.world_size]
-            axes = [torch.linspace(float(self.xyz_min[a]), float(self.xyz_max[a]), ws[a], device=dev) for a in range(3)]
-            xyz = torch.stack(torch.meshgrid(*axes, indexing='ij'), -1)
-            alpha = F.max_pool3d(self.activate_density(self.density.get_dense_grid().contiguous()), kernel_size=3,
-                                 padding=1, stride=1)[0, 0]
-            self.mask_cache = G.MaskGrid(path=None, mask=self.mask_cache(xyz) & (alpha > self.fast_color_thres),
-                                         xyz_min=self.xyz_min, xyz_max=self.xyz_max).to(dev)
-            self._mask_host = None
+        _scale_dense_model(self, num_voxels)
 
     @torch.no_grad()
     def update_occupancy_cache(self):
@@ -573,8 +587,19 @@ class DirectContractedVoxGO(_ContractedBase):
 
 # ======================================================================================================
 class DirectVoxGO(nn.Module):
-    """Bounded-scene model (FourierGrid/dvgo.py:26-425): ragged AABB sampling (sample_pts_on_rays) instead of the
-    contracted schedule; depth = sum w * step_id.  Composed from the drop-in ops (BASELINE config 1 family)."""
+    """Bounded-scene model (FourierGrid/dvgo.py:26-425): ragged AABB sampling (sample_pts_on_rays) instead of the contracted
+    schedule; depth = sum w * step_id.  ``forward`` runs the fused box march (march.BoxMarch: pass A, scan, pass B; one host read
+    of the survivor count) with the rgb from ``_shade`` -- the tensor-core rgbnet when shade.supported (the default fine config:
+    rgbnet_dim 12, rgbnet_direct, width 128) -- for a single-slab density and a 3- or 12-channel channels-last k0.  With
+    rgbnet_direct=False the march is fused and the torch epilogue sigmoid(rgbnet(cat[k0[:, 3:], emb]) + k0[:, :3]) stays.
+    ``forward_ops`` composes the drop-in ops in the reference's order (the cross-check and the path for other grids).
+
+    The coarse-to-fine schedule of run_train.py works: maskout_near_cam_vox, voxel_count_views (per-voxel lr), scale_volume_grid,
+    update_occupancy_cache, and ``mask_cache_path``.  The latter builds the fine mask as the reference does (dvgo.py:138-152):
+    MaskGrid(path, mask_cache_thres) looked up on this model's linspace(xyz_min, xyz_max, mask_cache_world_size) lattice.  The
+    lookup is a CUDA kernel, so a model built on the host (run_train.create_new_model constructs, then calls .to(device)) resolves
+    it when it first moves to a CUDA device; a state dict that carries ``mask_cache.mask`` (a checkpoint of the fine model)
+    supersedes it, so ckpt.load_model never reads the coarse file."""
 
     def __init__(self, xyz_min, xyz_max, num_voxels=0, num_voxels_base=0, alpha_init=None, mask_cache_path=None,
                  mask_cache_thres=1e-3, mask_cache_world_size=None, fast_color_thres=0, density_type='DenseGrid',
@@ -607,11 +632,46 @@ class DirectVoxGO(nn.Module):
         self.mask_cache_path, self.mask_cache_thres = mask_cache_path, mask_cache_thres
         if mask_cache_world_size is None:
             mask_cache_world_size = self.world_size
-        if mask_cache_path:
-            raise NotImplementedError('coarse-checkpoint mask cache needs a device at construction; build MaskGrid(path=...) '
-                                      'and assign model.mask_cache instead')
+        self._pending_mask = None
+        self._mask_host = None
         self.mask_cache = G.MaskGrid(path=None, mask=torch.ones([int(v) for v in mask_cache_world_size], dtype=torch.bool),
                                      xyz_min=self.xyz_min, xyz_max=self.xyz_max)
+        if mask_cache_path:
+            self._pending_mask = (mask_cache_path, mask_cache_thres, [int(v) for v in mask_cache_world_size])
+            if self.xyz_min.is_cuda:
+                self._resolve_mask_cache()
+
+    # ---- the coarse-checkpoint mask cache (dvgo.py:138-152) ----------------------------------------------------------------
+    @torch.no_grad()
+    def _resolve_mask_cache(self):
+        path, thres, ws = self._pending_mask
+        dev = self.xyz_min.device
+        coarse = G.MaskGrid(path=path, mask_cache_thres=thres).to(dev)
+        axes = [torch.linspace(float(self.xyz_min[a]), float(self.xyz_max[a]), ws[a], device=dev) for a in range(3)]
+        xyz = torch.stack(torch.meshgrid(*axes, indexing='ij'), -1)
+        self.mask_cache = G.MaskGrid(path=None, mask=coarse(xyz), xyz_min=self.xyz_min, xyz_max=self.xyz_max).to(dev)
+        self._pending_mask = None
+        self._mask_host = None
+
+    def _apply(self, fn, *a, **k):
+        self._mask_host = None
+        out = super()._apply(fn, *a, **k)
+        if self._pending_mask is not None and self.xyz_min.is_cuda:
+            self._resolve_mask_cache()
+        return out
+
+    def _load_from_state_dict(self, state_dict, prefix, *a, **k):
+        self._mask_host = None
+        if prefix + 'mask_cache.mask' in state_dict:
+            self._pending_mask = None
+        return super()._load_from_state_dict(state_dict, prefix, *a, **k)
+
+    def _mask_geometry(self):
+        if self._mask_host is None or self._mask_host[0] is not self.mask_cache:
+            self._mask_host = (self.mask_cache, self.mask_cache.xyz2ijk_scale.cpu().tolist(),
+                               self.mask_cache.xyz2ijk_shift.cpu().tolist(), self.xyz_min.cpu().tolist(),
+                               self.xyz_max.cpu().tolist())
+        return self._mask_host[1:]
 
     def _set_grid_resolution(self, num_voxels):
         self.num_voxels = num_voxels
@@ -628,6 +688,31 @@ class DirectVoxGO(nn.Module):
             'density_type': self.density_type, 'k0_type': self.k0_type, 'density_config': self.density_config,
             'k0_config': self.k0_config, **self.rgbnet_kwargs,
         }
+
+    # ---- grid maintenance (run_train.py's coarse and fine stages) -------------------------------------------------------------
+    def scale_volume_grid(self, num_voxels):
+        """dvgo.py:213-234 (the pg_scale steps of the fine stage)."""
+        _scale_dense_model(self, num_voxels)
+
+    @torch.no_grad()
+    def update_occupancy_cache(self):
+        """dvgo.py:236-246: mask &= max_pool3d(Raw2Alpha(density(mask lattice))) > fast_color_thres (ops.lattice_alpha +
+        ops.maxpool3_gt_and_)."""
+        _occupancy_update(self, self.density, self.mask_cache, float(self.voxel_size_ratio))
+
+    def voxel_count_views(self, rays_o_tr, rays_d_tr, imsz, near, far, stepsize, downrate=1, irregular_shape=False):
+        """dvgo.py:248-277 (see _count_views): feeds MaskedAdam.set_pervoxel_lr and the coarse stage's mask update."""
+        return _count_views(self.density, self.world_size, self.voxel_size, rays_o_tr, rays_d_tr, imsz, near, stepsize, downrate,
+                            irregular_shape)
+
+    @torch.no_grad()
+    def maskout_near_cam_vox(self, cam_o, near_clip):
+        """dvgo.py:185-198: density = -100 at the points of the world lattice linspace(xyz_min, xyz_max, world_size) that are
+        within near_clip of a camera position (one kernel: every voxel scans the camera list)."""
+        from . import ops
+        lo, hi = self.xyz_min.cpu().tolist(), self.xyz_max.cpu().tolist()
+        cams = cam_o.to(self.density.grid.device).reshape(-1, 3)
+        ops.maskout_near_cam_(self.density.grid.data[0][0], cams, near_clip, -100.0, lattice=(lo, hi))
 
     def activate_density(self, density, interval=None):
         interval = interval if interval is not None else self.voxel_size_ratio
@@ -674,7 +759,54 @@ class DirectVoxGO(nn.Module):
         hit[ray_id[mask_inbbox][self.mask_cache(ray_pts[mask_inbbox])]] = 1
         return hit.reshape(shape)
 
+    # ---- rendering ------------------------------------------------------------------------------------------------------------
+    def _stepdist(self, stepsize):
+        # what sample_ray hands ubn_sample_pts_* (the same fp32 value reaches the march); host_scalar caches the read per tensor,
+        # so a device-side voxel_size (after scale_volume_grid on a CUDA model) costs one sync per rescale, not per step
+        return stepsize * host_scalar(self.voxel_size)
+
+    def _fused_ok(self, stepsize):
+        if not march.box_supported(self.density.grid, self.k0.grid):
+            return False
+        _, _, lo, hi = self._mask_geometry()
+        return march.box_s_max(lo, hi, self._stepdist(stepsize)) <= march.BOX_S_MAX_LIMIT
+
+    _shade = _ContractedBase._shade        # sigmoid(k0), or the rgbnet on cat[k0, view embedding] (tensor cores when supported)
+
     def forward(self, rays_o, rays_d, viewdirs, global_step=None, **render_kwargs):
+        """dvgo.py:330-397 on the fused box march (see the class docstring); same keys as the reference's ret_dict."""
+        assert len(rays_o.shape) == 2 and rays_o.shape[-1] == 3, 'Only suuport point queries in [N, 3] format'
+        stepsize = render_kwargs['stepsize']
+        if not (rays_o.is_cuda and self._fused_ok(stepsize)):
+            return self.forward_ops(rays_o, rays_d, viewdirs, global_step=global_step, **render_kwargs)
+        if self._pending_mask is not None:
+            self._resolve_mask_cache()
+        N = len(rays_o)
+        mscale, mshift, lo, hi = self._mask_geometry()
+        cfg = march.make_box_cfg(lo, hi, render_kwargs['near'], self._stepdist(stepsize), host_scalar(self.act_shift),
+                                 stepsize * host_scalar(self.voxel_size_ratio), self.fast_color_thres, self.mask_cache.mask, mscale,
+                                 mshift)
+        ddesc = G.grid_desc(self.density.grid, *self.density._bounds(), 0)
+        kdesc = G.grid_desc(self.k0.grid, *self.k0._bounds(), 0)
+        weights, alphainv_last, alpha, k0, ray_id, step_id = march.BoxMarch.apply(
+            self.density.grid, self.k0.grid, rays_o, rays_d, self.mask_cache.mask, cfg, ddesc, kdesc)
+        if self.rgbnet is None or self.rgbnet_direct:
+            rgb = self._shade(k0, viewdirs, ray_id)
+        else:
+            emb = _view_embed(viewdirs, self.viewfreq).flatten(0, -2)[ray_id]
+            rgb = torch.sigmoid(self.rgbnet(torch.cat([k0[:, 3:], emb], -1)) + k0[:, :3])
+        rgb_marched = composite_rgb(weights, rgb, ray_id, N)
+        rgb_marched = rgb_marched + alphainv_last.unsqueeze(-1) * render_kwargs['bg']
+        ret = {'alphainv_last': alphainv_last, 'weights': weights, 'rgb_marched': rgb_marched, 'raw_alpha': alpha,
+               'raw_rgb': rgb, 'ray_id': ray_id}
+        if render_kwargs.get('render_depth', False):
+            with torch.no_grad():
+                ret['depth'] = segment_sum(weights * step_id, ray_id, N)
+        return ret
+
+    def forward_ops(self, rays_o, rays_d, viewdirs, global_step=None, **render_kwargs):
+        """Op-by-op composition in the reference's order (dvgo.py:330-397): ragged sample_pts_on_rays, boolean-mask compactions,
+        grid reads with their autograd, the rgbnet in torch."""
         assert len(rays_o.shape) == 2 and rays_o.shape[-1] == 3, 'Only suuport point queries in [N, 3] format'
         N, dev = len(rays_o), rays_o.device
         ray_pts, ray_id, step_id = self.sample_ray(rays_o=rays_o, rays_d=rays_d, **render_kwargs)

@@ -413,9 +413,10 @@ def count_gt_(count, grad, thres=1.0):
     return count
 
 
-def maskout_near_cam_(slab, cams, near_clip, fill=-100.0):
+def maskout_near_cam_(slab, cams, near_clip, fill=-100.0, lattice=None):
     """slab [X,Y,Z] (a view of one grid slab; unit or channel stride) <- fill where the nearest of ``cams`` [n,3] is within
-    near_clip of the lattice point (FourierGrid_model.py:383-388)."""
+    near_clip of the lattice point: linspace(-1, 1) per axis (FourierGrid_model.py:383-388), or linspace(lo[a], hi[a]) for
+    ``lattice = (lo, hi)`` host 3-sequences (DirectVoxGO's world lattice, dvgo.py:185-198)."""
     if slab.dim() != 3:
         raise RuntimeError('slab must be [X,Y,Z]')
     X, Y, Z = slab.shape
@@ -424,8 +425,13 @@ def maskout_near_cam_(slab, cams, near_clip, fill=-100.0):
         raise RuntimeError('slab must be a dense [X,Y,Z] view')
     cams = cams.contiguous().float()
     with _Guard(slab) as lib:
-        check(lib.ubn_maskout_near_cam(ptr(slab), c_i64(sv), c_i64(X), c_i64(Y), c_i64(Z), ptr(cams), c_i64(cams.shape[0]),
-                                       c_f(float(near_clip)), c_f(float(fill)), stream_of(slab)))
+        if lattice is None:
+            check(lib.ubn_maskout_near_cam(ptr(slab), c_i64(sv), c_i64(X), c_i64(Y), c_i64(Z), ptr(cams), c_i64(cams.shape[0]),
+                                           c_f(float(near_clip)), c_f(float(fill)), stream_of(slab)))
+        else:
+            lo, hi = ((c_f * 3)(*[float(v) for v in b]) for b in lattice)
+            check(lib.ubn_maskout_near_cam_lattice(ptr(slab), c_i64(sv), c_i64(X), c_i64(Y), c_i64(Z), lo, hi, ptr(cams),
+                                                   c_i64(cams.shape[0]), c_f(float(near_clip)), c_f(float(fill)), stream_of(slab)))
     return slab
 
 
