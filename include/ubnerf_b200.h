@@ -329,7 +329,9 @@ int ubn_set_density_scatter(int variant);
 int ubn_get_density_scatter(void);
 
 /* Pass B: for every survivor (flags bit1), in (ray, step) order at offsets[ray]+rank: recompute the
- * contracted point, query the feature grid (k0), and emit the compacted per-survivor records. */
+ * contracted point, query the feature grid (k0), and emit the compacted per-survivor records.
+ * k0: channels-last with C in {4, 8, 12, 16} (16-byte aligned), or C in {3, 15} with an odd slab count P <= 11 and >= 2 voxels
+ * per axis (4-byte aligned records; features bit-identical to F.grid_sample(...).mean(0)). */
 int ubn_march_feature_fwd(const float* rays_o, const float* rays_d, const float* t_table,
                           const float* k0_grid, const UbnGridDesc* k0_desc, const UbnMarchCfg* cfg,
                           int64_t n_rays, const uint8_t* flags, const int64_t* offsets,
@@ -514,6 +516,19 @@ int ubn_rgbnet_bwd_tc_fused(const float* feat, const int64_t* ray_id, const floa
                             float* grad_feat, float* grad_view_bias, float* grad_W1k, float* grad_W2, float* grad_b2,
                             float* grad_W3, float* grad_b3, uint32_t* h2_mask_scratch, const uint32_t* h1_mask, int single_pass,
                             void* stream);
+/* ubn_rgbnet_fwd_tc / ubn_rgbnet_bwd_tc_fused for n_feat in {3, 12, 15} feature columns (rgbnet_dim = 3: the Waymo / Mega-NeRF
+ * FourierGrid configs; 15: Tanks&Temples Train): feat / grad_feat are [n_pts, n_feat], W1k = W1[:, :n_feat] ([128, n_feat]
+ * row-major), grad_W1k [128, n_feat]; everything else as above.  n_feat = 12 runs the very kernels of the two functions above.
+ * At n_feat = 15 launch 1 of the backward always runs with 4 warps per CTA (8 would not fit shared memory).  Any other n_feat:
+ * cudaErrorInvalidValue. */
+int ubn_rgbnet_fwd_tc_k(int n_feat, const float* feat, const float* view_bias, const int64_t* ray_id, const float* W1k,
+                        const float* W2, const float* b2, const float* W3, const float* b3, int64_t n_pts, float* rgb, float* h1_save,
+                        float* h2_save, uint32_t* h1_mask, int single_pass, void* stream);
+int ubn_rgbnet_bwd_tc_fused_k(int n_feat, const float* feat, const int64_t* ray_id, const float* W1k, const float* W2,
+                              const float* W3, const float* rgb, const float* h1_save, const float* h2_save, const float* grad_rgb,
+                              int64_t n_pts, float* grad_feat, float* grad_view_bias, float* grad_W1k, float* grad_W2, float* grad_b2,
+                              float* grad_W3, float* grad_b3, uint32_t* h2_mask_scratch, const uint32_t* h1_mask, int single_pass,
+                              void* stream);
 
 #if defined(__GNUC__)
 #pragma GCC visibility pop

@@ -261,6 +261,70 @@ __device__ __forceinline__ void grid_density_scatter_fast(float* __restrict__ gr
   });
 }
 
+// v[kCh ..] added into q[kCh ..] when q + kCh sits at 4-byte phase kPh of a 16-byte line: the widest reduction the address
+// allows at every step (red.v4 at phase 0, red.v2 at even phases, scalar otherwise), all channel indices known at compile time
+template <int kC, int kCh, int kPh>
+__device__ __forceinline__ void red_add_from(float* q, const float* v) {
+  if constexpr (kCh < kC) {
+    if constexpr (kPh == 0 && kCh + 4 <= kC) {
+      red_add_v4(q + kCh, make_float4(v[kCh], v[kCh + 1], v[kCh + 2], v[kCh + 3]));
+      red_add_from<kC, kCh + 4, 0>(q, v);
+    } else if constexpr ((kPh & 1) == 0 && kCh + 2 <= kC) {
+      red_add_v2(q + kCh, v[kCh], v[kCh + 1]);
+      red_add_from<kC, kCh + 2, (kPh + 2) & 3>(q, v);
+    } else {
+      atomicAdd(q + kCh, v[kCh]);
+      red_add_from<kC, kCh + 1, (kPh + 1) & 3>(q, v);
+    }
+  }
+}
+
+// q[0 .. kC) += v with the widest reductions each address allows (red.v4 at 16-byte, red.v2 at 8-byte alignment, scalar
+// otherwise): the k0 scatters of the NDC / box march (C = 3, 9, 12) and of the contracted march at C = 3 and 15
+template <int kC>
+__device__ __forceinline__ void red_add_record(float* q, const float* v) {
+  if constexpr (kC % 4 == 0) {                // 16-byte aligned records (C = 12): all red.v4
+#pragma unroll
+    for (int c4 = 0; c4 < kC; c4 += 4) red_add_v4(q + c4, make_float4(v[c4], v[c4 + 1], v[c4 + 2], v[c4 + 3]));
+    return;
+  }
+  if constexpr (kC == 3) {                    // the same reductions as the loop below, without its run-time channel index
+    if ((reinterpret_cast<uintptr_t>(q) & 7) == 0) {
+      red_add_v2(q, v[0], v[1]);
+      atomicAdd(q + 2, v[2]);
+    } else {
+      atomicAdd(q, v[0]);
+      red_add_v2(q + 1, v[1], v[2]);
+    }
+    return;
+  }
+  if constexpr (kC == 15) {                   // a 60-byte record starts at any of the four phases of a 16-byte line
+    switch ((reinterpret_cast<uintptr_t>(q) >> 2) & 3) {
+      case 0: red_add_from<kC, 0, 0>(q, v); break;
+      case 1: red_add_from<kC, 0, 1>(q, v); break;
+      case 2: red_add_from<kC, 0, 2>(q, v); break;
+      default: red_add_from<kC, 0, 3>(q, v); break;
+    }
+    return;
+  }
+  int ch = 0;
+#pragma unroll
+  for (int step = 0; step < kC; ++step) {     // at most kC iterations; each consumes 1, 2 or 4 channels
+    if (ch >= kC) break;
+    const uintptr_t a = reinterpret_cast<uintptr_t>(q + ch);
+    if (ch + 4 <= kC && (a & 15) == 0) {
+      red_add_v4(q + ch, make_float4(v[ch], v[ch + 1], v[ch + 2], v[ch + 3]));
+      ch += 4;
+    } else if (ch + 2 <= kC && (a & 7) == 0) {
+      red_add_v2(q + ch, v[ch], v[ch + 1]);
+      ch += 2;
+    } else {
+      atomicAdd(q + ch, v[ch]);
+      ch += 1;
+    }
+  }
+}
+
 constexpr int kMarchWarps = 4;
 
 }  // namespace ubn

@@ -580,6 +580,223 @@ static int launch_bwd_slab(const float* rays_o, const float* rays_d, const float
   return 0;
 }
 
+// =====================================================================================================================
+// C = 3 and C = 15 (FourierGridModel with rgbnet_dim = 3 -- the Waymo / Mega-NeRF configs -- or 15, and every colour-grid stage
+// with rgbnet_dim <= 0).  A 12- or 60-byte record is only 4-byte aligned, so neither the float4 quads of the kernels above nor
+// their lane roles apply.
+//   Gather: lane = sample, as k_march_feature_v3: scalar loads, every channel accumulated in ATen's corner order (fma chain
+//   tnw .. bse) and the slabs combined in torch-CUDA's mean order, so the features are bit-identical to
+//   F.grid_sample(...).mean(0).
+//   Scatter: slab-major with the x-range split, as k_march_feature_bwd_slab.  Lane (corner = lane >> 2, run = lane & 3): the
+//   survivors of a chunk that this pass serves are cut into 4 contiguous runs, and the 8 corner lanes of a run walk its samples in
+//   order, adding the contributions of consecutive samples that share a cell in registers.  A cell leaves as one record of
+//   red_add_record (red.v4 / red.v2 / scalar, whatever each address allows) when the run moves on or ends.
+// =====================================================================================================================
+template <int kC, int kP>
+__global__ void __launch_bounds__(32 * kMarchWarps, 4) k_march_feature_narrow(
+    const float* __restrict__ rays_o, const float* __restrict__ rays_d, const float* __restrict__ t_table,
+    GridView g, MarchParams p, int64_t n_rays, const uint8_t* __restrict__ flags,
+    const int64_t* __restrict__ offsets, const float* __restrict__ density, const float* __restrict__ alpha,
+    const float* __restrict__ weight, float* __restrict__ feat, float* __restrict__ o_density, float* __restrict__ o_alpha,
+    float* __restrict__ o_weight, int64_t* __restrict__ o_ray_id, int64_t* __restrict__ o_step_id,
+    float* __restrict__ o_t, uint8_t* __restrict__ o_inner) {
+  const int lane = threadIdx.x & 31;
+  const int64_t ray = (int64_t)blockIdx.x * kMarchWarps + (threadIdx.x >> 5);
+  if (ray >= n_rays) return;
+  int64_t out_base = offsets[ray];
+  const int64_t out_end = offsets[ray + 1];
+  if (out_base == out_end) return;
+  const Ray r = load_ray(rays_o + 3 * ray, rays_d + 3 * ray, p);
+  const int S = p.S;
+  const int dY = g.Z * kC, dX = g.Y * g.Z * kC;
+
+  for (int base = 0; base < S && out_base < out_end; base += 32) {
+    const int s = base + lane;
+    const uint8_t f = (s < S) ? flags[ray * S + s] : 0;
+    const bool keep = (f & UBN_FLAG_KEEP) != 0;
+    const unsigned km = __ballot_sync(0xffffffffu, keep);
+    if (km == 0) continue;
+    const int n_here = __popc(km);
+    const int rank = __popc(km & ((1u << lane) - 1));
+    float nx = 0.f, ny = 0.f, nz = 0.f;
+    if (keep) {
+      float x, y, z;
+      const float t = t_table[s];
+      sample_point(r, t, p, x, y, z);
+      nx = norm_coord(x, g.mn[0], g.len[0]);
+      ny = norm_coord(y, g.mn[1], g.len[1]);
+      nz = norm_coord(z, g.mn[2], g.len[2]);
+      const int64_t o = out_base + rank;
+      const int64_t i = ray * S + s;
+      o_density[o] = density[i];
+      o_alpha[o] = alpha[i];
+      o_weight[o] = weight[i];
+      o_ray_id[o] = ray;
+      o_step_id[o] = s;
+      o_t[o] = t;
+      o_inner[o] = (f & UBN_FLAG_INNER) ? 1 : 0;
+    }
+    if (km != 0xffffffffu) {            // compact: lane i takes the i-th survivor of the chunk
+      const int src = __fns(km, 0, lane + 1) & 31;
+      nx = __shfl_sync(0xffffffffu, nx, src);
+      ny = __shfl_sync(0xffffffffu, ny, src);
+      nz = __shfl_sync(0xffffffffu, nz, src);
+    }
+    if (lane < n_here) {
+      // slabs visited in torch's mean order: accumulator a = slab & 3; `tot` = ((a0 + a1) + a2) + a3
+      float tot[kC], grp[kC];
+#pragma unroll
+      for (int a = 0; a < 4 && a < kP; ++a) {
+#pragma unroll
+        for (int sl = a; sl < kP; sl += 4) {
+          CellR cell;
+          slab_cell<kP>(g, sl, nx, ny, nz, cell);
+          const float* rec = g.data + sl * g.sp + (int64_t)cell.v * kC;
+          float val[kC];
+#pragma unroll
+          for (int c = 0; c < kC; ++c) val[c] = 0.f;
+#pragma unroll
+          for (int corner = 0; corner < 8; ++corner) {        // tnw, tne, tsw, tse, bnw, bne, bsw, bse (z fastest)
+            const int bx = corner >> 2, by = (corner >> 1) & 1, bz = corner & 1;
+            const float wgt = ((bz ? cell.fz : 1.f - cell.fz) * (by ? cell.fy : 1.f - cell.fy)) * (bx ? cell.fx : 1.f - cell.fx);
+            const float* q = rec + bx * dX + by * dY + bz * kC;
+#pragma unroll
+            for (int c = 0; c < kC; ++c) val[c] = fmaf(__ldg(q + c), wgt, val[c]);
+          }
+#pragma unroll
+          for (int c = 0; c < kC; ++c) grp[c] = (sl == a) ? __fadd_rn(0.f, val[c]) : __fadd_rn(grp[c], val[c]);
+        }
+#pragma unroll
+        for (int c = 0; c < kC; ++c) tot[c] = (a == 0) ? grp[c] : __fadd_rn(tot[c], grp[c]);
+      }
+      float* o = feat + (out_base + lane) * kC;
+#pragma unroll
+      for (int c = 0; c < kC; ++c) o[c] = slab_mean_scale(tot[c], kP);
+    }
+    out_base += n_here;
+  }
+}
+
+template <int kC, int kP>
+__global__ void __launch_bounds__(32 * kMarchWarps, 8) k_march_feature_bwd_narrow(
+    const float* __restrict__ rays_o, const float* __restrict__ rays_d, const float* __restrict__ t_table,
+    GridView g, MarchParams p, int64_t n_rays, const uint8_t* __restrict__ flags,
+    const int64_t* __restrict__ offsets, const float* __restrict__ gfeat, float* __restrict__ grad_grid, int n_split) {
+  const int lane = threadIdx.x & 31;
+  const int sl = blockIdx.y / n_split, part = blockIdx.y - sl * n_split;
+  const int v_lo = (int)(((int64_t)(g.X - 1) * part) / n_split) * g.Y * g.Z;
+  const int v_hi = (part + 1 == n_split) ? 0x7fffffff : (int)(((int64_t)(g.X - 1) * (part + 1)) / n_split) * g.Y * g.Z;
+  const int64_t ray = (int64_t)blockIdx.x * kMarchWarps + (threadIdx.x >> 5);
+  if (ray >= n_rays) return;
+  int64_t out_base = offsets[ray];
+  const int64_t out_end = offsets[ray + 1];
+  if (out_base == out_end) return;
+  const int corner = lane >> 2, run = lane & 3;
+  const bool bx = corner & 4, by = corner & 2, bz = corner & 1;
+  float* slab = grad_grid + sl * g.sp + (((bx ? 1 : 0) * g.Y + (by ? 1 : 0)) * g.Z + (bz ? 1 : 0)) * kC;
+  const Ray r = load_ray(rays_o + 3 * ray, rays_d + 3 * ray, p);
+  const int S = p.S;
+
+  for (int base = 0; base < S && out_base < out_end; base += 32) {
+    const int s = base + lane;
+    const uint8_t f = (s < S) ? flags[ray * S + s] : 0;
+    const bool keep = (f & UBN_FLAG_KEEP) != 0;
+    const unsigned km = __ballot_sync(0xffffffffu, keep);
+    if (km == 0) continue;
+    CellR cell;
+    {
+      float x = 0, y = 0, z = 0;
+      if (keep) sample_point(r, t_table[s], p, x, y, z);
+      const float nx = norm_coord(x, g.mn[0], g.len[0]);
+      const float ny = norm_coord(y, g.mn[1], g.len[1]);
+      const float nz = norm_coord(z, g.mn[2], g.len[2]);
+      if (kP == 1) cell = make_cell(src_index(nx, g.X), src_index(ny, g.Y), src_index(nz, g.Z), g.X, g.Y, g.Z);
+      else cell = make_cell(src_index(fourier_gamma(sl, nx), g.X), src_index(fourier_gamma(sl, ny), g.Y),
+                            src_index(fourier_gamma(sl, nz), g.Z), g.X, g.Y, g.Z);
+    }
+    // survivors of the chunk that this pass serves; `row` = their position in the compacted gradient rows
+    const unsigned sm = __ballot_sync(0xffffffffu, keep && cell.v >= v_lo && cell.v < v_hi);
+    const int n_here = __popc(sm);
+    int row = __popc(km & ((1u << lane) - 1));
+    if (sm != 0xffffffffu) {
+      const int src = __fns(sm, 0, lane + 1) & 31;
+      cell.v = __shfl_sync(0xffffffffu, cell.v, src);
+      cell.fx = __shfl_sync(0xffffffffu, cell.fx, src);
+      cell.fy = __shfl_sync(0xffffffffu, cell.fy, src);
+      cell.fz = __shfl_sync(0xffffffffu, cell.fz, src);
+      row = __shfl_sync(0xffffffffu, row, src);
+    }
+    const int len = (n_here + 3) >> 2;                     // samples per run (warp-uniform)
+    const int i0 = min(run * len, n_here), i1 = min(i0 + len, n_here);
+    int open = -1;                                         // cell of the open sum (-1: none)
+    float acc[kC];
+#pragma unroll
+    for (int c = 0; c < kC; ++c) acc[c] = 0.f;
+    for (int i = 0; i < len; ++i) {
+      const int src = (i0 + i) & 31;
+      const int v = __shfl_sync(0xffffffffu, cell.v, src);
+      const float fx = __shfl_sync(0xffffffffu, cell.fx, src);
+      const float fy = __shfl_sync(0xffffffffu, cell.fy, src);
+      const float fz = __shfl_sync(0xffffffffu, cell.fz, src);
+      const int rj = __shfl_sync(0xffffffffu, row, src);
+      if (i0 + i >= i1) continue;                          // the last run may be shorter; every lane keeps shuffling
+      // 1 / P folded into the corner weight
+      const float wgt = slab_mean_scale(((bz ? fz : 1.f - fz) * (by ? fy : 1.f - fy)) * (bx ? fx : 1.f - fx), kP);
+      const float* gi = gfeat + (out_base + rj) * kC;
+      if (v != open) {
+        if (open >= 0) red_add_record<kC>(slab + (int64_t)open * kC, acc);
+        open = v;
+#pragma unroll
+        for (int c = 0; c < kC; ++c) acc[c] = wgt * __ldg(gi + c);
+      } else {
+#pragma unroll
+        for (int c = 0; c < kC; ++c) acc[c] += wgt * __ldg(gi + c);
+      }
+    }
+    if (open >= 0) red_add_record<kC>(slab + (int64_t)open * kC, acc);
+    out_base += __popc(km);
+  }
+}
+
+template <int kC, int kP>
+static int launch_narrow(bool backward, const float* rays_o, const float* rays_d, const float* t_table, const GridView& g,
+                         const MarchParams& p, int64_t n_rays, const uint8_t* flags, const int64_t* offsets, const float* density,
+                         const float* alpha, const float* weight, float* feat, float* grad_grid, float* o_density, float* o_alpha,
+                         float* o_weight, int64_t* o_ray_id, int64_t* o_step_id, float* o_t, uint8_t* o_inner, int n_split,
+                         cudaStream_t st) {
+  if (backward)
+    k_march_feature_bwd_narrow<kC, kP><<<dim3(blocks_for(n_rays, kMarchWarps), kP * n_split), 32 * kMarchWarps, 0, st>>>(
+        rays_o, rays_d, t_table, g, p, n_rays, flags, offsets, feat, grad_grid, n_split);
+  else
+    k_march_feature_narrow<kC, kP><<<blocks_for(n_rays, kMarchWarps), 32 * kMarchWarps, 0, st>>>(
+        rays_o, rays_d, t_table, g, p, n_rays, flags, offsets, density, alpha, weight, feat, o_density, o_alpha, o_weight, o_ray_id,
+        o_step_id, o_t, o_inner);
+  UBN_LAUNCH_CHECK();
+  return 0;
+}
+
+template <int kC>
+static int march_feature_narrow(bool backward, const float* rays_o, const float* rays_d, const float* t_table, const GridView& g,
+                                const MarchParams& p, int64_t n_rays, const uint8_t* flags, const int64_t* offsets,
+                                const float* density, const float* alpha, const float* weight, float* feat, float* grad_grid,
+                                float* o_density, float* o_alpha, float* o_weight, int64_t* o_ray_id, int64_t* o_step_id, float* o_t,
+                                uint8_t* o_inner, int n_split, cudaStream_t st) {
+#define UBN_NARROW(P)                                                                                                            \
+  case P:                                                                                                                        \
+    return launch_narrow<kC, P>(backward, rays_o, rays_d, t_table, g, p, n_rays, flags, offsets, density, alpha, weight, feat,    \
+                                grad_grid, o_density, o_alpha, o_weight, o_ray_id, o_step_id, o_t, o_inner, n_split, st)
+  switch (g.P) {
+    UBN_NARROW(1);
+    UBN_NARROW(3);
+    UBN_NARROW(5);
+    UBN_NARROW(7);
+    UBN_NARROW(9);
+    UBN_NARROW(11);
+    default: return -1;
+  }
+#undef UBN_NARROW
+}
+
 // Pass-B kernel family, set through ubn_set_feature_kernel (the GPU tests exercise every value):
 //   0  warp-cooperative gather and scatter (k_march_feature_v2)
 //   1  lane-per-sample gather (k_march_feature_v3) + cooperative scatter
@@ -605,6 +822,14 @@ int march_feature_v2(bool backward, const float* rays_o, const float* rays_d, co
                      uint8_t* o_inner, cudaStream_t st) {
   if (g.X < 2 || g.Y < 2 || g.Z < 2) return -1;
   if ((int64_t)g.X * g.Y * g.Z * g.C >= (1ll << 31)) return -1;   // 32-bit voxel offsets inside a slab
+  if (g.C == 3 || g.C == 15) {                            // every variant: the lane-per-sample gather, the slab-major run scatter
+    const int n_split = g_feature_kernel == 4 ? 2 : g_feature_kernel == 5 ? 4 : 1;
+    if (g.C == 3)
+      return march_feature_narrow<3>(backward, rays_o, rays_d, t_table, g, p, n_rays, flags, offsets, density, alpha, weight, feat,
+                                     grad_grid, o_density, o_alpha, o_weight, o_ray_id, o_step_id, o_t, o_inner, n_split, st);
+    return march_feature_narrow<15>(backward, rays_o, rays_d, t_table, g, p, n_rays, flags, offsets, density, alpha, weight, feat,
+                                    grad_grid, o_density, o_alpha, o_weight, o_ray_id, o_step_id, o_t, o_inner, n_split, st);
+  }
   if (backward && g_feature_kernel >= 3 && g.P > 1) {     // 3 / 4 / 5: slab-major scatter, each slab swept in 1 / 2 / 4 x-ranges; 6: as 3
     const int n_split = g_feature_kernel == 6 ? 1 : 1 << (g_feature_kernel - 3);
     switch (g.P) {

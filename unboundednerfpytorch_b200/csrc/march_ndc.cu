@@ -18,41 +18,6 @@
 
 namespace ubn {
 
-template <int kC>
-__device__ __forceinline__ void red_add_record(float* q, const float* v) {
-  if constexpr (kC % 4 == 0) {                // 16-byte aligned records (C = 12): all red.v4
-#pragma unroll
-    for (int c4 = 0; c4 < kC; c4 += 4) red_add_v4(q + c4, make_float4(v[c4], v[c4 + 1], v[c4 + 2], v[c4 + 3]));
-    return;
-  }
-  if constexpr (kC == 3) {                    // the same reductions as the loop below, without its run-time channel index
-    if ((reinterpret_cast<uintptr_t>(q) & 7) == 0) {
-      red_add_v2(q, v[0], v[1]);
-      atomicAdd(q + 2, v[2]);
-    } else {
-      atomicAdd(q, v[0]);
-      red_add_v2(q + 1, v[1], v[2]);
-    }
-    return;
-  }
-  int ch = 0;
-#pragma unroll
-  for (int step = 0; step < kC; ++step) {     // at most kC iterations; each consumes 1, 2 or 4 channels
-    if (ch >= kC) break;
-    const uintptr_t a = reinterpret_cast<uintptr_t>(q + ch);
-    if (ch + 4 <= kC && (a & 15) == 0) {
-      red_add_v4(q + ch, make_float4(v[ch], v[ch + 1], v[ch + 2], v[ch + 3]));
-      ch += 4;
-    } else if (ch + 2 <= kC && (a & 7) == 0) {
-      red_add_v2(q + ch, v[ch], v[ch + 1]);
-      ch += 2;
-    } else {
-      atomicAdd(q + ch, v[ch]);
-      ch += 1;
-    }
-  }
-}
-
 template <class Smp, int kC, bool kBackward>
 __global__ void __launch_bounds__(32 * kMarchWarps) k_march_ndc_feature(
     const float* __restrict__ rays_o, const float* __restrict__ rays_d, GridView g, MarchParams p, int64_t n_rays,

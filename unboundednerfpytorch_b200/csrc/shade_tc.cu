@@ -26,7 +26,7 @@ namespace ubn {
 namespace tc {
 
 constexpr int kHidden = 128;
-constexpr int kFeat = 12;
+constexpr int kFeat = 12;               // feature columns of every shipped 12-channel config; kernels take kF in {3, 12, 15}
 constexpr int kNT = kHidden / 8;        // 8-column tiles of a 128-wide layer
 constexpr int kUnit = 16;               // samples per warp unit (the M of one mma)
 constexpr int kPanelRows = 128;         // row block of the panel save layout
@@ -34,8 +34,8 @@ constexpr int kStride = kHidden + 8;    // floats per row of a shared-memory ope
 
 // B-fragment tables (uint4 per lane): [n-tile][k-step][32 lanes]
 constexpr uint32_t kFragW2 = kNT * kNT * 32 * 16;          // 128 KB
-constexpr uint32_t kFragW1 = kNT * 2 * 32 * 16;            // layer 1: K = 12 (2 k-steps), N = 128
-constexpr uint32_t kFragW1T = 2 * kNT * 32 * 16;           // dX: K = 128, N = 12 (2 n-tiles)
+constexpr uint32_t kFragW1 = kNT * 2 * 32 * 16;            // layer 1: K <= 16 (at most 2 k-steps), N = 128
+constexpr uint32_t kFragW1T = 2 * kNT * 32 * 16;           // dX: K = 128, N <= 16 (at most 2 n-tiles)
 
 __device__ __forceinline__ uint32_t tf32_hi_bits(float x) { return __float_as_uint(x) & 0xFFFFE000u; }
 
@@ -127,7 +127,8 @@ constexpr uint32_t oFW3 = oFW1 + kFragW1;                 // [3][128]
 constexpr uint32_t oFB2 = oFW3 + 3 * kHidden * 4;
 constexpr uint32_t kSmemFwd = oFB2 + kHidden * 4;
 
-template <bool kSave, bool kThree, int kWarps, bool kPanel>
+// kF feature columns: ceil(kF / 8) k-steps of layer 1 (1 for kF = 3, 2 for 12 and 15); odd kF rows are 4-byte aligned
+template <int kF, bool kSave, bool kThree, int kWarps, bool kPanel>
 __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_fwd_tc(
     const float* __restrict__ feat, const float* __restrict__ vb, const int64_t* __restrict__ ray_id,
     const float* __restrict__ W1k, const float* __restrict__ W2, const float* __restrict__ b2,
@@ -140,7 +141,8 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_fwd_tc(
   float* sW3 = reinterpret_cast<float*>(smem + oFW3);
   float* sB2 = reinterpret_cast<float*>(smem + oFB2);
   stage_frags(W2, kHidden, true, kHidden, kHidden, kNT, kNT, reinterpret_cast<uint4*>(smem + oFW2), tid, 32 * kWarps);
-  stage_frags(W1k, kFeat, true, kFeat, kHidden, 2, kNT, reinterpret_cast<uint4*>(smem + oFW1), tid, 32 * kWarps);
+  constexpr int kKS = (kF + 7) / 8;
+  stage_frags(W1k, kF, true, kF, kHidden, kKS, kNT, reinterpret_cast<uint4*>(smem + oFW1), tid, 32 * kWarps);
   for (int i = tid; i < 3 * kHidden; i += 32 * kWarps) sW3[i] = W3[i];
   for (int i = tid; i < kHidden; i += 32 * kWarps) sB2[i] = b2[i];
   __syncthreads();
@@ -150,14 +152,20 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_fwd_tc(
   for (int64_t u = (int64_t)blockIdx.x * kWarps + (tid >> 5); u < n_units; u += (int64_t)gridDim.x * kWarps) {
     const int64_t row[2] = {u * kUnit + g, u * kUnit + g + 8};
     const bool live[2] = {row[0] < n_pts, row[1] < n_pts};
-    // layer 1: X in accumulator layout, column tile s = features 8 s .. 8 s + 7 (12..15 are zero)
-    float x[2][4];
+    // layer 1: X in accumulator layout, column tile s = features 8 s .. 8 s + 7 (kF .. 8 kKS - 1 are zero)
+    float x[kKS][4];
 #pragma unroll
-    for (int s = 0; s < 2; ++s)
+    for (int s = 0; s < kKS; ++s)
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         float2 v = make_float2(0.f, 0.f);
-        if (live[r] && 8 * s + 2 * t < kFeat) v = *reinterpret_cast<const float2*>(feat + row[r] * kFeat + 8 * s + 2 * t);
+        if constexpr (kF % 2 == 0) {
+          if (live[r] && 8 * s + 2 * t < kF) v = *reinterpret_cast<const float2*>(feat + row[r] * kF + 8 * s + 2 * t);
+        } else if (live[r]) {
+          const int c = 8 * s + 2 * t;
+          if (c < kF) v.x = feat[row[r] * kF + c];
+          if (c + 1 < kF) v.y = feat[row[r] * kF + c + 1];
+        }
         x[s][2 * r] = v.x;
         x[s][2 * r + 1] = v.y;
       }
@@ -165,7 +173,7 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_fwd_tc(
     float h[kNT][4];
 #pragma unroll
     for (int j = 0; j < kNT; ++j) h[j][0] = h[j][1] = h[j][2] = h[j][3] = 0.f;
-    warp_gemm<2, kNT, kThree>(h, x, fW1, lane);
+    warp_gemm<kKS, kNT, kThree>(h, x, fW1, lane);
     // epilogue 1: + vb[ray], ReLU
 #pragma unroll
     for (int j = 0; j < kNT; ++j)
@@ -245,9 +253,9 @@ constexpr uint32_t oWarp = oW3 + 3 * kHidden * 4;
 // per warp: operand tile [16][kStride], the running sums dW1k^T [12][kStride], dW3 [3][kStride], E [3][kStride], and the
 // open ray's dZ1 sum [kStride]
 constexpr uint32_t kTileBytes = kUnit * kStride * 4;
-constexpr int kSumRows = kFeat + 3 + 3;
-constexpr uint32_t kWarpBytes = kTileBytes + (kSumRows + 1) * kStride * 4;
-constexpr uint32_t smem_bytes(int warps) { return oWarp + warps * kWarpBytes; }
+__host__ __device__ constexpr int sum_rows(int f) { return f + 3 + 3; }
+__host__ __device__ constexpr uint32_t warp_bytes(int f) { return kTileBytes + (sum_rows(f) + 1) * kStride * 4; }
+__host__ __device__ constexpr uint32_t smem_bytes(int warps, int f) { return oWarp + warps * warp_bytes(f); }
 }  // namespace bk
 
 // lane (g, t) of (n-tile j, k-step s) gets the fp32 pair {B[8s+2t][8j+g], B[8s+2t+1][8j+g]}, B[k][n] = W[k * ld + n]
@@ -324,8 +332,10 @@ __device__ __forceinline__ void emit_ray(float* grad_view_bias, int64_t ray, con
   }
 }
 
-template <bool kThree, int kWarps, bool kPanel, bool kMask1, bool kDz1Out>
-__global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc(
+// kF feature columns: dX has ceil(kF / 8) n-tiles.  The dW1k^T sums and the ray-segment indicators share one 16-row A tile
+// while kF <= 12 (features in rows 0 .. kF - 1, indicators in rows 12 .. 15); at kF = 15 the indicators get an m-tile of their own.
+template <int kF, bool kThree, int kWarps, bool kPanel, bool kMask1, bool kDz1Out>
+__device__ __forceinline__ void shade_bwd_tc(
     const float* __restrict__ feat, const int64_t* __restrict__ ray_id, const float* __restrict__ W1k,
     const float* __restrict__ W2, const float* __restrict__ W3, const float* __restrict__ rgb,
     const float* __restrict__ h1_save, const float* __restrict__ h2_save, const float* __restrict__ grad_rgb, int64_t n_pts,
@@ -334,20 +344,23 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc(
     float* __restrict__ dz1_out) {
   extern __shared__ __align__(16) uint8_t smem[];
   constexpr int kThreads = 32 * kWarps;
+  constexpr int kNTX = (kF + 7) / 8;                      // n-tiles of dX
+  constexpr bool kSegTile = kF > 12;                      // indicators in a second m-tile
+  constexpr uint32_t kWarpBytes = bk::warp_bytes(kF);
   const int tid = threadIdx.x, lane = tid & 31, g = lane >> 2, t = lane & 3, warp = tid >> 5;
   const uint2* fW2 = reinterpret_cast<const uint2*>(smem + bk::oW2);
   const uint2* fW1T = reinterpret_cast<const uint2*>(smem + bk::oW1T);
   float* sW3 = reinterpret_cast<float*>(smem + bk::oW3);
-  float* S = reinterpret_cast<float*>(smem + bk::oWarp + warp * bk::kWarpBytes);
+  float* S = reinterpret_cast<float*>(smem + bk::oWarp + warp * kWarpBytes);
   float* sumW1 = S + kUnit * kStride;                     // dW1k^T [feature][unit]
-  float* sumW3 = sumW1 + kFeat * kStride;
+  float* sumW3 = sumW1 + kF * kStride;
   float* sumE = sumW3 + 3 * kStride;
   float* vbc = sumE + 3 * kStride;                        // lanes g == 4: the open ray's sum of dZ1 so far
   stage_frags_f32(W2, kHidden, kHidden, kHidden, kNT, kNT, reinterpret_cast<uint2*>(smem + bk::oW2), tid, kThreads);
-  if (!kDz1Out) stage_frags_f32(W1k, kFeat, kHidden, kFeat, kNT, 2, reinterpret_cast<uint2*>(smem + bk::oW1T), tid, kThreads);
+  if (!kDz1Out) stage_frags_f32(W1k, kF, kHidden, kF, kNT, kNTX, reinterpret_cast<uint2*>(smem + bk::oW1T), tid, kThreads);
   for (int i = tid; i < 3 * kHidden; i += kThreads) sW3[i] = W3[i];
   if (!kDz1Out)
-    for (int i = lane; i < bk::kSumRows * kStride; i += 32) sumW1[i] = 0.f;
+    for (int i = lane; i < bk::sum_rows(kF) * kStride; i += 32) sumW1[i] = 0.f;
   __syncthreads();
 
   float db3 = 0.f;                                        // lane i < 3: this warp's sum of dz3_i
@@ -502,16 +515,23 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc(
     }
     // dX = dZ1 . W1k
     {
-      float dx[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-      warp_gemm_f<kNT, 2, kThree>(dx, d1, fW1T, lane);
+      float dx[kNTX][4] = {};
+      warp_gemm_f<kNT, kNTX, kThree>(dx, d1, fW1T, lane);
 #pragma unroll
-      for (int j = 0; j < 2; ++j)
+      for (int j = 0; j < kNTX; ++j)
 #pragma unroll
-        for (int r = 0; r < 2; ++r)
-          if (live[r] && 8 * j + 2 * t < kFeat)
-            *reinterpret_cast<float2*>(grad_feat + row[r] * kFeat + 8 * j + 2 * t) = make_float2(dx[j][2 * r], dx[j][2 * r + 1]);
+        for (int r = 0; r < 2; ++r) {
+          const int c = 8 * j + 2 * t;
+          if constexpr (kF % 2 == 0) {
+            if (live[r] && c < kF) *reinterpret_cast<float2*>(grad_feat + row[r] * kF + c) = make_float2(dx[j][2 * r], dx[j][2 * r + 1]);
+          } else if (live[r]) {
+            if (c < kF) grad_feat[row[r] * kF + c] = dx[j][2 * r];
+            if (c + 1 < kF) grad_feat[row[r] * kF + c + 1] = dx[j][2 * r + 1];
+          }
+        }
     }
-    // dW1k^T = X^T . dZ1 (A rows 0..11) and per-ray sums of dZ1 (A rows 12..15 = indicators of up to 4 ray segments)
+    // dW1k^T = X^T . dZ1 (A rows 0 .. kF - 1) and per-ray sums of dZ1 (A rows 12..15 = indicators of up to 4 ray segments; at
+    // kF > 12 those rows of a second m-tile)
     tile_store(S, d1, g, t);
     __syncwarp();                                             // the tile is read back across lanes as B fragments below
     const int64_t my_ray = (lane < kUnit && r0 + lane < n_pts) ? ray_id[r0 + lane] : -1;
@@ -521,39 +541,80 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc(
     const bool segs_fit = nseg <= 4;
     {
       float acc[kNT][4];
+      // kF <= 12: one m-tile -- row g feature g, row g + 8 feature g + 8 (g < 4) or the indicator of segment g - 4 (g >= 4).
+      // kF > 12: the features fill rows 0 .. kF - 1 and the indicators get rows 12..15 of a second m-tile.
+      if constexpr (!kSegTile) {
 #pragma unroll
-      for (int j = 0; j < kNT; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
+        for (int j = 0; j < kNT; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
 #pragma unroll
-      for (int s = 0; s < 2; ++s) {
-        float av[4];
+        for (int s = 0; s < 2; ++s) {
+          float av[4];
 #pragma unroll
-        for (int q = 0; q < 2; ++q) {                         // sample k = 8 s + t + 4 q
-          const int64_t rr = r0 + 8 * s + t + 4 * q;
-          const int ks = 8 * s + t + 4 * q;
-          const bool ok = rr < n_pts;
-          av[2 * q] = ok ? feat[rr * kFeat + g] : 0.f;                         // A row g: feature g
-          float lo = 0.f;                                                       // A row g + 8: feature g + 8 or segment g - 4
-          if (ok) {
-            if (g < 4) lo = feat[rr * kFeat + g + 8];
-            else if (segs_fit) lo = (__popc(starts & ((2u << ks) - 1u)) - 1 == g - 4) ? 1.f : 0.f;
+          for (int q = 0; q < 2; ++q) {                       // sample k = 8 s + t + 4 q
+            const int64_t rr = r0 + 8 * s + t + 4 * q;
+            const int ks = 8 * s + t + 4 * q;
+            const bool ok = rr < n_pts;
+            av[2 * q] = (ok && (kF >= 8 || g < kF)) ? feat[rr * kF + g] : 0.f;   // A row g: feature g
+            float lo = 0.f;                                                     // A row g + 8: feature g + 8 or segment g - 4
+            if (ok) {
+              if (g < 4) { if (kF >= 12 || g + 8 < kF) lo = feat[rr * kF + g + 8]; }
+              else if (segs_fit) lo = (__popc(starts & ((2u << ks) - 1u)) - 1 == g - 4) ? 1.f : 0.f;
+            }
+            av[2 * q + 1] = lo;
           }
-          av[2 * q + 1] = lo;
+          const float a[4] = {av[0], av[1], av[2], av[3]};
+          uint32_t ah[4], al[4];
+          split4(a, ah, al);
+#pragma unroll
+          for (int j = 0; j < kNT; ++j) {
+            uint32_t bh[2], bl[2];
+            tile_frag(S, s, j, g, t, bh, bl);
+            mma3<kThree>(acc[j], ah, al, make_uint4(bh[0], bh[1], bl[0], bl[1]));
+          }
         }
-        const float a[4] = {av[0], av[1], av[2], av[3]};
-        uint32_t ah[4], al[4];
-        split4(a, ah, al);
 #pragma unroll
         for (int j = 0; j < kNT; ++j) {
-          uint32_t bh[2], bl[2];
-          tile_frag(S, s, j, g, t, bh, bl);
-          mma3<kThree>(acc[j], ah, al, make_uint4(bh[0], bh[1], bl[0], bl[1]));
+          const int c = 8 * j + 2 * t;
+          if (kF >= 8 || g < kF) sum_add2(sumW1 + g * kStride + c, acc[j][0], acc[j][1]);
+          if (g < 4 && (kF >= 12 || g + 8 < kF)) sum_add2(sumW1 + (g + 8) * kStride + c, acc[j][2], acc[j][3]);
         }
-      }
+      } else {
+        // A[row][sample k] from row_lo (rows g) and row_hi (rows g + 8) of sample rr = r0 + k, zero past the last sample
+        auto tile_gemm = [&](auto row_lo, auto row_hi) {
 #pragma unroll
-      for (int j = 0; j < kNT; ++j) {
-        const int c = 8 * j + 2 * t;
-        sum_add2(sumW1 + g * kStride + c, acc[j][0], acc[j][1]);
-        if (g < 4) sum_add2(sumW1 + (g + 8) * kStride + c, acc[j][2], acc[j][3]);
+          for (int j = 0; j < kNT; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
+#pragma unroll
+          for (int s = 0; s < 2; ++s) {
+            float av[4];
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {                     // sample k = 8 s + t + 4 q
+              const int ks = 8 * s + t + 4 * q;
+              const bool ok = r0 + ks < n_pts;
+              av[2 * q] = ok ? row_lo(r0 + ks) : 0.f;
+              av[2 * q + 1] = ok ? row_hi(r0 + ks, ks) : 0.f;
+            }
+            uint32_t ah[4], al[4];
+            split4(av, ah, al);
+#pragma unroll
+            for (int j = 0; j < kNT; ++j) {
+              uint32_t bh[2], bl[2];
+              tile_frag(S, s, j, g, t, bh, bl);
+              mma3<kThree>(acc[j], ah, al, make_uint4(bh[0], bh[1], bl[0], bl[1]));
+            }
+          }
+        };
+        tile_gemm([&](int64_t rr) { return feat[rr * kF + g]; },                               // features 0 .. kF - 1
+                  [&](int64_t rr, int) { return g + 8 < kF ? feat[rr * kF + g + 8] : 0.f; });
+#pragma unroll
+        for (int j = 0; j < kNT; ++j) {
+          const int c = 8 * j + 2 * t;
+          sum_add2(sumW1 + g * kStride + c, acc[j][0], acc[j][1]);
+          if (g + 8 < kF) sum_add2(sumW1 + (g + 8) * kStride + c, acc[j][2], acc[j][3]);
+        }
+        tile_gemm([&](int64_t) { return 0.f; },                                                  // rows 12..15: segments g - 4
+                  [&](int64_t, int ks) {
+                    return (g >= 4 && segs_fit && __popc(starts & ((2u << ks) - 1u)) - 1 == g - 4) ? 1.f : 0.f;
+                  });
       }
       // rays of the unit's first and last segment, and (lanes g = 4 + q) of segment q
       const int64_t first_ray = __shfl_sync(0xffffffffu, my_ray, __ffs(starts) - 1);
@@ -609,21 +670,44 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc(
   auto warp_sum = [&](int r, int c) {
     float v = 0.f;
 #pragma unroll
-    for (int w = 0; w < kWarps; ++w) v += sums[w * (bk::kWarpBytes / 4) + r * kStride + c];
+    for (int w = 0; w < kWarps; ++w) v += sums[w * (kWarpBytes / 4) + r * kStride + c];
     return v;
   };
-  for (int i = tid; i < kFeat * kHidden; i += kThreads) {        // row f of the sums is column f of dW1k
+  for (int i = tid; i < kF * kHidden; i += kThreads) {           // row f of the sums is column f of dW1k
     const int f = i / kHidden, c = i % kHidden;
-    atomicAdd(grad_W1k + c * kFeat + f, warp_sum(f, c));
+    atomicAdd(grad_W1k + c * kF + f, warp_sum(f, c));
   }
-  for (int i = tid; i < 3 * kHidden; i += kThreads) atomicAdd(grad_W3 + i, warp_sum(kFeat + i / kHidden, i % kHidden));
+  for (int i = tid; i < 3 * kHidden; i += kThreads) atomicAdd(grad_W3 + i, warp_sum(kF + i / kHidden, i % kHidden));
   for (int c = tid; c < kHidden; c += kThreads) {
     float v = 0.f;
 #pragma unroll
-    for (int i = 0; i < 3; ++i) v += sW3[i * kHidden + c] * warp_sum(kFeat + 3 + i, c);
+    for (int i = 0; i < 3; ++i) v += sW3[i * kHidden + c] * warp_sum(kF + 3 + i, c);
     atomicAdd(grad_b2 + c, v);
   }
 }
+
+#define UBN_SHADE_BWD_PARAMS                                                                                                    \
+  const float* __restrict__ feat, const int64_t* __restrict__ ray_id, const float* __restrict__ W1k, const float* __restrict__ W2, \
+      const float* __restrict__ W3, const float* __restrict__ rgb, const float* __restrict__ h1_save,                             \
+      const float* __restrict__ h2_save, const float* __restrict__ grad_rgb, int64_t n_pts, float* __restrict__ grad_feat,        \
+      float* __restrict__ grad_view_bias, float* __restrict__ grad_W1k, float* __restrict__ grad_b2, float* __restrict__ grad_W3, \
+      float* __restrict__ grad_b3, uint32_t* __restrict__ h2_mask, const uint32_t* __restrict__ h1_mask, float* __restrict__ dz1_out
+#define UBN_SHADE_BWD_ARGS                                                                                                     \
+  feat, ray_id, W1k, W2, W3, rgb, h1_save, h2_save, grad_rgb, n_pts, grad_feat, grad_view_bias, grad_W1k, grad_b2, grad_W3, grad_b3, \
+      h2_mask, h1_mask, dz1_out
+
+// the 12-feature kernel keeps its own name; k_shade_bwd_tc_k carries the other feature counts
+template <bool kThree, int kWarps, bool kPanel, bool kMask1, bool kDz1Out>
+__global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc(UBN_SHADE_BWD_PARAMS) {
+  shade_bwd_tc<kFeat, kThree, kWarps, kPanel, kMask1, kDz1Out>(UBN_SHADE_BWD_ARGS);
+}
+
+template <int kF, bool kThree, int kWarps, bool kPanel, bool kMask1, bool kDz1Out>
+__global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc_k(UBN_SHADE_BWD_PARAMS) {
+  shade_bwd_tc<kF, kThree, kWarps, kPanel, kMask1, kDz1Out>(UBN_SHADE_BWD_ARGS);
+}
+#undef UBN_SHADE_BWD_ARGS
+#undef UBN_SHADE_BWD_PARAMS
 
 // ---- backward, launch 2: dW2 += dZ2^T . H1 -------------------------------------------------------------------------------
 // A split-K GEMM over samples: each CTA takes 32-sample chunks, stages dZ2 (rebuilt from dz3, W3 and H2 or its ReLU masks) as a
@@ -769,30 +853,33 @@ unsigned unit_grid(int64_t n_pts, int warps) {
   return (unsigned)std::min<int64_t>(kNumSMs, (n_units + warps - 1) / warps);
 }
 
-template <bool kSave, bool kThree, int kWarps, bool kPanel>
+template <int kF, bool kSave, bool kThree, int kWarps, bool kPanel>
 int launch_fwd(const float* feat, const float* vb, const int64_t* ray_id, const float* W1k, const float* W2, const float* b2,
                const float* W3, const float* b3, int64_t n, float* rgb, float* h1, float* h2, uint32_t* m1, cudaStream_t st) {
-  auto k = tc::k_shade_fwd_tc<kSave, kThree, kWarps, kPanel>;
+  auto k = tc::k_shade_fwd_tc<kF, kSave, kThree, kWarps, kPanel>;
   if (int e = set_smem(k, tc::kSmemFwd)) return e;
   k<<<unit_grid(n, kWarps), 32 * kWarps, tc::kSmemFwd, st>>>(feat, vb, ray_id, W1k, W2, b2, W3, b3, n, rgb, h1, h2, m1);
   UBN_LAUNCH_CHECK();
   return 0;
 }
 
-template <bool kSave, bool kThree, int kWarps>
+template <int kF, bool kSave, bool kThree, int kWarps>
 int launch_fwd_p(bool panel, const float* feat, const float* vb, const int64_t* ray_id, const float* W1k, const float* W2,
                  const float* b2, const float* W3, const float* b3, int64_t n, float* rgb, float* h1, float* h2, uint32_t* m1,
                  cudaStream_t st) {
-  return panel ? launch_fwd<kSave, kThree, kWarps, true>(feat, vb, ray_id, W1k, W2, b2, W3, b3, n, rgb, h1, h2, m1, st)
-               : launch_fwd<kSave, kThree, kWarps, false>(feat, vb, ray_id, W1k, W2, b2, W3, b3, n, rgb, h1, h2, nullptr, st);
+  return panel ? launch_fwd<kF, kSave, kThree, kWarps, true>(feat, vb, ray_id, W1k, W2, b2, W3, b3, n, rgb, h1, h2, m1, st)
+               : launch_fwd<kF, kSave, kThree, kWarps, false>(feat, vb, ray_id, W1k, W2, b2, W3, b3, n, rgb, h1, h2, nullptr, st);
 }
 
-template <bool kThree, int kWarps, bool kPanel, bool kMask1, bool kDz1Out>
+template <int kF, bool kThree, int kWarps, bool kPanel, bool kMask1, bool kDz1Out>
 int launch_bwd(const float* feat, const int64_t* ray_id, const float* W1k, const float* W2, const float* W3, const float* rgb,
                const float* h1, const float* h2, const float* grad_rgb, int64_t n, float* grad_feat, float* grad_vb, float* gW1k,
                float* gb2, float* gW3, float* gb3, uint32_t* m2, const uint32_t* m1, float* dz1, cudaStream_t st) {
-  auto k = tc::k_shade_bwd_tc<kThree, kWarps, kPanel, kMask1, kDz1Out>;
-  const uint32_t bytes = tc::bk::smem_bytes(kWarps);
+  auto k = [] {
+    if constexpr (kF == tc::kFeat) return tc::k_shade_bwd_tc<kThree, kWarps, kPanel, kMask1, kDz1Out>;
+    else return tc::k_shade_bwd_tc_k<kF, kThree, kWarps, kPanel, kMask1, kDz1Out>;
+  }();
+  const uint32_t bytes = tc::bk::smem_bytes(kWarps, kF);
   if (int e = set_smem(k, bytes)) return e;
   k<<<unit_grid(n, kWarps), 32 * kWarps, bytes, st>>>(feat, ray_id, W1k, W2, W3, rgb, h1, h2, grad_rgb, n, grad_feat, grad_vb, gW1k,
                                                       gb2, gW3, gb3, m2, m1, dz1);
@@ -812,17 +899,16 @@ int launch_dw2(const float* W3, const float* rgb, const float* h1, const float* 
   return 0;
 }
 
-}  // namespace
-
-extern "C" int ubn_rgbnet_fwd_tc(const float* feat, const float* view_bias, const int64_t* ray_id, const float* W1k,
-                                 const float* W2, const float* b2, const float* W3, const float* b3, int64_t n_pts,
-                                 float* rgb, float* h1_save, float* h2_save, uint32_t* h1_mask, int single_pass, void* stream) {
+template <int kF>
+int rgbnet_fwd_tc(const float* feat, const float* view_bias, const int64_t* ray_id, const float* W1k, const float* W2, const float* b2,
+                  const float* W3, const float* b3, int64_t n_pts, float* rgb, float* h1_save, float* h2_save, uint32_t* h1_mask,
+                  int single_pass, void* stream) {
   if (n_pts <= 0) return 0;
   const bool save = h1_save != nullptr && h2_save != nullptr;
   const bool one = (single_pass & 1) != 0, four = (single_pass & 2) != 0, panel = save && (single_pass & 4) != 0;
   cudaStream_t st = as_stream(stream);
 #define UBN_FWD(SAVE, THREE, W) \
-  return launch_fwd_p<SAVE, THREE, W>(panel, feat, view_bias, ray_id, W1k, W2, b2, W3, b3, n_pts, rgb, h1_save, h2_save, h1_mask, st)
+  return launch_fwd_p<kF, SAVE, THREE, W>(panel, feat, view_bias, ray_id, W1k, W2, b2, W3, b3, n_pts, rgb, h1_save, h2_save, h1_mask, st)
   if (save) {
     if (one) { if (four) UBN_FWD(true, false, 4); else UBN_FWD(true, false, 8); }
     if (four) UBN_FWD(true, true, 4); else UBN_FWD(true, true, 8);
@@ -832,34 +918,23 @@ extern "C" int ubn_rgbnet_fwd_tc(const float* feat, const float* view_bias, cons
 #undef UBN_FWD
 }
 
-extern "C" int ubn_rgbnet_bwd_tc_data(const float* W2, const float* W3, const float* rgb, const float* h1_save,
-                                      const float* h2_save, const float* grad_rgb, int64_t n_pts, float* dz1_out,
-                                      float* grad_W2, void* stream) {
+template <int kF>
+int rgbnet_bwd_tc_fused(const float* feat, const int64_t* ray_id, const float* W1k, const float* W2, const float* W3, const float* rgb,
+                        const float* h1_save, const float* h2_save, const float* grad_rgb, int64_t n_pts, float* grad_feat,
+                        float* grad_view_bias, float* grad_W1k, float* grad_W2, float* grad_b2, float* grad_W3, float* grad_b3,
+                        uint32_t* h2_mask_scratch, const uint32_t* h1_mask, int single_pass, void* stream) {
   if (n_pts <= 0) return 0;
   cudaStream_t st = as_stream(stream);
-  if (int e = launch_bwd<true, 8, false, false, true>(nullptr, nullptr, nullptr, W2, W3, rgb, h1_save, h2_save, grad_rgb, n_pts,
-                                                     nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                                     dz1_out, st))
-    return e;
-  return launch_dw2<true, false, false>(W3, rgb, h1_save, h2_save, nullptr, grad_rgb, n_pts, grad_W2, st);
-}
-
-extern "C" int ubn_rgbnet_bwd_tc_fused(const float* feat, const int64_t* ray_id, const float* W1k, const float* W2, const float* W3,
-                                       const float* rgb, const float* h1_save, const float* h2_save, const float* grad_rgb,
-                                       int64_t n_pts, float* grad_feat, float* grad_view_bias, float* grad_W1k, float* grad_W2,
-                                       float* grad_b2, float* grad_W3, float* grad_b3, uint32_t* h2_mask_scratch,
-                                       const uint32_t* h1_mask, int single_pass, void* stream) {
-  if (n_pts <= 0) return 0;
-  cudaStream_t st = as_stream(stream);
-  const bool one = (single_pass & 1) != 0, four = (single_pass & 2) != 0, panel = (single_pass & 4) != 0;
+  // kF = 15: three more sum rows per warp -- 8 warps would need 240 640 B of shared memory (the limit is 232 448 B), so 4 warps
+  const bool one = (single_pass & 1) != 0, four = (single_pass & 2) != 0 || kF > 12, panel = (single_pass & 4) != 0;
   const bool mask1 = panel && h1_mask != nullptr, mask2 = panel && h2_mask_scratch != nullptr;
   uint32_t* m2 = mask2 ? h2_mask_scratch : nullptr;
   int e = 0;
 #define UBN_BWD(THREE, W, P, M1)                                                                                              \
-  e = launch_bwd<THREE, W, P, M1, false>(feat, ray_id, W1k, W2, W3, rgb, h1_save, h2_save, grad_rgb, n_pts, grad_feat,        \
+  e = launch_bwd<kF, THREE, W, P, M1, false>(feat, ray_id, W1k, W2, W3, rgb, h1_save, h2_save, grad_rgb, n_pts, grad_feat,        \
                                          grad_view_bias, grad_W1k, grad_b2, grad_W3, grad_b3, m2, h1_mask, nullptr, st)
 #define UBN_BWD_W(THREE, P, M1) \
-  do { if (four) UBN_BWD(THREE, 4, P, M1); else UBN_BWD(THREE, 8, P, M1); } while (0)
+  do { if (four) UBN_BWD(THREE, 4, P, M1); else if constexpr (kF <= 12) UBN_BWD(THREE, 8, P, M1); } while (0)
 #define UBN_BWD_T(P, M1) \
   do { if (one) UBN_BWD_W(false, P, M1); else UBN_BWD_W(true, P, M1); } while (0)
   if (mask1) UBN_BWD_T(true, true);
@@ -874,4 +949,65 @@ extern "C" int ubn_rgbnet_bwd_tc_fused(const float* feat, const int64_t* ray_id,
   if (panel) { if (one) UBN_DW(false, true, false); else UBN_DW(true, true, false); }
   if (one) UBN_DW(false, false, false); else UBN_DW(true, false, false);
 #undef UBN_DW
+}
+
+}  // namespace
+
+extern "C" int ubn_rgbnet_fwd_tc(const float* feat, const float* view_bias, const int64_t* ray_id, const float* W1k,
+                                 const float* W2, const float* b2, const float* W3, const float* b3, int64_t n_pts,
+                                 float* rgb, float* h1_save, float* h2_save, uint32_t* h1_mask, int single_pass, void* stream) {
+  return rgbnet_fwd_tc<tc::kFeat>(feat, view_bias, ray_id, W1k, W2, b2, W3, b3, n_pts, rgb, h1_save, h2_save, h1_mask, single_pass,
+                                  stream);
+}
+
+extern "C" int ubn_rgbnet_fwd_tc_k(int n_feat, const float* feat, const float* view_bias, const int64_t* ray_id, const float* W1k,
+                                   const float* W2, const float* b2, const float* W3, const float* b3, int64_t n_pts, float* rgb,
+                                   float* h1_save, float* h2_save, uint32_t* h1_mask, int single_pass, void* stream) {
+#define UBN_FWD_K(F) \
+  return rgbnet_fwd_tc<F>(feat, view_bias, ray_id, W1k, W2, b2, W3, b3, n_pts, rgb, h1_save, h2_save, h1_mask, single_pass, stream)
+  switch (n_feat) {
+    case 3: UBN_FWD_K(3);
+    case 12: UBN_FWD_K(12);
+    case 15: UBN_FWD_K(15);
+    default: return finish(cudaErrorInvalidValue);
+  }
+#undef UBN_FWD_K
+}
+
+extern "C" int ubn_rgbnet_bwd_tc_data(const float* W2, const float* W3, const float* rgb, const float* h1_save,
+                                      const float* h2_save, const float* grad_rgb, int64_t n_pts, float* dz1_out,
+                                      float* grad_W2, void* stream) {
+  if (n_pts <= 0) return 0;
+  cudaStream_t st = as_stream(stream);
+  if (int e = launch_bwd<tc::kFeat, true, 8, false, false, true>(nullptr, nullptr, nullptr, W2, W3, rgb, h1_save, h2_save, grad_rgb, n_pts,
+                                                     nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                                     dz1_out, st))
+    return e;
+  return launch_dw2<true, false, false>(W3, rgb, h1_save, h2_save, nullptr, grad_rgb, n_pts, grad_W2, st);
+}
+
+extern "C" int ubn_rgbnet_bwd_tc_fused(const float* feat, const int64_t* ray_id, const float* W1k, const float* W2, const float* W3,
+                                       const float* rgb, const float* h1_save, const float* h2_save, const float* grad_rgb,
+                                       int64_t n_pts, float* grad_feat, float* grad_view_bias, float* grad_W1k, float* grad_W2,
+                                       float* grad_b2, float* grad_W3, float* grad_b3, uint32_t* h2_mask_scratch,
+                                       const uint32_t* h1_mask, int single_pass, void* stream) {
+  return rgbnet_bwd_tc_fused<tc::kFeat>(feat, ray_id, W1k, W2, W3, rgb, h1_save, h2_save, grad_rgb, n_pts, grad_feat, grad_view_bias,
+                                        grad_W1k, grad_W2, grad_b2, grad_W3, grad_b3, h2_mask_scratch, h1_mask, single_pass, stream);
+}
+
+extern "C" int ubn_rgbnet_bwd_tc_fused_k(int n_feat, const float* feat, const int64_t* ray_id, const float* W1k, const float* W2,
+                                         const float* W3, const float* rgb, const float* h1_save, const float* h2_save,
+                                         const float* grad_rgb, int64_t n_pts, float* grad_feat, float* grad_view_bias, float* grad_W1k,
+                                         float* grad_W2, float* grad_b2, float* grad_W3, float* grad_b3, uint32_t* h2_mask_scratch,
+                                         const uint32_t* h1_mask, int single_pass, void* stream) {
+#define UBN_BWD_K(F)                                                                                                             \
+  return rgbnet_bwd_tc_fused<F>(feat, ray_id, W1k, W2, W3, rgb, h1_save, h2_save, grad_rgb, n_pts, grad_feat, grad_view_bias, \
+                                grad_W1k, grad_W2, grad_b2, grad_W3, grad_b3, h2_mask_scratch, h1_mask, single_pass, stream)
+  switch (n_feat) {
+    case 3: UBN_BWD_K(3);
+    case 12: UBN_BWD_K(12);
+    case 15: UBN_BWD_K(15);
+    default: return finish(cudaErrorInvalidValue);
+  }
+#undef UBN_BWD_K
 }
