@@ -321,9 +321,10 @@ int ubn_exclusive_scan_i32(const int32_t* in, int64_t n, int64_t* offsets, int64
  * launches.  Returns cudaErrorInvalidValue for other values. */
 int ubn_set_feature_kernel(int variant);
 int ubn_get_feature_kernel(void);
-/* How ubn_march_density_bwd scatters into the density-grid gradient (contiguous single-channel grids): 1 (the default) = two-phase
- * kernel whose second phase walks runs of consecutive samples per lane and merges the contributions of samples that stay in the same
- * cell before they leave as pair reductions; 0 = every sample scatters its own 8 corners.  Same sums up to fp32 addition order.
+/* How ubn_march_density_bwd scatters into the density-grid gradient (contiguous single-channel grids): 1 (the default) = two
+ * launches, the reverse scan writing per-sample gradients to gd_scratch, then a frequency-major scatter that walks runs of
+ * consecutive samples per lane and merges the contributions of samples that stay in the same cell before they leave as pair
+ * reductions; 0 = every sample scatters its own 8 corners from the scan kernel.  Same sums up to fp32 addition order.
  * Process-wide like ubn_set_feature_kernel. */
 int ubn_set_density_scatter(int variant);
 int ubn_get_density_scatter(void);
@@ -359,13 +360,15 @@ int ubn_march_feature_bwd(const float* rays_o, const float* rays_d, const float*
                           float* grad_k0, void* stream);
 
 /* Backward of pass A: grads wrt compacted weights / alpha / density and alphainv_last -> exact reverse
- * scan (alpha2weight_backward arithmetic) -> raw2alpha_backward -> scatter into grad_density. */
+ * scan (alpha2weight_backward arithmetic) -> raw2alpha_backward -> scatter into grad_density.
+ * gd_scratch: device float[n_rays * S] (S = the records' stride) that the run scatter passes the per-sample gradients through
+ * from its first launch to its second; its contents are overwritten.  May be NULL only under ubn_set_density_scatter(0). */
 int ubn_march_density_bwd(const float* rays_o, const float* rays_d, const float* t_table,
                           const UbnGridDesc* density_desc, const UbnMarchCfg* cfg, int64_t n_rays,
                           const float* density, const float* alpha, const float* weight, const float* T,
                           const uint8_t* flags, const float* alphainv_last, const int64_t* offsets,
                           const float* g_weight, const float* g_alpha, const float* g_density,
-                          const float* g_last, float* grad_density_grid, void* stream);
+                          const float* g_last, float* grad_density_grid, float* gd_scratch, void* stream);
 
 /* ---- fused NDC ray march for the forward-facing model DirectMPIGO.forward (FourierGrid/dmpigo.py:224-340):
  *      sample_ndc_pts_on_rays + bbox drop + mask cache + (density + act_shift) + Raw2Alpha(shift 0) + Alphas2Weights + both
@@ -409,12 +412,12 @@ int ubn_march_ndc_feature_bwd(const float* rays_o, const float* rays_d, const Ub
                               float* grad_k0, void* stream);
 
 /* Backward of pass A: exact reverse scan (alpha2weight_backward) -> raw2alpha_backward -> scatter into the density-grid gradient.
- * act_shift gets no gradient (requires_grad = False, dmpigo.py:50). */
+ * act_shift gets no gradient (requires_grad = False, dmpigo.py:50).  gd_scratch as for ubn_march_density_bwd. */
 int ubn_march_ndc_density_bwd(const float* rays_o, const float* rays_d, const UbnGridDesc* density_desc,
                               const UbnNdcMarchCfg* cfg, int64_t n_rays, const float* density, const float* alpha,
                               const float* weight, const float* T, const uint8_t* flags, const float* alphainv_last,
                               const int64_t* offsets, const float* g_weight, const float* g_alpha, const float* g_last,
-                              float* grad_density_grid, void* stream);
+                              float* grad_density_grid, float* gd_scratch, void* stream);
 
 /* ---- fused box march for the bounded-scene model DirectVoxGO.forward (FourierGrid/dvgo.py:306-397): sample_pts_on_rays +
  *      in-box drop + mask cache + density + Raw2Alpha + Alphas2Weights + both thresholds + k0 query.  Same three-launch forward
@@ -455,12 +458,13 @@ int ubn_march_box_feature_fwd(const float* rays_o, const float* rays_d, const fl
 int ubn_march_box_feature_bwd(const float* rays_o, const float* rays_d, const UbnGridDesc* k0_desc, const UbnBoxMarchCfg* cfg,
                               int64_t n_rays, const uint8_t* flags, const int64_t* offsets, const float* grad_feat,
                               float* grad_k0, void* stream);
-/* Backward of pass A: exact reverse scan -> raw2alpha_backward -> scatter into the density-grid gradient. */
+/* Backward of pass A: exact reverse scan -> raw2alpha_backward -> scatter into the density-grid gradient.  gd_scratch as for
+ * ubn_march_density_bwd, with S = cfg->s_max. */
 int ubn_march_box_density_bwd(const float* rays_o, const float* rays_d, const UbnGridDesc* density_desc,
                               const UbnBoxMarchCfg* cfg, int64_t n_rays, const float* density, const float* alpha,
                               const float* weight, const float* T, const uint8_t* flags, const float* alphainv_last,
                               const int64_t* offsets, const float* g_weight, const float* g_alpha, const float* g_last,
-                              float* grad_density_grid, void* stream);
+                              float* grad_density_grid, float* gd_scratch, void* stream);
 
 /* ---- rgbnet: rgb = sigmoid(rgbnet(cat[k0_feat, viewdirs_emb[ray_id]])) (FourierGrid_model.py:231-242,631-637;
  *      dcvgo.py:103-114,337-342) for the 3-layer, width-128, 12-feature configuration every shipped config uses.

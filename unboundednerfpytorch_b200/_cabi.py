@@ -113,7 +113,7 @@ _SIGNATURES = {
     'ubn_march_feature_bwd': [c_p, c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnMarchCfg), c_i64,
                               c_p, c_p, c_p, c_p, c_p],
     'ubn_march_density_bwd': [c_p, c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnMarchCfg), c_i64,
-                              c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
+                              c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
     'ubn_march_ndc_density_fwd': [c_p, c_p, c_p, ctypes.POINTER(UbnGridDesc), c_p, ctypes.POINTER(UbnGridDesc), c_p,
                                   ctypes.POINTER(UbnNdcMarchCfg), c_i64, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
     'ubn_march_ndc_feature_fwd': [c_p, c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnNdcMarchCfg), c_i64,
@@ -121,7 +121,7 @@ _SIGNATURES = {
     'ubn_march_ndc_feature_bwd': [c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnNdcMarchCfg), c_i64,
                                   c_p, c_p, c_p, c_p, c_p],
     'ubn_march_ndc_density_bwd': [c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnNdcMarchCfg), c_i64,
-                                  c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
+                                  c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
     'ubn_march_box_density_fwd': [c_p, c_p, c_p, ctypes.POINTER(UbnGridDesc), c_p, ctypes.POINTER(UbnBoxMarchCfg), c_i64,
                                   c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
     'ubn_march_box_feature_fwd': [c_p, c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnBoxMarchCfg), c_i64,
@@ -129,7 +129,7 @@ _SIGNATURES = {
     'ubn_march_box_feature_bwd': [c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnBoxMarchCfg), c_i64,
                                   c_p, c_p, c_p, c_p, c_p],
     'ubn_march_box_density_bwd': [c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnBoxMarchCfg), c_i64,
-                                  c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
+                                  c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
 }
 _RESTYPE = {'ubn_last_error_string': ctypes.c_char_p, 'ubn_launch_count': c_i64, 'ubn_reset_launch_count': None}
 

@@ -243,12 +243,9 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_feature(
 // ------------------------------------------------------------------------------------------------
 constexpr int kMaxChunks = 128;   // S <= 4096
 
-// kRuns (kP > 0 only): the scatter is a SECOND phase with lane = a run of consecutive samples of the ray.  Phase 1 (reverse scan,
-// lane = sample of a 32-sample chunk) parks the per-sample density gradients in shared memory; in phase 2 every lane walks its
-// ceil(S / 32) consecutive samples slab by slab and keeps the cell it is in open in registers (cell index + its 8 corner sums):
-// samples that stay in the cell -- a large share of the steps in slab 0 and the lowest sin / cos slabs at half-voxel spacing -- are added in
-// registers, and a cell leaves as four pair reductions only when the ray moves on.  The scatter is bound by the count of L2
-// reduction requests (profiled: the L2 reduction path saturates while issue stays low), so fewer requests is the only lever.
+// kRuns (kP > 0 only): launch 1 of the run scatter.  The reverse scan (lane = sample of a 32-sample chunk) writes every sample's
+// density gradient, already divided by the slab count, to gd_out[ray * S + s] and scatters nothing; k_march_density_scatter
+// (launch 2) adds them into the grid.  Otherwise every sample scatters its own 8 corners in every slab right here.
 template <class Smp, int kP, bool kRuns>
 __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_bwd(
     const float* __restrict__ rays_o, const float* __restrict__ rays_d, const float* __restrict__ t_table,
@@ -256,10 +253,9 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_bwd(
     const float* __restrict__ alpha, const float* __restrict__ weight, const float* __restrict__ T,
     const uint8_t* __restrict__ flags, const float* __restrict__ last, const int64_t* __restrict__ offsets,
     const float* __restrict__ g_weight, const float* __restrict__ g_alpha, const float* __restrict__ g_density,
-    const float* __restrict__ g_last, float* __restrict__ grad_grid) {
+    const float* __restrict__ g_last, float* __restrict__ grad_grid, float* __restrict__ gd_out) {
   __shared__ int s_cnt[kMarchWarps][kMaxChunks];
   __shared__ __align__(16) float2 s_pair[kMarchWarps][32];
-  extern __shared__ float s_gd_all[];                      // kRuns: [kMarchWarps][S + 33] parked gradients, index s + s / L
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int64_t ray = (int64_t)blockIdx.x * kMarchWarps + w;
   if (ray >= n_rays) return;
@@ -267,8 +263,6 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_bwd(
   const int S = p.S;                                       // record stride
   const int n = r.n;                                       // samples of this ray (S, or the box march's n_steps)
   const int n_chunks = (n + 31) / 32;
-  const int L = n_chunks;                                  // kRuns: consecutive samples per lane in phase 2 (= ceil(n / 32))
-  float* s_gd = s_gd_all + w * (S + 33);                   // index s + s / L < n + 32 <= S + 33
 
   // exclusive prefix of KEEP counts per chunk -> compact index of every kept sample
   int run = 0;
@@ -329,8 +323,8 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_bwd(
         gd += (float)(fmin((double)e, 1e10) * powf(1 + e, -p.interval - 1) * p.interval * ga);
       }
     }
-    if (kRuns) {                                           // park it (already divided by the slab count) for phase 2
-      if (valid) s_gd[s + s / L] = slab_mean_scale(gd, g.P);
+    if (kRuns) {
+      if (valid) gd_out[i] = slab_mean_scale(gd, g.P);
       continue;
     }
     if (gd == 0.f) continue;
@@ -354,11 +348,32 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_bwd(
       else trilerp1_scatter(grad_grid + sl * g.sp, g.sv, g.X, g.Y, g.Z, cx, cy, cz, gd);
     }
   }
-  if (!kRuns || kP <= 0) return;
+}
 
-  // ---- phase 2: lane = samples lane * L .. lane * L + L - 1, one pass per frequency (slab 0 | sin, cos of 2^k x) ----
-  __syncwarp();
-  constexpr int kPP = kP > 0 ? kP : 1;
+// Launch 2 of the run scatter: adds launch 1's per-sample gradients gd[ray * S + s] into the density-grid gradient.
+// Warp = ray, lane = a run of L = ceil(n / 32) consecutive samples.  The lane keeps the cell it is in open in registers (cell
+// index + its 8 corner sums): samples that stay in the cell -- a large share of the steps in slab 0 and the lowest sin / cos slabs
+// at half-voxel spacing -- are added in registers, and a cell leaves as four pair reductions only when the ray moves on.  The
+// scatter is bound by L2 reduction requests, so it needs both few requests and requests that hit in L2.
+// Frequency-major: blockIdx.y = k * n_split + part.  Pass k = 0 scatters slab 0, pass k > 0 the sin / cos slab pair 2k - 1 / 2k
+// (one sincosf per axis serves both).  The CTAs of one blockIdx.y are scheduled before those of the next, so the live part of the
+// gradient is one slab or one pair instead of all P slabs (129 MB for the 153^3 x 9 truck grid, against the H100's 50 MB L2).
+// n_split > 1 cuts it further into x-ranges, as k_march_feature_bwd_slab does: part `part` adds only the cells whose base voxel
+// lies in its range of x planes.
+template <class Smp, int kP>
+__global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_scatter(
+    const float* __restrict__ rays_o, const float* __restrict__ rays_d, const float* __restrict__ t_table, GridView g,
+    MarchParams p, int64_t n_rays, const float* __restrict__ gd_in, float* __restrict__ grad_grid, int n_split) {
+  const int lane = threadIdx.x & 31;
+  const int64_t ray = (int64_t)blockIdx.x * kMarchWarps + (threadIdx.x >> 5);
+  if (ray >= n_rays) return;
+  const int k = blockIdx.y / n_split, part = blockIdx.y - k * n_split;
+  const int v_lo = (int)(((int64_t)(g.X - 1) * part) / n_split) * g.Y * g.Z;
+  const int v_hi = (part + 1 == n_split) ? 0x7fffffff : (int)(((int64_t)(g.X - 1) * (part + 1)) / n_split) * g.Y * g.Z;
+  const Ray r = Smp::load(rays_o + 3 * ray, rays_d + 3 * ray, p);
+  const int n = r.n;
+  const int L = (n + 31) / 32;
+  const float* gd_ray = gd_in + ray * p.S;
   const int dY = g.Z, dX = g.Y * g.Z;
   struct Run { int v; float c[8]; };
   auto flush = [&](const Run& run, float* slab) {          // the four (x, y) edges of the open cell as pair reductions
@@ -374,6 +389,7 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_bwd(
   };
   auto visit = [&](Run& run, float* slab, float cx, float cy, float cz, float gd) {
     const CellR c = make_cell(cx, cy, cz, g.X, g.Y, g.Z);
+    if (c.v < v_lo || c.v >= v_hi) return;                 // another part's cell
     float wgt[8];
 #pragma unroll
     for (int e = 0; e < 4; ++e) {                          // same products as grid_density_scatter_fast: ((wz * wy) * wx) * gd
@@ -392,38 +408,35 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_bwd(
       for (int q = 0; q < 8; ++q) run.c[q] = wgt[q];
     }
   };
-#pragma unroll 1
-  for (int k = 0; k <= (kPP - 1) / 2; ++k) {
-    Run ra, rb;
-    ra.v = -1; rb.v = -1;
-    float* slab_a = grad_grid + (int64_t)(k == 0 ? 0 : 2 * k - 1) * g.sp;
-    float* slab_b = grad_grid + (int64_t)(2 * k) * g.sp;
-    const float m = (float)(1 << (k > 0 ? k - 1 : 0));
-    for (int i = 0; i < L; ++i) {
-      const int s = lane * L + i;
-      if (s >= n) break;
-      const float gd = s_gd[s + lane];
-      if (gd == 0.f) continue;
-      float x, y, z;
-      bool inner;
-      Smp::point(r, t_table, s, p, x, y, z, inner);
-      const float nx = norm_coord(x, g.mn[0], g.len[0]);
-      const float ny = norm_coord(y, g.mn[1], g.len[1]);
-      const float nz = norm_coord(z, g.mn[2], g.len[2]);
-      if (k == 0) {
-        visit(ra, slab_a, src_index(nx, g.X), src_index(ny, g.Y), src_index(nz, g.Z), gd);
-      } else {
-        float sx, cx, sy, cy, sz, cz;
-        sincosf(__fmul_rn(m, nx), &sx, &cx);
-        sincosf(__fmul_rn(m, ny), &sy, &cy);
-        sincosf(__fmul_rn(m, nz), &sz, &cz);
-        visit(ra, slab_a, src_index(sx, g.X), src_index(sy, g.Y), src_index(sz, g.Z), gd);
-        visit(rb, slab_b, src_index(cx, g.X), src_index(cy, g.Y), src_index(cz, g.Z), gd);
-      }
+  Run ra, rb;
+  ra.v = -1; rb.v = -1;
+  float* slab_a = grad_grid + (int64_t)(k == 0 ? 0 : 2 * k - 1) * g.sp;
+  float* slab_b = grad_grid + (int64_t)(2 * k) * g.sp;
+  const float m = (float)(1 << (k > 0 ? k - 1 : 0));
+  for (int i = 0; i < L; ++i) {
+    const int s = lane * L + i;
+    if (s >= n) break;
+    const float gd = gd_ray[s];
+    if (gd == 0.f) continue;
+    float x, y, z;
+    bool inner;
+    Smp::point(r, t_table, s, p, x, y, z, inner);
+    const float nx = norm_coord(x, g.mn[0], g.len[0]);
+    const float ny = norm_coord(y, g.mn[1], g.len[1]);
+    const float nz = norm_coord(z, g.mn[2], g.len[2]);
+    if (kP == 1 || k == 0) {
+      visit(ra, slab_a, src_index(nx, g.X), src_index(ny, g.Y), src_index(nz, g.Z), gd);
+    } else {
+      float sx, cx, sy, cy, sz, cz;
+      sincosf(__fmul_rn(m, nx), &sx, &cx);
+      sincosf(__fmul_rn(m, ny), &sy, &cy);
+      sincosf(__fmul_rn(m, nz), &sz, &cz);
+      visit(ra, slab_a, src_index(sx, g.X), src_index(sy, g.Y), src_index(sz, g.Z), gd);
+      visit(rb, slab_b, src_index(cx, g.X), src_index(cy, g.Y), src_index(cz, g.Z), gd);
     }
-    if (ra.v >= 0) flush(ra, slab_a);
-    if (rb.v >= 0) flush(rb, slab_b);
   }
+  if (ra.v >= 0) flush(ra, slab_a);
+  if (rb.v >= 0) flush(rb, slab_b);
 }
 
 // the fast density paths need: contiguous single channel, >= 2 voxels per axis, 32-bit offsets inside a slab, and an 8-byte aligned
@@ -445,7 +458,7 @@ int march_feature_v2(bool backward, const float* rays_o, const float* rays_d, co
 
 void set_feature_kernel(int v);
 int get_feature_kernel();
-static int g_density_scatter = 1;      // 1 = run-merging two-phase scatter (default), 0 = per-sample scatter
+static int g_density_scatter = 1;      // 1 = run-merging two-launch scatter (default), 0 = per-sample scatter
 static int get_density_scatter() { return g_density_scatter; }
 
 static bool feature_grid_ok(const GridView& g) {
@@ -481,42 +494,77 @@ static int launch_density_fwd(const float* rays_o, const float* rays_d, const fl
   return 0;
 }
 
+// x-ranges per frequency pass of k_march_density_scatter.  A pass reduces into its live part of the gradient (one slab, or a
+// sin / cos pair) while the per-sample gradients stream through the same L2; n_split = ceil((live part + per-sample gradients) /
+// (3/4 of the L2)).  A rule fit to measurements on an H100 (50 MB L2, launch 2's time by split count): truck, 153^3 x 9 slabs,
+// 8192 x 512 samples -> 2 (1 / 2 / 4: 1.66 / 1.57 / 1.88 ms for both launches); bicycle, one 320^3 slab -> 4 (1 / 2 / 4 / 8: 0.33 /
+// 0.28 / 0.29 / 0.40 ms).  Fewer parts leave the reductions missing in L2, more repeat the per-sample work of the pass.
+static int density_scatter_split(const GridView& g, int kP, int64_t n_samples, int& n_split) {
+  int dev = 0, l2 = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev);
+  if (e != cudaSuccess) return finish(e);
+  const int64_t live = (int64_t)(kP > 1 ? 2 : 1) * g.X * g.Y * g.Z * (int64_t)sizeof(float);
+  const int64_t need = live + n_samples * (int64_t)sizeof(float);
+  const int64_t budget = std::max<int64_t>((int64_t)l2 * 3 / 4, 1);
+  n_split = (int)std::min<int64_t>((need + budget - 1) / budget, g.X - 1);
+  return 0;
+}
+
+template <class Smp, int kP>
+static int launch_density_bwd_p(const float* rays_o, const float* rays_d, const float* t_table, const GridView& g,
+                                const MarchParams& p, int64_t n_rays, const float* density, const float* alpha,
+                                const float* weight, const float* T, const uint8_t* flags, const float* alphainv_last,
+                                const int64_t* offsets, const float* g_weight, const float* g_alpha, const float* g_density,
+                                const float* g_last, float* grad_density_grid, float* gd_scratch, cudaStream_t st) {
+  const unsigned blocks = blocks_for(n_rays, kMarchWarps);
+  // run-merging scatter (two launches) by default; ubn_set_density_scatter(0) selects the per-sample scatter (A/B, tests)
+  if constexpr (kP > 0) {
+    if (get_density_scatter() == 1) {
+      if (!gd_scratch) return finish(cudaErrorInvalidValue);
+      int n_split = 1;
+      if (const int e = density_scatter_split(g, kP, n_rays * p.S, n_split)) return e;
+      k_march_density_bwd<Smp, kP, true><<<blocks, 32 * kMarchWarps, 0, st>>>(
+          rays_o, rays_d, t_table, g, p, n_rays, density, alpha, weight, T, flags, alphainv_last, offsets, g_weight, g_alpha,
+          g_density, g_last, grad_density_grid, gd_scratch);
+      UBN_LAUNCH_CHECK();
+      k_march_density_scatter<Smp, kP><<<dim3(blocks, (kP + 1) / 2 * n_split), 32 * kMarchWarps, 0, st>>>(
+          rays_o, rays_d, t_table, g, p, n_rays, gd_scratch, grad_density_grid, n_split);
+      UBN_LAUNCH_CHECK();
+      return 0;
+    }
+  }
+  k_march_density_bwd<Smp, kP, false><<<blocks, 32 * kMarchWarps, 0, st>>>(
+      rays_o, rays_d, t_table, g, p, n_rays, density, alpha, weight, T, flags, alphainv_last, offsets, g_weight, g_alpha,
+      g_density, g_last, grad_density_grid, nullptr);
+  UBN_LAUNCH_CHECK();
+  return 0;
+}
+
 template <class Smp>
 static int launch_density_bwd(const float* rays_o, const float* rays_d, const float* t_table, const GridView& g,
                               const MarchParams& p, int64_t n_rays, const float* density, const float* alpha, const float* weight,
                               const float* T, const uint8_t* flags, const float* alphainv_last, const int64_t* offsets,
                               const float* g_weight, const float* g_alpha, const float* g_density, const float* g_last,
-                              float* grad_density_grid, cudaStream_t st) {
-  // run-merging scatter (two-phase kernel) by default; ubn_set_density_scatter(0) selects the per-sample scatter (A/B, tests)
-  const size_t smem_runs = sizeof(float) * kMarchWarps * (size_t)(p.S + 33);
-  const bool runs = get_density_scatter() == 1 && smem_runs <= 40 * 1024;
-#define UBN_DBWD(P)                                                                                                  \
-  do {                                                                                                               \
-    if (runs && (P) > 0)                                                                                             \
-      k_march_density_bwd<Smp, P, true><<<blocks_for(n_rays, kMarchWarps), 32 * kMarchWarps, smem_runs, st>>>(     \
-          rays_o, rays_d, t_table, g, p, n_rays, density, alpha, weight, T, flags, alphainv_last, offsets, g_weight,  \
-          g_alpha, g_density, g_last, grad_density_grid);                                                            \
-    else                                                                                                             \
-      k_march_density_bwd<Smp, P, false><<<blocks_for(n_rays, kMarchWarps), 32 * kMarchWarps, 0, st>>>(            \
-          rays_o, rays_d, t_table, g, p, n_rays, density, alpha, weight, T, flags, alphainv_last, offsets, g_weight,  \
-          g_alpha, g_density, g_last, grad_density_grid);                                                            \
-  } while (0)
+                              float* grad_density_grid, float* gd_scratch, cudaStream_t st) {
+#define UBN_DBWD(P)                                                                                                      \
+  return launch_density_bwd_p<Smp, P>(rays_o, rays_d, t_table, g, p, n_rays, density, alpha, weight, T, flags,          \
+                                      alphainv_last, offsets, g_weight, g_alpha, g_density, g_last, grad_density_grid,  \
+                                      gd_scratch, st)
   if constexpr (std::is_same<Smp, BoxSampler>::value) {
     if (density_fast_slabs(g) != 1) return finish(cudaErrorInvalidValue);
     UBN_DBWD(1);
   } else {
     switch (density_fast_slabs(g)) {
-      case 1: UBN_DBWD(1); break;
-      case 3: UBN_DBWD(3); break;
-      case 5: UBN_DBWD(5); break;
-      case 7: UBN_DBWD(7); break;
-      case 9: UBN_DBWD(9); break;
-      default: UBN_DBWD(0); break;
+      case 1: UBN_DBWD(1);
+      case 3: UBN_DBWD(3);
+      case 5: UBN_DBWD(5);
+      case 7: UBN_DBWD(7);
+      case 9: UBN_DBWD(9);
+      default: UBN_DBWD(0);
     }
   }
 #undef UBN_DBWD
-  UBN_LAUNCH_CHECK();
-  return 0;
 }
 
 }  // namespace ubn
@@ -603,7 +651,7 @@ int ubn_march_density_bwd(const float* rays_o, const float* rays_d, const float*
                           const float* alpha, const float* weight, const float* T, const uint8_t* flags,
                           const float* alphainv_last, const int64_t* offsets, const float* g_weight,
                           const float* g_alpha, const float* g_density, const float* g_last, float* grad_density_grid,
-                          void* stream) {
+                          float* gd_scratch, void* stream) {
   if (n_rays <= 0) return 0;
   const GridView g = make_view(grad_density_grid, density_desc);
   if (g.C != 1) return finish(cudaErrorInvalidValue);
@@ -611,7 +659,7 @@ int ubn_march_density_bwd(const float* rays_o, const float* rays_d, const float*
   if (p.S > 32 * kMaxChunks) return finish(cudaErrorInvalidValue);
   return launch_density_bwd<ContractedSampler>(rays_o, rays_d, t_table, g, p, n_rays, density, alpha, weight, T, flags,
                                                alphainv_last, offsets, g_weight, g_alpha, g_density, g_last, grad_density_grid,
-                                               as_stream(stream));
+                                               gd_scratch, as_stream(stream));
 }
 
 int ubn_march_ndc_density_fwd(const float* rays_o, const float* rays_d, const float* density_grid,
@@ -633,7 +681,7 @@ int ubn_march_ndc_density_bwd(const float* rays_o, const float* rays_d, const Ub
                               const UbnNdcMarchCfg* cfg, int64_t n_rays, const float* density, const float* alpha,
                               const float* weight, const float* T, const uint8_t* flags, const float* alphainv_last,
                               const int64_t* offsets, const float* g_weight, const float* g_alpha, const float* g_last,
-                              float* grad_density_grid, void* stream) {
+                              float* grad_density_grid, float* gd_scratch, void* stream) {
   if (n_rays <= 0) return 0;
   const GridView g = make_view(grad_density_grid, density_desc);
   if (g.C != 1 || g.P != 1 || cfg->n_samples < 2) return finish(cudaErrorInvalidValue);
@@ -641,7 +689,8 @@ int ubn_march_ndc_density_bwd(const float* rays_o, const float* rays_d, const Ub
   const MarchParams p = make_ndc_params(cfg, none);
   if (p.S > 32 * kMaxChunks) return finish(cudaErrorInvalidValue);
   return launch_density_bwd<NdcSampler>(rays_o, rays_d, nullptr, g, p, n_rays, density, alpha, weight, T, flags, alphainv_last,
-                                         offsets, g_weight, g_alpha, nullptr, g_last, grad_density_grid, as_stream(stream));
+                                         offsets, g_weight, g_alpha, nullptr, g_last, grad_density_grid, gd_scratch,
+                                         as_stream(stream));
 }
 
 // S_max (cfg->s_max) is the record stride of pass A; the backward's chunk table holds 32 * kMaxChunks samples of a ray
@@ -664,13 +713,14 @@ int ubn_march_box_density_bwd(const float* rays_o, const float* rays_d, const Ub
                               const UbnBoxMarchCfg* cfg, int64_t n_rays, const float* density, const float* alpha,
                               const float* weight, const float* T, const uint8_t* flags, const float* alphainv_last,
                               const int64_t* offsets, const float* g_weight, const float* g_alpha, const float* g_last,
-                              float* grad_density_grid, void* stream) {
+                              float* grad_density_grid, float* gd_scratch, void* stream) {
   if (n_rays <= 0) return 0;
   const GridView g = make_view(grad_density_grid, density_desc);
   if (g.C != 1 || g.P != 1 || !box_cfg_ok(cfg)) return finish(cudaErrorInvalidValue);
   const MarchParams p = make_box_params(cfg, nullptr);
   return launch_density_bwd<BoxSampler>(rays_o, rays_d, nullptr, g, p, n_rays, density, alpha, weight, T, flags, alphainv_last,
-                                        offsets, g_weight, g_alpha, nullptr, g_last, grad_density_grid, as_stream(stream));
+                                        offsets, g_weight, g_alpha, nullptr, g_last, grad_density_grid, gd_scratch,
+                                        as_stream(stream));
 }
 
 }  // extern "C"

@@ -182,11 +182,12 @@ class March(torch.autograd.Function):
                     check(lib.ubn_march_feature_bwd(ptr(rays_o), ptr(rays_d), ptr(t_table), ctx.kdesc, ctx.cfg, c_i64(N),
                                                     ptr(flags), ptr(offsets), ptr(g_feat), ptr(grad_k), stream_of(rays_o)))
             if want_d:
+                gd = torch.empty_like(dens)     # per-sample density gradients between the run scatter's two launches
                 with _cabi.timed('march_density_bwd'):
                     check(lib.ubn_march_density_bwd(ptr(rays_o), ptr(rays_d), ptr(t_table), ctx.ddesc, ctx.cfg, c_i64(N),
                                                     ptr(dens), ptr(alpha), ptr(weight), ptr(T), ptr(flags), ptr(last),
                                                     ptr(offsets), ptr(g_weight), ptr(g_alpha), ptr(g_dens), ptr(g_last),
-                                                    ptr(grad_d), stream_of(rays_o)))
+                                                    ptr(grad_d), ptr(gd), stream_of(rays_o)))
         grad_d = _hand_over(ctx.dparam, grad_d, buf_d)
         grad_k = _hand_over(ctx.kparam, grad_k, buf_k)
         return grad_d, grad_k, None, None, None, None, None, None, None, None, None
@@ -270,10 +271,11 @@ class NdcMarch(torch.autograd.Function):
                     check(lib.ubn_march_ndc_feature_bwd(ptr(rays_o), ptr(rays_d), ctx.kdesc, ctx.cfg, c_i64(N), ptr(flags),
                                                         ptr(offsets), ptr(g_feat), ptr(grad_k), st))
             if want_d:
+                gd = torch.empty_like(dens)
                 with _cabi.timed('march_ndc_density_bwd'):
                     check(lib.ubn_march_ndc_density_bwd(ptr(rays_o), ptr(rays_d), ctx.ddesc, ctx.cfg, c_i64(N), ptr(dens),
                                                         ptr(alpha), ptr(weight), ptr(T), ptr(flags), ptr(last), ptr(offsets),
-                                                        ptr(g_weight), ptr(g_alpha), ptr(g_last), ptr(grad_d), st))
+                                                        ptr(g_weight), ptr(g_alpha), ptr(g_last), ptr(grad_d), ptr(gd), st))
         grad_d = _hand_over(ctx.dparam, grad_d, buf_d)
         grad_k = _hand_over(ctx.kparam, grad_k, buf_k)
         return grad_d, grad_k, None, None, None, None, None, None, None, None
@@ -386,10 +388,11 @@ class BoxMarch(torch.autograd.Function):
                     check(lib.ubn_march_box_feature_bwd(ptr(rays_o), ptr(rays_d), ctx.kdesc, ctx.cfg, c_i64(N), ptr(flags),
                                                         ptr(offsets), ptr(g_feat), ptr(grad_k), st))
             if want_d:
+                gd = torch.empty_like(dens)
                 with _cabi.timed('march_box_density_bwd'):
                     check(lib.ubn_march_box_density_bwd(ptr(rays_o), ptr(rays_d), ctx.ddesc, ctx.cfg, c_i64(N), ptr(dens),
                                                         ptr(alpha), ptr(weight), ptr(T), ptr(flags), ptr(last), ptr(offsets),
-                                                        ptr(g_weight), ptr(g_alpha), ptr(g_last), ptr(grad_d), st))
+                                                        ptr(g_weight), ptr(g_alpha), ptr(g_last), ptr(grad_d), ptr(gd), st))
         grad_d = _hand_over(ctx.dparam, grad_d, buf_d)
         grad_k = _hand_over(ctx.kparam, grad_k, buf_k)
         return grad_d, grad_k, None, None, None, None, None, None

@@ -450,7 +450,7 @@ def get_feature_kernel():
 
 
 def set_density_scatter(variant):
-    """Density-grid scatter of the fused march backward: 1 = run-merging two-phase kernel (default), 0 = per-sample scatter
+    """Density-grid scatter of the fused march backward: 1 = run-merging two-launch scatter (default), 0 = per-sample scatter
     (ubn_set_density_scatter).  Process-wide."""
     from ._cabi import load
     check(load().ubn_set_density_scatter(c_int(int(variant))))
