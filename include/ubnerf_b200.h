@@ -533,6 +533,24 @@ int ubn_rgbnet_bwd_tc_fused_k(int n_feat, const float* feat, const int64_t* ray_
                               int64_t n_pts, float* grad_feat, float* grad_view_bias, float* grad_W1k, float* grad_W2, float* grad_b2,
                               float* grad_W3, float* grad_b3, uint32_t* h2_mask_scratch, const uint32_t* h1_mask, int single_pass,
                               void* stream);
+/* ubn_rgbnet_fwd_tc_k / ubn_rgbnet_bwd_tc_fused_k with the hidden width as an argument (rgbnet_width), for the forward-facing
+ * DirectMPIGO of llff_default (rgbnet_dim = 9, rgbnet_width = 64, viewbase_pe = 0: a 12 -> 64 -> 64 -> 3 MLP; replaces
+ * dmpigo.py:84-92, 297-306).  Every buffer that is 128 wide above is n_hidden wide here: view_bias / grad_view_bias
+ * [n_rays, n_hidden], W1k / grad_W1k [n_hidden, n_feat], W2 / grad_W2 [n_hidden, n_hidden], b2 [n_hidden], W3 [3, n_hidden];
+ * the panel saves hold ceil(n_pts/128)*128 rows of n_hidden floats ([tile][n_hidden/4 column quads][128 rows][4]) and the
+ * ReLU masks ceil(n_pts/128)*128*n_hidden/32 uint32 ([tile][n_hidden/32 chunks][128 rows]).
+ * (n_feat, n_hidden) = (3 | 12 | 15, 128) runs exactly the kernels of the _k pair.  (9, 64): the forward writes saves only in the
+ * panel layout (bit 2 must be set when h1_save / h2_save are given), the backward needs bit 2, h1_mask and h2_mask_scratch, and
+ * bit 1 (4 warps) is ignored: the width-64 kernels have one launch configuration each.  Any other pair, or a width-64 call
+ * without what it needs: cudaErrorInvalidValue. */
+int ubn_rgbnet_fwd_tc_kw(int n_feat, int n_hidden, const float* feat, const float* view_bias, const int64_t* ray_id,
+                         const float* W1k, const float* W2, const float* b2, const float* W3, const float* b3, int64_t n_pts,
+                         float* rgb, float* h1_save, float* h2_save, uint32_t* h1_mask, int single_pass, void* stream);
+int ubn_rgbnet_bwd_tc_fused_kw(int n_feat, int n_hidden, const float* feat, const int64_t* ray_id, const float* W1k,
+                               const float* W2, const float* W3, const float* rgb, const float* h1_save, const float* h2_save,
+                               const float* grad_rgb, int64_t n_pts, float* grad_feat, float* grad_view_bias, float* grad_W1k,
+                               float* grad_W2, float* grad_b2, float* grad_W3, float* grad_b3, uint32_t* h2_mask_scratch,
+                               const uint32_t* h1_mask, int single_pass, void* stream);
 
 #if defined(__GNUC__)
 #pragma GCC visibility pop

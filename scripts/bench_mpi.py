@@ -9,13 +9,18 @@ line:
                      was not built); every leg starts from the same parameters;
 * render_frame_ms -- one 1008x756 frame (762,048 rays) in 8192-ray chunks through the fused forward;
 * kernels_ms      -- per-launch times of the march kernels, and the rgbnet's forward and backward time and share of the fused
-                     step (CUDA events; module hooks around the rgbnet; a separate pass);
+                     step (CUDA events around the C-ABI calls -- ``rgbnet_fwd`` / ``rgbnet_bwd`` of the tensor-core rgbnet, the
+                     per-ray bias GEMM outside them -- or, on the torch rgbnet, module hooks around it; a separate pass);
+* legs            -- with ``--rgbnet kernel,torch``: the fused step, the rgbnet times and share and the frame time of each rgbnet
+                     path (``torch``: shade.supported patched to False, so DirectMPIGO runs its nn.Sequential on cuBLAS), the
+                     legs alternating --runs times in this one process after the top-level figures, which are always
+                     those of the shipped path;
 * march_hbm       -- algorithmic bytes of the march kernels (32 B density + 8 B act_shift + 1 B mask per queried sample in pass A,
                      8 x 36 B per survivor in pass B, doubled for the scatter) over their time, against 3.35 TB/s;
 * outputs         -- fused vs forward_ops at the timed size (max error over scale, survivor sets equal);
 * gpu / power_limit_w -- where it ran, read in the same run.
 
-    python scripts/bench_mpi.py [--steps 20] [--warmup 5] [--rays 4096]
+    python scripts/bench_mpi.py [--steps 20] [--warmup 5] [--rays 4096] [--rgbnet kernel,torch] [--runs 2]
 """
 import argparse
 import json
@@ -129,9 +134,10 @@ def main():
     ap.add_argument('--steps', type=int, default=20)
     ap.add_argument('--warmup', type=int, default=5)
     ap.add_argument('--rays', type=int, default=4096)
+    ap.add_argument('--rgbnet', default='kernel', help="comma-separated rgbnet paths to time in alternation: kernel, torch")
+    ap.add_argument('--runs', type=int, default=2, help='alternating runs of each --rgbnet path')
     args = ap.parse_args()
     assert torch.cuda.is_available(), 'bench_mpi.py needs a GPU'
-    from unboundednerfpytorch_b200 import _cabi
     from unboundednerfpytorch_b200.masked_adam import create_optimizer_or_freeze_model
     name, power = _gpu_info()
     res = dict(metric='llff_default DirectMPIGO', gpu=name, power_limit_w=power, rays=args.rays)
@@ -162,6 +168,79 @@ def main():
         res['speedup_vs_reference_gpu'] = res['train_step_ms']['reference_gpu'] / res['train_step_ms']['fused']
 
     # per-launch times (CUDA events around the C-ABI calls) and the rgbnet's forward / backward, in a pass of its own
+    k, step_ms, rg = _instrumented(m, state0, cfg, ro, rd, vd, target, args)
+    res['kernels_ms'] = k
+    res.update(rg)
+    res['rgbnet_share_of_step'] = (res['rgbnet_fwd_ms'] + res['rgbnet_bwd_ms']) / step_ms
+    res['instrumented_step_ms'] = step_ms
+    # algorithmic bytes of the march kernels at the timed size
+    with torch.no_grad():
+        out = m(ro, rd, vd, **RK)
+        from unboundednerfpytorch_b200 import ops
+        S = m._n_samples(0.5)
+        pts, outb = ops.sample_ndc_pts_on_rays(ro, rd, m.xyz_min, m.xyz_max, S)
+        queried = int(m.mask_cache(pts[~outb]).sum())
+    M = int(out['ray_id'].numel())
+    bytes_a = queried * (32 + 8 + 1)
+    bytes_b = M * 8 * 36
+    t_a = k.get('march_ndc_density_fwd', float('nan'))
+    t_b = k.get('march_ndc_feature_fwd', float('nan'))
+    t_bb = k.get('march_ndc_feature_bwd', float('nan'))
+    res['march_hbm'] = dict(queried=queried, survivors=M, bytes_pass_a=bytes_a, bytes_pass_b=bytes_b,
+                            density_fwd_frac_of_peak=bytes_a / (t_a * 1e-3) / HBM_PEAK,
+                            feature_fwd_frac_of_peak=bytes_b / (t_b * 1e-3) / HBM_PEAK,
+                            feature_bwd_frac_of_peak=2 * bytes_b / (t_bb * 1e-3) / HBM_PEAK)
+
+    # one 1008x756 frame in 8192-ray chunks
+    fro, frd, fvd = rays(1008 * 756)
+    res['render_frame_ms'] = _frame(m, fro, frd, fvd, args)
+    res['render_rays'] = 1008 * 756
+
+    # the rgbnet paths, alternating: fused step, rgbnet times and share, frame
+    legs = [leg.strip() for leg in args.rgbnet.split(',') if leg.strip()]
+    if legs != ['kernel']:
+        res['legs'] = {leg: [] for leg in legs}
+        for _ in range(args.runs):
+            for leg in legs:
+                with _rgbnet_path(leg):
+                    m.load_state_dict(state0)
+                    opt = create_optimizer_or_freeze_model(m, cfg, global_step=0)
+                    step = _time(lambda i: _train_step(m, opt, m.forward, ro, rd, vd, target, i + 1), args.steps, args.warmup)
+                    _, ist, rg = _instrumented(m, state0, cfg, ro, rd, vd, target, args)
+                    res['legs'][leg].append(dict(train_step_ms=step, **rg, rgbnet_share_of_step=(rg['rgbnet_fwd_ms'] + rg['rgbnet_bwd_ms']) / ist,
+                                                 instrumented_step_ms=ist, render_frame_ms=_frame(m, fro, frd, fvd, args)))
+    print(json.dumps(res))
+
+
+def _rgbnet_path(leg):
+    """'kernel': as shipped; 'torch': shade.supported patched to False, so the model runs its nn.Sequential rgbnet"""
+    import contextlib
+    from unboundednerfpytorch_b200 import shade
+    assert leg in ('kernel', 'torch'), leg
+
+    @contextlib.contextmanager
+    def ctx():
+        orig = shade.supported
+        if leg == 'torch':
+            shade.supported = lambda *a, **k: False
+        try:
+            yield
+        finally:
+            shade.supported = orig
+    return ctx()
+
+
+def _frame(m, fro, frd, fvd, args):
+    from unboundednerfpytorch_b200 import render
+    return _time(lambda i: render.render_rays(m, fro, frd, fvd, dict(RK), chunk=8192), max(2, args.steps // 5), 1)
+
+
+def _instrumented(m, state0, cfg, ro, rd, vd, target, args):
+    """One timed pass with CUDA events around the C-ABI calls and module hooks around the rgbnet: per-launch times, the step
+    time of this pass, and the rgbnet's forward / backward ms (the tensor-core rgbnet's ``rgbnet_fwd`` / ``rgbnet_bwd`` ranges,
+    or the hooks when the model ran the torch rgbnet)."""
+    from unboundednerfpytorch_b200 import _cabi
+    from unboundednerfpytorch_b200.masked_adam import create_optimizer_or_freeze_model
     m.load_state_dict(state0)
     opt = create_optimizer_or_freeze_model(m, cfg, global_step=0)
     timer = _cabi.KernelTimer()
@@ -186,36 +265,14 @@ def main():
         for h in hooks:
             h.remove()
     k = {n: v[0] for n, v in timer.summary().items()}
-    res['kernels_ms'] = k
+    rg = {}
     for kind in ('fwd', 'bwd'):
-        ms = sum(s.elapsed_time(e) for s, e in marks[kind][-args.steps:]) / args.steps
-        res[f'rgbnet_{kind}_ms'] = ms
-    res['rgbnet_share_of_step'] = (res['rgbnet_fwd_ms'] + res['rgbnet_bwd_ms']) / step_ms
-    res['instrumented_step_ms'] = step_ms
-    # algorithmic bytes of the march kernels at the timed size
-    with torch.no_grad():
-        out = m(ro, rd, vd, **RK)
-        from unboundednerfpytorch_b200 import ops
-        S = m._n_samples(0.5)
-        pts, outb = ops.sample_ndc_pts_on_rays(ro, rd, m.xyz_min, m.xyz_max, S)
-        queried = int(m.mask_cache(pts[~outb]).sum())
-    M = int(out['ray_id'].numel())
-    bytes_a = queried * (32 + 8 + 1)
-    bytes_b = M * 8 * 36
-    t_a = k.get('march_ndc_density_fwd', float('nan'))
-    t_b = k.get('march_ndc_feature_fwd', float('nan'))
-    t_bb = k.get('march_ndc_feature_bwd', float('nan'))
-    res['march_hbm'] = dict(queried=queried, survivors=M, bytes_pass_a=bytes_a, bytes_pass_b=bytes_b,
-                            density_fwd_frac_of_peak=bytes_a / (t_a * 1e-3) / HBM_PEAK,
-                            feature_fwd_frac_of_peak=bytes_b / (t_b * 1e-3) / HBM_PEAK,
-                            feature_bwd_frac_of_peak=2 * bytes_b / (t_bb * 1e-3) / HBM_PEAK)
-
-    # one 1008x756 frame in 8192-ray chunks
-    from unboundednerfpytorch_b200 import render
-    fro, frd, fvd = rays(1008 * 756)
-    res['render_frame_ms'] = _time(lambda i: render.render_rays(m, fro, frd, fvd, dict(RK), chunk=8192), max(2, args.steps // 5), 1)
-    res['render_rays'] = 1008 * 756
-    print(json.dumps(res))
+        if f'rgbnet_{kind}' in k:
+            rg[f'rgbnet_{kind}_ms'] = k[f'rgbnet_{kind}']
+        else:
+            rg[f'rgbnet_{kind}_ms'] = sum(s.elapsed_time(e) for s, e in marks[kind][-args.steps:]) / args.steps
+    rg['rgbnet_path'] = 'kernel' if 'rgbnet_fwd' in k else 'torch'
+    return k, step_ms, rg
 
 
 if __name__ == '__main__':

@@ -1,5 +1,12 @@
-"""The rgbnet alone (shade.shade forward + backward, csrc/shade_tc.cu) at the truck training shape: M = 4,194,304 samples, 8192
-rays with sorted ray_id (512 consecutive samples per ray), seeded inputs.  Prints one JSON line:
+"""The rgbnet alone (shade.shade forward + backward, csrc/shade_tc.cu) at one of two shapes, seeded inputs:
+
+* ``--shape truck`` (default): 12 -> 128 -> 128 -> 3 (27 view-embedding columns), M = 4,194,304 samples, 8192 rays with sorted
+  ray_id (512 consecutive samples per ray);
+* ``--shape llff``: DirectMPIGO of llff_default, 9 -> 64 -> 64 -> 3 (3 view-direction columns), M = the survivor count
+  scripts/bench_mpi.py reports for its 4096 rays (override with --samples), in rays of 255 consecutive samples (mpi_depth 128 at
+  stepsize 0.5).
+
+Prints one JSON line:
 
 * ms             -- CUDA events around the forward launch (``rgbnet_fwd``) and around the two backward launches
                     (``rgbnet_bwd``), mean over --iters steps after --warmup;
@@ -13,7 +20,7 @@ rays with sorted ray_id (512 consecutive samples per ray), seeded inputs.  Print
                     dropped for this check, as in tests/test_gpu_models.py);
 * gpu / power_limit_w -- where it ran, read in the same run.
 
-    python scripts/bench_rgbnet.py [--iters 20] [--warmup 3] [--profile DIR] [--no-check]
+    python scripts/bench_rgbnet.py [--shape truck|llff] [--iters 20] [--warmup 3] [--profile DIR] [--no-check]
 """
 import argparse
 import json
@@ -29,14 +36,25 @@ sys.path.insert(0, ROOT)
 TF32_PEAK = 495e12          # H100 SXM data sheet, dense
 HBM_PEAK = 3.35e12
 MMA_FLOP = 16 * 8 * 8 * 2
+LLFF_SURVIVORS = 412_419     # outputs.survivors of scripts/bench_mpi.py at its 4096 rays (seeded scene, before training)
 # issued mma.m16n8k8 per sample in the default 3xTF32 build (read off the SASS of the kernels)
 HMMA_PER_SAMPLE = {'k_shade_fwd_tc': 864 / 16,      # layer 1 (2 k-steps) + layer 2 (16 k-steps), 16 column tiles, 3 passes
                    'k_shade_bwd_tc': 1120 / 16,     # dH1 768 + dX 96 + dW1k/view bias 96 + dW3 96 + E 64, per 16-sample unit
-                   'k_shade_dw2_tc': 1536 / 32}     # 8 warps x 4 k-steps x 16 column tiles x 3 passes per 32-sample chunk
+                   'k_shade_dw2_tc': 1536 / 32,     # 8 warps x 4 k-steps x 16 column tiles x 3 passes per 32-sample chunk
+                   # width 64, 9 features
+                   'k_shade_fwd_tc_w': 240 / 16,    # layer 1 (2 k-steps) + layer 2 (8 k-steps), 8 column tiles, 3 passes
+                   'k_shade_bwd_tc_w': 368 / 16,    # dH1 192 + dX 48 + dW1k/view bias 48 + dW3 48 + E 32, per 16-sample unit
+                   'k_shade_dw2_tc_w': 384 / 32}    # 8 warps x 4 k-steps x 4 column tiles x 3 passes per 32-sample chunk
 # bytes each kernel must move per sample (fp32 unless noted)
 BYTES_PER_SAMPLE = {'k_shade_fwd_tc': 48 + 8 + 12 + 512 + 512 + 16,          # feat, ray_id, rgb, H1 + H2 saves, H1 masks
                     'k_shade_bwd_tc': 512 + 48 + 12 + 12 + 8 + 16 + 48 + 16,  # H2, feat, rgb, grad_rgb, ray_id, H1 masks; grad_feat, H2 masks
-                    'k_shade_dw2_tc': 512 + 16 + 12 + 12}                     # H1, H2 masks, rgb, grad_rgb
+                    'k_shade_dw2_tc': 512 + 16 + 12 + 12,                     # H1, H2 masks, rgb, grad_rgb
+                    'k_shade_fwd_tc_w': 36 + 8 + 12 + 256 + 256 + 8,          # the same at width 64 with 9 features
+                    'k_shade_bwd_tc_w': 256 + 36 + 12 + 12 + 8 + 8 + 36 + 8,
+                    'k_shade_dw2_tc_w': 256 + 8 + 12 + 12}
+# shape -> feature columns, hidden width, view-embedding columns, kernel-name suffix, default samples and rays
+SHAPES = {'truck': dict(K=12, W=128, E=27, sfx='', samples=4_194_304, rays=8192),
+          'llff': dict(K=9, W=64, E=3, sfx='_w', samples=LLFF_SURVIVORS, rays=None)}
 
 
 def _gpu_info():
@@ -50,14 +68,19 @@ def _gpu_info():
     return name, power
 
 
-def _inputs(M, n_rays, seed=0):
+def _inputs(M, n_rays, K, W, E, seed=0):
+    """n_rays = None: rays of 255 consecutive samples (the last one shorter)"""
     from unboundednerfpytorch_b200 import models
     torch.manual_seed(seed)
-    net = models._make_rgbnet(39, 128, 3).cuda()
+    net = models._make_rgbnet(K + E, W, 3).cuda()
     g = torch.Generator().manual_seed(seed)
-    k0 = torch.randn(M, 12, generator=g).cuda()
-    emb = torch.randn(n_rays, 27, generator=g).cuda()
-    ray_id = torch.arange(n_rays).repeat_interleave(M // n_rays).cuda()
+    k0 = torch.randn(M, K, generator=g).cuda()
+    if n_rays is None:
+        ray_id = (torch.arange(M) // 255).cuda()
+        n_rays = -(-M // 255)
+    else:
+        ray_id = torch.arange(n_rays).repeat_interleave(M // n_rays).cuda()
+    emb = torch.randn(n_rays, E, generator=g).cuda()
     gr = torch.randn(M, 3, generator=g).cuda()
     return net, k0, emb, ray_id, gr
 
@@ -88,7 +111,7 @@ def _check(shade, net, k0, emb, ray_id, gr, chunk=200_000):
             z2 = torch.relu(z1) @ W2.t() + b2
             ok[sl] = torch.minimum(z1.abs().amin(1), z2.abs().amin(1)) > 1e-5
     k0, ray_id, gr = k0[ok].clone().requires_grad_(True), ray_id[ok].contiguous(), gr[ok].contiguous()
-    net64 = models._make_rgbnet(39, 128, 3).cuda().double()
+    net64 = models._make_rgbnet(net[0].weight.shape[1], net[0].weight.shape[0], 3).cuda().double()
     net64.load_state_dict({k: v.double() for k, v in net.state_dict().items()})
     k64 = k0.detach().double().requires_grad_(True)
     for lo in range(0, k0.shape[0], chunk):
@@ -106,8 +129,9 @@ def _check(shade, net, k0, emb, ray_id, gr, chunk=200_000):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument('--samples', type=int, default=4_194_304)
-    ap.add_argument('--rays', type=int, default=8192)
+    ap.add_argument('--shape', choices=sorted(SHAPES), default='truck')
+    ap.add_argument('--samples', type=int, default=None)
+    ap.add_argument('--rays', type=int, default=None)
     ap.add_argument('--iters', type=int, default=20)
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--profile', default=None, help='also run a torch.profiler pass and write its trace under this directory')
@@ -117,11 +141,15 @@ def main():
         sys.exit('bench_rgbnet.py needs a GPU')
     from unboundednerfpytorch_b200 import _cabi, shade
     name, power = _gpu_info()
-    M = args.samples
-    net, k0, emb, ray_id, gr = _inputs(M, args.rays)
+    sh = SHAPES[args.shape]
+    M = args.samples or sh['samples']
+    assert M > 0, '--samples is required at this shape'
+    net, k0, emb, ray_id, gr = _inputs(M, args.rays or sh['rays'], sh['K'], sh['W'], sh['E'])
+    assert shade.supported(net, sh['K'])
     k0.requires_grad_(True)
-    res = dict(metric='rgbnet forward + backward, truck shape', gpu=name, power_limit_w=power, samples=M, rays=args.rays,
-               mode=shade.MODE, bwd_mode=shade.BWD_MODE)
+    fwd_k, bwd_k, dw2_k = (f'k_shade_{n}_tc{sh["sfx"]}' for n in ('fwd', 'bwd', 'dw2'))
+    res = dict(metric=f'rgbnet forward + backward, {args.shape} shape', gpu=name, power_limit_w=power, samples=M,
+               rays=emb.shape[0], features=sh['K'], width=sh['W'], mode=shade.MODE, bwd_mode=shade.BWD_MODE)
     for _ in range(args.warmup):
         _step(shade, net, k0, emb, ray_id, gr)
     torch.cuda.synchronize()
@@ -131,9 +159,9 @@ def main():
     summ = _cabi.TIMER.summary()
     _cabi.TIMER = None
     res['ms'] = {k: round(v[0], 3) for k, v in summ.items()}
-    res['rates'] = {'k_shade_fwd_tc': _rates('k_shade_fwd_tc', summ['rgbnet_fwd'][0], M)}
+    res['rates'] = {fwd_k: _rates(fwd_k, summ['rgbnet_fwd'][0], M)}
     bwd = summ['rgbnet_bwd'][0]
-    pair_flop = (HMMA_PER_SAMPLE['k_shade_bwd_tc'] + HMMA_PER_SAMPLE['k_shade_dw2_tc']) * MMA_FLOP * M
+    pair_flop = (HMMA_PER_SAMPLE[bwd_k] + HMMA_PER_SAMPLE[dw2_k]) * MMA_FLOP * M
     res['rates']['backward_pair'] = dict(ms=round(bwd, 3), tflops_hmma_equiv=round(pair_flop / bwd / 1e9, 1),
                                          share_of_tf32_datasheet=round(pair_flop / bwd / 1e9 / (TF32_PEAK / 1e12), 3))
     if args.profile:
@@ -146,8 +174,8 @@ def main():
         prof.export_chrome_trace(os.path.join(args.profile, 'bench_rgbnet.pt.trace.json'))
         kms = {}
         for ev in prof.key_averages():
-            for kname in HMMA_PER_SAMPLE:
-                if kname in ev.key:
+            for kname in (fwd_k, bwd_k, dw2_k):
+                if kname + '<' in ev.key:
                     t = getattr(ev, 'device_time_total', None) or getattr(ev, 'cuda_time_total', 0.0)
                     kms[kname] = kms.get(kname, 0.0) + t / 1e3 / args.iters
         res['kernels_ms'] = {k: round(v, 3) for k, v in kms.items()}

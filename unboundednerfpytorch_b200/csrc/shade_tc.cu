@@ -25,17 +25,19 @@
 namespace ubn {
 namespace tc {
 
-constexpr int kHidden = 128;
-constexpr int kFeat = 12;               // feature columns of every shipped 12-channel config; kernels take kF in {3, 12, 15}
-constexpr int kNT = kHidden / 8;        // 8-column tiles of a 128-wide layer
+// Hidden width kW is a template parameter of every kernel: 128 (every 12-channel config, the FourierGrid K = 3 / 15 configs)
+// or 64 (DirectMPIGO's llff_default, K = 9).  Everything below that sizes a layer derives from it.
+constexpr int kHidden = 128;            // the width of the kernels that keep their own names (k_shade_fwd_tc, k_shade_bwd_tc, ...)
+constexpr int kFeat = 12;               // feature columns of every shipped 12-channel config; kernels take kF in {3, 9, 12, 15}
 constexpr int kUnit = 16;               // samples per warp unit (the M of one mma)
 constexpr int kPanelRows = 128;         // row block of the panel save layout
-constexpr int kStride = kHidden + 8;    // floats per row of a shared-memory operand tile (conflict-free both ways)
+__host__ __device__ constexpr int n_tiles(int w) { return w / 8; }      // 8-column tiles of a w-wide layer
+__host__ __device__ constexpr int stride(int w) { return w + 8; }       // floats per row of a shared-memory operand tile
+                                                                        // (conflict-free both ways)
 
 // B-fragment tables (uint4 per lane): [n-tile][k-step][32 lanes]
-constexpr uint32_t kFragW2 = kNT * kNT * 32 * 16;          // 128 KB
-constexpr uint32_t kFragW1 = kNT * 2 * 32 * 16;            // layer 1: K <= 16 (at most 2 k-steps), N = 128
-constexpr uint32_t kFragW1T = 2 * kNT * 32 * 16;           // dX: K = 128, N <= 16 (at most 2 n-tiles)
+__host__ __device__ constexpr uint32_t frag_w2(int w) { return n_tiles(w) * n_tiles(w) * 32 * 16; }  // 128 KB at w = 128
+__host__ __device__ constexpr uint32_t frag_w1(int w) { return n_tiles(w) * 2 * 32 * 16; }  // layer 1: K <= 16 (2 k-steps)
 
 __device__ __forceinline__ uint32_t tf32_hi_bits(float x) { return __float_as_uint(x) & 0xFFFFE000u; }
 
@@ -96,17 +98,21 @@ __device__ __forceinline__ void warp_gemm(float (&acc)[NT][4], const float (&x)[
   }
 }
 
-// element offset of (row, col) in a save buffer: row-major [n][128], or the panel layout [n/128][32 quads][128 rows][4]
-template <bool kPanel>
+// element offset of (row, col) in a save buffer: row-major [n][kW], or the panel layout [n/128][kW/4 quads][128 rows][4]
+template <bool kPanel, int kW>
 __device__ __forceinline__ int64_t save_idx(int64_t row, int col) {
-  if (kPanel) return (row >> 7) * (kPanelRows * kHidden) + (int64_t)(col >> 2) * (kPanelRows * 4) + (row & 127) * 4 + (col & 3);
-  return row * kHidden + col;
+  if (kPanel) return (row >> 7) * (kPanelRows * kW) + (int64_t)(col >> 2) * (kPanelRows * 4) + (row & 127) * 4 + (col & 3);
+  return row * kW + col;
 }
 
-// ReLU mask words: [n/128][4 chunks of 32 units][128 rows], bit e = unit 32 c + e
-__device__ __forceinline__ int64_t mask_idx(int64_t row, int chunk) { return (row >> 7) * 512 + chunk * 128 + (row & 127); }
+// ReLU mask words: [n/128][kW/32 chunks of 32 units][128 rows], bit e = unit 32 c + e
+template <int kW>
+__device__ __forceinline__ int64_t mask_idx(int64_t row, int chunk) {
+  return (row >> 7) * (kW / 32 * kPanelRows) + chunk * kPanelRows + (row & 127);
+}
 
 // OR of this thread's bits of chunk c (units 8 j + 2 t, + 1 for j = 4 c .. 4 c + 3) over the four t lanes of a row
+template <int kNT>
 __device__ __forceinline__ uint32_t mask_chunk(const float (&h)[kNT][4], int c, int e0, int t) {
   uint32_t w = 0;
 #pragma unroll
@@ -121,30 +127,36 @@ __device__ __forceinline__ uint32_t mask_chunk(const float (&h)[kNT][4], int c, 
 }
 
 // ---- forward ---------------------------------------------------------------------------------------------------------
-constexpr uint32_t oFW2 = 0;
-constexpr uint32_t oFW1 = oFW2 + kFragW2;
-constexpr uint32_t oFW3 = oFW1 + kFragW1;                 // [3][128]
-constexpr uint32_t oFB2 = oFW3 + 3 * kHidden * 4;
-constexpr uint32_t kSmemFwd = oFB2 + kHidden * 4;
+// shared memory: W2 fragments, W1k fragments, W3 [3][kW], b2 [kW]
+namespace fw {
+__host__ __device__ constexpr uint32_t oW1(int w) { return frag_w2(w); }
+__host__ __device__ constexpr uint32_t oW3(int w) { return oW1(w) + frag_w1(w); }
+__host__ __device__ constexpr uint32_t oB2(int w) { return oW3(w) + 3 * w * 4; }
+__host__ __device__ constexpr uint32_t smem(int w) { return oB2(w) + w * 4; }
+}  // namespace fw
 
-// kF feature columns: ceil(kF / 8) k-steps of layer 1 (1 for kF = 3, 2 for 12 and 15); odd kF rows are 4-byte aligned
-template <int kF, bool kSave, bool kThree, int kWarps, bool kPanel>
-__global__ void __launch_bounds__(32 * kWarps, 1) k_shade_fwd_tc(
-    const float* __restrict__ feat, const float* __restrict__ vb, const int64_t* __restrict__ ray_id,
-    const float* __restrict__ W1k, const float* __restrict__ W2, const float* __restrict__ b2,
-    const float* __restrict__ W3, const float* __restrict__ b3, int64_t n_pts, float* __restrict__ rgb,
-    float* __restrict__ h1_out, float* __restrict__ h2_out, uint32_t* __restrict__ h1_mask) {
+#define UBN_SHADE_FWD_PARAMS                                                                                                 \
+  const float* __restrict__ feat, const float* __restrict__ vb, const int64_t* __restrict__ ray_id,                          \
+      const float* __restrict__ W1k, const float* __restrict__ W2, const float* __restrict__ b2, const float* __restrict__ W3, \
+      const float* __restrict__ b3, int64_t n_pts, float* __restrict__ rgb, float* __restrict__ h1_out,                      \
+      float* __restrict__ h2_out, uint32_t* __restrict__ h1_mask
+#define UBN_SHADE_FWD_ARGS feat, vb, ray_id, W1k, W2, b2, W3, b3, n_pts, rgb, h1_out, h2_out, h1_mask
+
+// kF feature columns: ceil(kF / 8) k-steps of layer 1 (1 for kF = 3, 2 for 9, 12 and 15); odd kF rows are 4-byte aligned
+template <int kF, int kW, bool kSave, bool kThree, int kWarps, bool kPanel>
+__device__ __forceinline__ void shade_fwd_tc(UBN_SHADE_FWD_PARAMS) {
+  constexpr int kNT = n_tiles(kW);
   extern __shared__ __align__(16) uint8_t smem[];
   const int tid = threadIdx.x, lane = tid & 31, g = lane >> 2, t = lane & 3;
-  const uint4* fW2 = reinterpret_cast<const uint4*>(smem + oFW2);
-  const uint4* fW1 = reinterpret_cast<const uint4*>(smem + oFW1);
-  float* sW3 = reinterpret_cast<float*>(smem + oFW3);
-  float* sB2 = reinterpret_cast<float*>(smem + oFB2);
-  stage_frags(W2, kHidden, true, kHidden, kHidden, kNT, kNT, reinterpret_cast<uint4*>(smem + oFW2), tid, 32 * kWarps);
+  const uint4* fW2 = reinterpret_cast<const uint4*>(smem);
+  const uint4* fW1 = reinterpret_cast<const uint4*>(smem + fw::oW1(kW));
+  float* sW3 = reinterpret_cast<float*>(smem + fw::oW3(kW));
+  float* sB2 = reinterpret_cast<float*>(smem + fw::oB2(kW));
+  stage_frags(W2, kW, true, kW, kW, kNT, kNT, reinterpret_cast<uint4*>(smem), tid, 32 * kWarps);
   constexpr int kKS = (kF + 7) / 8;
-  stage_frags(W1k, kF, true, kF, kHidden, kKS, kNT, reinterpret_cast<uint4*>(smem + oFW1), tid, 32 * kWarps);
-  for (int i = tid; i < 3 * kHidden; i += 32 * kWarps) sW3[i] = W3[i];
-  for (int i = tid; i < kHidden; i += 32 * kWarps) sB2[i] = b2[i];
+  stage_frags(W1k, kF, true, kF, kW, kKS, kNT, reinterpret_cast<uint4*>(smem + fw::oW1(kW)), tid, 32 * kWarps);
+  for (int i = tid; i < 3 * kW; i += 32 * kWarps) sW3[i] = W3[i];
+  for (int i = tid; i < kW; i += 32 * kWarps) sB2[i] = b2[i];
   __syncthreads();
   const float b3v[3] = {b3[0], b3[1], b3[2]};
 
@@ -179,19 +191,19 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_fwd_tc(
     for (int j = 0; j < kNT; ++j)
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
-        const float2 bias = __ldg(reinterpret_cast<const float2*>(vb + ray[r] * kHidden + 8 * j + 2 * t));
+        const float2 bias = __ldg(reinterpret_cast<const float2*>(vb + ray[r] * kW + 8 * j + 2 * t));
         h[j][2 * r] = fmaxf(h[j][2 * r] + bias.x, 0.f);
         h[j][2 * r + 1] = fmaxf(h[j][2 * r + 1] + bias.y, 0.f);
         if (kSave && live[r])
-          *reinterpret_cast<float2*>(h1_out + save_idx<kPanel>(row[r], 8 * j + 2 * t)) = make_float2(h[j][2 * r], h[j][2 * r + 1]);
+          *reinterpret_cast<float2*>(h1_out + save_idx<kPanel, kW>(row[r], 8 * j + 2 * t)) = make_float2(h[j][2 * r], h[j][2 * r + 1]);
       }
     if (kSave && kPanel && h1_mask) {
 #pragma unroll
-      for (int c = 0; c < 4; ++c)
+      for (int c = 0; c < kW / 32; ++c)
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
           const uint32_t w = mask_chunk(h, c, 2 * r, t);
-          if (t == 0 && live[r]) h1_mask[mask_idx(row[r], c)] = w;
+          if (t == 0 && live[r]) h1_mask[mask_idx<kW>(row[r], c)] = w;
         }
     }
     // layer 2
@@ -208,9 +220,9 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_fwd_tc(
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         const float a0 = fmaxf(z[j][2 * r] + bb.x, 0.f), a1 = fmaxf(z[j][2 * r + 1] + bb.y, 0.f);
-        if (kSave && live[r]) *reinterpret_cast<float2*>(h2_out + save_idx<kPanel>(row[r], c)) = make_float2(a0, a1);
+        if (kSave && live[r]) *reinterpret_cast<float2*>(h2_out + save_idx<kPanel, kW>(row[r], c)) = make_float2(a0, a1);
 #pragma unroll
-        for (int i = 0; i < 3; ++i) p[r][i] = fmaf(a1, sW3[i * kHidden + c + 1], fmaf(a0, sW3[i * kHidden + c], p[r][i]));
+        for (int i = 0; i < 3; ++i) p[r][i] = fmaf(a1, sW3[i * kW + c + 1], fmaf(a0, sW3[i * kW + c], p[r][i]));
       }
     }
 #pragma unroll
@@ -232,6 +244,19 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_fwd_tc(
   }
 }
 
+template <int kF, bool kSave, bool kThree, int kWarps, bool kPanel>
+__global__ void __launch_bounds__(32 * kWarps, 1) k_shade_fwd_tc(UBN_SHADE_FWD_PARAMS) {
+  shade_fwd_tc<kF, kHidden, kSave, kThree, kWarps, kPanel>(UBN_SHADE_FWD_ARGS);
+}
+
+// other widths: kCtas resident CTAs per SM
+template <int kF, int kW, bool kSave, bool kThree, int kWarps, int kCtas, bool kPanel>
+__global__ void __launch_bounds__(32 * kWarps, kCtas) k_shade_fwd_tc_w(UBN_SHADE_FWD_PARAMS) {
+  shade_fwd_tc<kF, kW, kSave, kThree, kWarps, kPanel>(UBN_SHADE_FWD_ARGS);
+}
+#undef UBN_SHADE_FWD_ARGS
+#undef UBN_SHADE_FWD_PARAMS
+
 // ---- backward, launch 1 --------------------------------------------------------------------------------------------------
 //   dz3 = g_rgb * rgb (1 - rgb);  dZ2 = (dz3 . W3) * [H2 > 0];  dH1 = dZ2 . W2;  dZ1 = dH1 * [H1 > 0]
 //   kDz1Out: write dZ1 [n,128] row-major and stop (ubn_rgbnet_bwd_small finishes on the CUDA cores); otherwise also
@@ -244,18 +269,17 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_fwd_tc(
 // contiguous and ray_id is sorted, the dZ1 sum of the ray that is still open at the end of a unit is carried (one more row of
 // the warp's slice) into the next unit and written to grad_view_bias once, when its ray ends.
 namespace bk {
-constexpr uint32_t kFragW2f = kNT * kNT * 32 * 8;          // 64 KB: fp32 B fragments, split into hi / lo at the MMA
-constexpr uint32_t kFragW1Tf = 2 * kNT * 32 * 8;
-constexpr uint32_t oW2 = 0;                                // dH1 = dZ2 . W2: B[k][n] = W2[k][n]
-constexpr uint32_t oW1T = oW2 + kFragW2f;                  // dX = dZ1 . W1k: B[k][n] = W1k[k][n]
-constexpr uint32_t oW3 = oW1T + kFragW1Tf;
-constexpr uint32_t oWarp = oW3 + 3 * kHidden * 4;
-// per warp: operand tile [16][kStride], the running sums dW1k^T [12][kStride], dW3 [3][kStride], E [3][kStride], and the
-// open ray's dZ1 sum [kStride]
-constexpr uint32_t kTileBytes = kUnit * kStride * 4;
+// W2 fragments at offset 0 (dH1 = dZ2 . W2: B[k][n] = W2[k][n]), fp32 and split into hi / lo at the MMA: 64 KB at w = 128
+__host__ __device__ constexpr uint32_t frag_w2f(int w) { return n_tiles(w) * n_tiles(w) * 32 * 8; }
+__host__ __device__ constexpr uint32_t oW1T(int w) { return frag_w2f(w); }              // dX = dZ1 . W1k: B[k][n] = W1k[k][n]
+__host__ __device__ constexpr uint32_t oW3(int w) { return oW1T(w) + 2 * n_tiles(w) * 32 * 8; }
+__host__ __device__ constexpr uint32_t oWarp(int w) { return oW3(w) + 3 * w * 4; }
+// per warp: operand tile [16][stride], the running sums dW1k^T [kF][stride], dW3 [3][stride], E [3][stride], and the
+// open ray's dZ1 sum [stride]
+__host__ __device__ constexpr uint32_t tile_bytes(int w) { return kUnit * stride(w) * 4; }
 __host__ __device__ constexpr int sum_rows(int f) { return f + 3 + 3; }
-__host__ __device__ constexpr uint32_t warp_bytes(int f) { return kTileBytes + (sum_rows(f) + 1) * kStride * 4; }
-__host__ __device__ constexpr uint32_t smem_bytes(int warps, int f) { return oWarp + warps * warp_bytes(f); }
+__host__ __device__ constexpr uint32_t warp_bytes(int f, int w) { return tile_bytes(w) + (sum_rows(f) + 1) * stride(w) * 4; }
+__host__ __device__ constexpr uint32_t smem_bytes(int warps, int f, int w) { return oWarp(w) + warps * warp_bytes(f, w); }
 }  // namespace bk
 
 // lane (g, t) of (n-tile j, k-step s) gets the fp32 pair {B[8s+2t][8j+g], B[8s+2t+1][8j+g]}, B[k][n] = W[k * ld + n]
@@ -294,6 +318,7 @@ __device__ __forceinline__ void warp_gemm_f(float (&acc)[NT][4], const float (&x
 }
 
 // B fragment of the warp tile S[16][kStride] (sample = k): k-step s, column tile j -> S[8 s + t][8 j + g], S[8 s + t + 4][..]
+template <int kStride>
 __device__ __forceinline__ void tile_frag(const float* S, int s, int j, int g, int t, uint32_t (&hi)[2], uint32_t (&lo)[2]) {
   const float v[2] = {S[(8 * s + t) * kStride + 8 * j + g], S[(8 * s + t + 4) * kStride + 8 * j + g]};
 #pragma unroll
@@ -303,7 +328,8 @@ __device__ __forceinline__ void tile_frag(const float* S, int s, int j, int g, i
   }
 }
 
-// store a [16][128] accumulator-layout block into the warp tile
+// store a [16][8 kNT] accumulator-layout block into the warp tile
+template <int kStride, int kNT>
 __device__ __forceinline__ void tile_store(float* S, const float (&v)[kNT][4], int g, int t) {
 #pragma unroll
   for (int j = 0; j < kNT; ++j) {
@@ -323,18 +349,19 @@ __device__ __forceinline__ void red_add2(float* p, float a, float b) {
   asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
 }
 
-// grad_view_bias[ray] += V for the columns 8 j + 2 t, + 1 (j < 16) of a g-row of lanes
+// grad_view_bias[ray] += V for the columns 8 j + 2 t, + 1 (j < kW / 8) of a g-row of lanes
+template <int kW>
 __device__ __forceinline__ void emit_ray(float* grad_view_bias, int64_t ray, const float* V, int t) {
 #pragma unroll
-  for (int j = 0; j < kNT; ++j) {
+  for (int j = 0; j < n_tiles(kW); ++j) {
     const float2 v = *reinterpret_cast<const float2*>(V + 8 * j + 2 * t);
-    red_add2(grad_view_bias + ray * kHidden + 8 * j + 2 * t, v.x, v.y);
+    red_add2(grad_view_bias + ray * kW + 8 * j + 2 * t, v.x, v.y);
   }
 }
 
 // kF feature columns: dX has ceil(kF / 8) n-tiles.  The dW1k^T sums and the ray-segment indicators share one 16-row A tile
 // while kF <= 12 (features in rows 0 .. kF - 1, indicators in rows 12 .. 15); at kF = 15 the indicators get an m-tile of their own.
-template <int kF, bool kThree, int kWarps, bool kPanel, bool kMask1, bool kDz1Out>
+template <int kF, int kW, bool kThree, int kWarps, bool kPanel, bool kMask1, bool kDz1Out>
 __device__ __forceinline__ void shade_bwd_tc(
     const float* __restrict__ feat, const int64_t* __restrict__ ray_id, const float* __restrict__ W1k,
     const float* __restrict__ W2, const float* __restrict__ W3, const float* __restrict__ rgb,
@@ -346,19 +373,20 @@ __device__ __forceinline__ void shade_bwd_tc(
   constexpr int kThreads = 32 * kWarps;
   constexpr int kNTX = (kF + 7) / 8;                      // n-tiles of dX
   constexpr bool kSegTile = kF > 12;                      // indicators in a second m-tile
-  constexpr uint32_t kWarpBytes = bk::warp_bytes(kF);
+  constexpr int kNT = n_tiles(kW), kStride = stride(kW), kChunks = kW / 32;
+  constexpr uint32_t kWarpBytes = bk::warp_bytes(kF, kW);
   const int tid = threadIdx.x, lane = tid & 31, g = lane >> 2, t = lane & 3, warp = tid >> 5;
-  const uint2* fW2 = reinterpret_cast<const uint2*>(smem + bk::oW2);
-  const uint2* fW1T = reinterpret_cast<const uint2*>(smem + bk::oW1T);
-  float* sW3 = reinterpret_cast<float*>(smem + bk::oW3);
-  float* S = reinterpret_cast<float*>(smem + bk::oWarp + warp * kWarpBytes);
+  const uint2* fW2 = reinterpret_cast<const uint2*>(smem);
+  const uint2* fW1T = reinterpret_cast<const uint2*>(smem + bk::oW1T(kW));
+  float* sW3 = reinterpret_cast<float*>(smem + bk::oW3(kW));
+  float* S = reinterpret_cast<float*>(smem + bk::oWarp(kW) + warp * kWarpBytes);
   float* sumW1 = S + kUnit * kStride;                     // dW1k^T [feature][unit]
   float* sumW3 = sumW1 + kF * kStride;
   float* sumE = sumW3 + 3 * kStride;
   float* vbc = sumE + 3 * kStride;                        // lanes g == 4: the open ray's sum of dZ1 so far
-  stage_frags_f32(W2, kHidden, kHidden, kHidden, kNT, kNT, reinterpret_cast<uint2*>(smem + bk::oW2), tid, kThreads);
-  if (!kDz1Out) stage_frags_f32(W1k, kF, kHidden, kF, kNT, kNTX, reinterpret_cast<uint2*>(smem + bk::oW1T), tid, kThreads);
-  for (int i = tid; i < 3 * kHidden; i += kThreads) sW3[i] = W3[i];
+  stage_frags_f32(W2, kW, kW, kW, kNT, kNT, reinterpret_cast<uint2*>(smem), tid, kThreads);
+  if (!kDz1Out) stage_frags_f32(W1k, kF, kW, kF, kNT, kNTX, reinterpret_cast<uint2*>(smem + bk::oW1T(kW)), tid, kThreads);
+  for (int i = tid; i < 3 * kW; i += kThreads) sW3[i] = W3[i];
   if (!kDz1Out)
     for (int i = lane; i < bk::sum_rows(kF) * kStride; i += 32) sumW1[i] = 0.f;
   __syncthreads();
@@ -383,17 +411,17 @@ __device__ __forceinline__ void shade_bwd_tc(
       }
     // dZ2 in accumulator layout; H2 values kept for dW3 below (through the warp tile)
     float d2[kNT][4];
-    uint32_t m2[2][4] = {{0u, 0u, 0u, 0u}, {0u, 0u, 0u, 0u}};
+    uint32_t m2[2][kChunks] = {};
 #pragma unroll
     for (int j = 0; j < kNT; ++j) {
       const int c = 8 * j + 2 * t;
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
-        const float2 hv = live[r] ? *reinterpret_cast<const float2*>(h2_save + save_idx<kPanel>(row[r], c)) : make_float2(0.f, 0.f);
+        const float2 hv = live[r] ? *reinterpret_cast<const float2*>(h2_save + save_idx<kPanel, kW>(row[r], c)) : make_float2(0.f, 0.f);
         const float hv2[2] = {hv.x, hv.y};
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
-          const float dh = dz3[r][0] * sW3[c + e] + dz3[r][1] * sW3[kHidden + c + e] + dz3[r][2] * sW3[2 * kHidden + c + e];
+          const float dh = dz3[r][0] * sW3[c + e] + dz3[r][1] * sW3[kW + c + e] + dz3[r][2] * sW3[2 * kW + c + e];
           d2[j][2 * r + e] = hv2[e] > 0.f ? dh : 0.f;
           if (hv2[e] > 0.f) m2[r][j >> 2] |= 1u << (8 * (j & 3) + 2 * t + e);
         }
@@ -404,11 +432,11 @@ __device__ __forceinline__ void shade_bwd_tc(
 #pragma unroll
       for (int r = 0; r < 2; ++r)
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
+        for (int c = 0; c < kChunks; ++c) {
           uint32_t w = m2[r][c];
           w |= __shfl_xor_sync(0xffffffffu, w, 1);
           w |= __shfl_xor_sync(0xffffffffu, w, 2);
-          if (t == 0 && live[r]) h2_mask[mask_idx(row[r], c)] = w;
+          if (t == 0 && live[r]) h2_mask[mask_idx<kW>(row[r], c)] = w;
         }
     }
     if (!kDz1Out) {
@@ -435,8 +463,8 @@ __device__ __forceinline__ void shade_bwd_tc(
 #pragma unroll
         for (int s = 0; s < 2; ++s) split4(av[s], ah[s], al[s]);
 #pragma unroll
-        for (int jh = 0; jh < 2; ++jh) {                     // two halves of the column tiles: 64 accumulators live, not 128
-          constexpr int kH = kNT / 2;
+        for (int jh = 0; jh < kNT / 8; ++jh) {               // groups of 8 column tiles: at most 64 accumulators live
+          constexpr int kH = 8;
           float dW3a[kH][4], Ea[kH][4];
 #pragma unroll
           for (int jj = 0; jj < kH; ++jj) dW3a[jj][0] = dW3a[jj][1] = dW3a[jj][2] = dW3a[jj][3] = Ea[jj][0] = Ea[jj][1] = Ea[jj][2] = Ea[jj][3] = 0.f;
@@ -445,7 +473,7 @@ __device__ __forceinline__ void shade_bwd_tc(
 #pragma unroll
             for (int jj = 0; jj < kH; ++jj) {
               uint32_t bh[2], bl[2];
-              tile_frag(S, s, kH * jh + jj, g, t, bh, bl);
+              tile_frag<kStride>(S, s, kH * jh + jj, g, t, bh, bl);
               mma3<kThree>(dW3a[jj], ah[s], al[s], make_uint4(bh[0], bh[1], bl[0], bl[1]));
               const uint32_t one = 0x3f800000u;
               const uint32_t mb0 = __uint_as_float(bh[0]) + __uint_as_float(bl[0]) > 0.f ? one : 0u;
@@ -483,10 +511,10 @@ __device__ __forceinline__ void shade_bwd_tc(
     if (kMask1) {
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
-        uint32_t w[4] = {0u, 0u, 0u, 0u};
+        uint32_t w[kChunks] = {};
         if (live[r]) {
 #pragma unroll
-          for (int c = 0; c < 4; ++c) w[c] = h1_mask[mask_idx(row[r], c)];
+          for (int c = 0; c < kChunks; ++c) w[c] = h1_mask[mask_idx<kW>(row[r], c)];
         }
 #pragma unroll
         for (int j = 0; j < kNT; ++j)
@@ -499,7 +527,7 @@ __device__ __forceinline__ void shade_bwd_tc(
       for (int j = 0; j < kNT; ++j)
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
-          const float2 hv = live[r] ? *reinterpret_cast<const float2*>(h1_save + save_idx<kPanel>(row[r], 8 * j + 2 * t))
+          const float2 hv = live[r] ? *reinterpret_cast<const float2*>(h1_save + save_idx<kPanel, kW>(row[r], 8 * j + 2 * t))
                                     : make_float2(0.f, 0.f);
           if (!(hv.x > 0.f)) d1[j][2 * r] = 0.f;
           if (!(hv.y > 0.f)) d1[j][2 * r + 1] = 0.f;
@@ -510,7 +538,7 @@ __device__ __forceinline__ void shade_bwd_tc(
       for (int j = 0; j < kNT; ++j)
 #pragma unroll
         for (int r = 0; r < 2; ++r)
-          if (live[r]) *reinterpret_cast<float2*>(dz1_out + row[r] * kHidden + 8 * j + 2 * t) = make_float2(d1[j][2 * r], d1[j][2 * r + 1]);
+          if (live[r]) *reinterpret_cast<float2*>(dz1_out + row[r] * kW + 8 * j + 2 * t) = make_float2(d1[j][2 * r], d1[j][2 * r + 1]);
       continue;
     }
     // dX = dZ1 . W1k
@@ -532,7 +560,7 @@ __device__ __forceinline__ void shade_bwd_tc(
     }
     // dW1k^T = X^T . dZ1 (A rows 0 .. kF - 1) and per-ray sums of dZ1 (A rows 12..15 = indicators of up to 4 ray segments; at
     // kF > 12 those rows of a second m-tile)
-    tile_store(S, d1, g, t);
+    tile_store<kStride>(S, d1, g, t);
     __syncwarp();                                             // the tile is read back across lanes as B fragments below
     const int64_t my_ray = (lane < kUnit && r0 + lane < n_pts) ? ray_id[r0 + lane] : -1;
     const int64_t prev_ray = __shfl_up_sync(0xffffffffu, my_ray, 1);
@@ -568,7 +596,7 @@ __device__ __forceinline__ void shade_bwd_tc(
 #pragma unroll
           for (int j = 0; j < kNT; ++j) {
             uint32_t bh[2], bl[2];
-            tile_frag(S, s, j, g, t, bh, bl);
+            tile_frag<kStride>(S, s, j, g, t, bh, bl);
             mma3<kThree>(acc[j], ah, al, make_uint4(bh[0], bh[1], bl[0], bl[1]));
           }
         }
@@ -598,7 +626,7 @@ __device__ __forceinline__ void shade_bwd_tc(
 #pragma unroll
             for (int j = 0; j < kNT; ++j) {
               uint32_t bh[2], bl[2];
-              tile_frag(S, s, j, g, t, bh, bl);
+              tile_frag<kStride>(S, s, j, g, t, bh, bl);
               mma3<kThree>(acc[j], ah, al, make_uint4(bh[0], bh[1], bl[0], bl[1]));
             }
           }
@@ -625,19 +653,19 @@ __device__ __forceinline__ void shade_bwd_tc(
       if (segs_fit) {
         const bool cont = first_ray == open_ray;
         if (g == 4) {
-          if (!cont && open_ray >= 0) emit_ray(grad_view_bias, open_ray, vbc, t);    // the carried ray ended with the last unit
+          if (!cont && open_ray >= 0) emit_ray<kW>(grad_view_bias, open_ray, vbc, t);    // the carried ray ended with the last unit
 #pragma unroll
           for (int j = 0; j < kNT; ++j) {
             float* v = vbc + 8 * j + 2 * t;
             const float2 o = cont ? *reinterpret_cast<const float2*>(v) : make_float2(0.f, 0.f);
             *reinterpret_cast<float2*>(v) = make_float2(o.x + acc[j][2], o.y + acc[j][3]);
           }
-          if (nseg > 1) emit_ray(grad_view_bias, first_ray, vbc, t);                 // segment 0 ends inside this unit
+          if (nseg > 1) emit_ray<kW>(grad_view_bias, first_ray, vbc, t);                 // segment 0 ends inside this unit
         }
         if (nseg > 1) {
           if (g > 4 && g - 4 < nseg - 1) {                   // inner segments
 #pragma unroll
-            for (int j = 0; j < kNT; ++j) red_add2(grad_view_bias + seg_ray * kHidden + 8 * j + 2 * t, acc[j][2], acc[j][3]);
+            for (int j = 0; j < kNT; ++j) red_add2(grad_view_bias + seg_ray * kW + 8 * j + 2 * t, acc[j][2], acc[j][3]);
           }
           __syncwarp();                                       // lanes g == 4 have read vbc
           if (g == 3 + nseg) {                                // the last segment stays open
@@ -649,39 +677,39 @@ __device__ __forceinline__ void shade_bwd_tc(
       }
     }
     if (!segs_fit) {                                          // more than 4 rays in 16 samples: per-sample adds
-      if (open_ray >= 0 && g == 4) emit_ray(grad_view_bias, open_ray, vbc, t);
+      if (open_ray >= 0 && g == 4) emit_ray<kW>(grad_view_bias, open_ray, vbc, t);
       open_ray = -1;
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         if (!live[r]) continue;
         const int64_t ray = ray_id[row[r]];
 #pragma unroll
-        for (int j = 0; j < kNT; ++j) red_add2(grad_view_bias + ray * kHidden + 8 * j + 2 * t, d1[j][2 * r], d1[j][2 * r + 1]);
+        for (int j = 0; j < kNT; ++j) red_add2(grad_view_bias + ray * kW + 8 * j + 2 * t, d1[j][2 * r], d1[j][2 * r + 1]);
       }
     }
     __syncwarp();
   }
   if (kDz1Out) return;
-  if (open_ray >= 0 && g == 4) emit_ray(grad_view_bias, open_ray, vbc, t);
+  if (open_ray >= 0 && g == 4) emit_ray<kW>(grad_view_bias, open_ray, vbc, t);
   if (lane < 3) atomicAdd(grad_b3 + lane, db3);
   __syncthreads();
   // the warps' running sums, added in warp order, go to global once per CTA
-  const float* sums = reinterpret_cast<const float*>(smem + bk::oWarp + bk::kTileBytes);
+  const float* sums = reinterpret_cast<const float*>(smem + bk::oWarp(kW) + bk::tile_bytes(kW));
   auto warp_sum = [&](int r, int c) {
     float v = 0.f;
 #pragma unroll
     for (int w = 0; w < kWarps; ++w) v += sums[w * (kWarpBytes / 4) + r * kStride + c];
     return v;
   };
-  for (int i = tid; i < kF * kHidden; i += kThreads) {           // row f of the sums is column f of dW1k
-    const int f = i / kHidden, c = i % kHidden;
+  for (int i = tid; i < kF * kW; i += kThreads) {                // row f of the sums is column f of dW1k
+    const int f = i / kW, c = i % kW;
     atomicAdd(grad_W1k + c * kF + f, warp_sum(f, c));
   }
-  for (int i = tid; i < 3 * kHidden; i += kThreads) atomicAdd(grad_W3 + i, warp_sum(kF + i / kHidden, i % kHidden));
-  for (int c = tid; c < kHidden; c += kThreads) {
+  for (int i = tid; i < 3 * kW; i += kThreads) atomicAdd(grad_W3 + i, warp_sum(kF + i / kW, i % kW));
+  for (int c = tid; c < kW; c += kThreads) {
     float v = 0.f;
 #pragma unroll
-    for (int i = 0; i < 3; ++i) v += sW3[i * kHidden + c] * warp_sum(kF + 3 + i, c);
+    for (int i = 0; i < 3; ++i) v += sW3[i * kW + c] * warp_sum(kF + 3 + i, c);
     atomicAdd(grad_b2 + c, v);
   }
 }
@@ -699,12 +727,18 @@ __device__ __forceinline__ void shade_bwd_tc(
 // the 12-feature kernel keeps its own name; k_shade_bwd_tc_k carries the other feature counts
 template <bool kThree, int kWarps, bool kPanel, bool kMask1, bool kDz1Out>
 __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc(UBN_SHADE_BWD_PARAMS) {
-  shade_bwd_tc<kFeat, kThree, kWarps, kPanel, kMask1, kDz1Out>(UBN_SHADE_BWD_ARGS);
+  shade_bwd_tc<kFeat, kHidden, kThree, kWarps, kPanel, kMask1, kDz1Out>(UBN_SHADE_BWD_ARGS);
 }
 
 template <int kF, bool kThree, int kWarps, bool kPanel, bool kMask1, bool kDz1Out>
 __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc_k(UBN_SHADE_BWD_PARAMS) {
-  shade_bwd_tc<kF, kThree, kWarps, kPanel, kMask1, kDz1Out>(UBN_SHADE_BWD_ARGS);
+  shade_bwd_tc<kF, kHidden, kThree, kWarps, kPanel, kMask1, kDz1Out>(UBN_SHADE_BWD_ARGS);
+}
+
+// other widths: kCtas resident CTAs per SM
+template <int kF, int kW, bool kThree, int kWarps, int kCtas, bool kPanel, bool kMask1>
+__global__ void __launch_bounds__(32 * kWarps, kCtas) k_shade_bwd_tc_w(UBN_SHADE_BWD_PARAMS) {
+  shade_bwd_tc<kF, kW, kThree, kWarps, kPanel, kMask1, false>(UBN_SHADE_BWD_ARGS);
 }
 #undef UBN_SHADE_BWD_ARGS
 #undef UBN_SHADE_BWD_PARAMS
@@ -712,30 +746,31 @@ __global__ void __launch_bounds__(32 * kWarps, 1) k_shade_bwd_tc_k(UBN_SHADE_BWD
 // ---- backward, launch 2: dW2 += dZ2^T . H1 -------------------------------------------------------------------------------
 // A split-K GEMM over samples: each CTA takes 32-sample chunks, stages dZ2 (rebuilt from dz3, W3 and H2 or its ReLU masks) as a
 // [32][kStride] fp32 tile and H1 as a [32][kStrideB] tile of ready-split {hi, lo} pairs (split once per element, not once per
-// warp), and warp w accumulates output rows 16 w .. 16 w + 15.  The tiles are double-buffered and each thread loads the next
+// warp), and warp w accumulates output rows 16 w .. 16 w + 15 (at kW = 64, rows 16 (w % 4) .. + 15 and half of the columns).  The tiles are double-buffered and each thread loads the next
 // chunk's rows into registers before the MMAs of the current one, so the HBM reads overlap the tensor cores and one barrier
 // per chunk suffices.  The MMA accumulator restarts every chunk and is added into an fp32 running sum, so the tensor core
 // never carries a long accumulation chain.
 namespace dw {
 constexpr int kThreads = 256;
 constexpr int kK = 32;
-constexpr int kStrideB = kHidden + 4;                      // uint2 per element: conflict-free fragment reads
-constexpr uint32_t oW3 = 0;
-constexpr uint32_t kBufA = kK * kStride * 4;
-constexpr uint32_t kBuf = kBufA + kK * kStrideB * 8;
-constexpr uint32_t oBuf = oW3 + 3 * kHidden * 4;
-constexpr uint32_t kSmem = oBuf + 2 * kBuf;
+__host__ __device__ constexpr int stride_b(int w) { return w + 4; }    // uint2 per element: conflict-free fragment reads
+// W3 [3][kW] at offset 0, then two buffers of a dZ2 tile [kK][stride] and an H1 tile [kK][stride_b]
+__host__ __device__ constexpr uint32_t buf_a(int w) { return kK * stride(w) * 4; }
+__host__ __device__ constexpr uint32_t buf(int w) { return buf_a(w) + kK * stride_b(w) * 8; }
+__host__ __device__ constexpr uint32_t oBuf(int w) { return 3 * w * 4; }
+__host__ __device__ constexpr uint32_t smem(int w) { return oBuf(w) + 2 * buf(w); }
 }  // namespace dw
 
 // one thread's share of a chunk (sample row r, columns 32 q + 4 (tid & 7) .. + 3), straight from global memory
+template <int kW>
 struct Dw2Rows {
-  float4 h1[4], h2[4];
-  uint32_t m2[4];
+  float4 h1[kW / 32], h2[kW / 32];
+  uint32_t m2[kW / 32];
   float y[3], gy[3];
 };
 
-template <bool kPanel, bool kMask2>
-__device__ __forceinline__ void dw2_load(Dw2Rows& d, const float* __restrict__ rgb, const float* __restrict__ h1_save,
+template <int kW, bool kPanel, bool kMask2>
+__device__ __forceinline__ void dw2_load(Dw2Rows<kW>& d, const float* __restrict__ rgb, const float* __restrict__ h1_save,
                                          const float* __restrict__ h2_save, const uint32_t* __restrict__ h2_mask,
                                          const float* __restrict__ grad_rgb, int64_t r, int64_t n_pts, int c0) {
   const bool ok = r < n_pts;
@@ -746,40 +781,46 @@ __device__ __forceinline__ void dw2_load(Dw2Rows& d, const float* __restrict__ r
     d.gy[i] = ok ? grad_rgb[r * 3 + i] : 0.f;
   }
 #pragma unroll
-  for (int q = 0; q < 4; ++q) {
+  for (int q = 0; q < kW / 32; ++q) {
     const int c = 32 * q + c0;
-    d.h1[q] = ok ? *reinterpret_cast<const float4*>(h1_save + save_idx<kPanel>(r, c)) : zero;
-    if (kMask2) d.m2[q] = ok ? h2_mask[mask_idx(r, q)] : 0u;
-    else d.h2[q] = ok ? *reinterpret_cast<const float4*>(h2_save + save_idx<kPanel>(r, c)) : zero;
+    d.h1[q] = ok ? *reinterpret_cast<const float4*>(h1_save + save_idx<kPanel, kW>(r, c)) : zero;
+    if (kMask2) d.m2[q] = ok ? h2_mask[mask_idx<kW>(r, q)] : 0u;
+    else d.h2[q] = ok ? *reinterpret_cast<const float4*>(h2_save + save_idx<kPanel, kW>(r, c)) : zero;
   }
 }
 
-template <bool kThree, bool kPanel, bool kMask2>
-__global__ void __launch_bounds__(dw::kThreads, 1) k_shade_dw2_tc(
-    const float* __restrict__ W3, const float* __restrict__ rgb, const float* __restrict__ h1_save,
-    const float* __restrict__ h2_save, const uint32_t* __restrict__ h2_mask, const float* __restrict__ grad_rgb, int64_t n_pts,
-    float* __restrict__ grad_W2) {
+#define UBN_SHADE_DW2_PARAMS                                                                                                 \
+  const float* __restrict__ W3, const float* __restrict__ rgb, const float* __restrict__ h1_save,                            \
+      const float* __restrict__ h2_save, const uint32_t* __restrict__ h2_mask, const float* __restrict__ grad_rgb, int64_t n_pts, \
+      float* __restrict__ grad_W2
+#define UBN_SHADE_DW2_ARGS W3, rgb, h1_save, h2_save, h2_mask, grad_rgb, n_pts, grad_W2
+
+template <int kW, bool kThree, bool kPanel, bool kMask2>
+__device__ __forceinline__ void shade_dw2_tc(UBN_SHADE_DW2_PARAMS) {
+  // output tiles: kMT 16-row m-tiles, each shared by kThreads / 32 / kMT warps that take kNT of its 8-column n-tiles apiece
+  constexpr int kMT = kW / 16, kNT = n_tiles(kW) * kMT / (dw::kThreads / 32), kStride = stride(kW), kStrideB = dw::stride_b(kW);
   extern __shared__ __align__(16) uint8_t smem[];
   const int tid = threadIdx.x, lane = tid & 31, g = lane >> 2, t = lane & 3, warp = tid >> 5;
-  float* sW3 = reinterpret_cast<float*>(smem + dw::oW3);
-  for (int i = tid; i < 3 * kHidden; i += dw::kThreads) sW3[i] = W3[i];
+  const int mt = kMT == dw::kThreads / 32 ? warp : warp % kMT, j0 = kMT == dw::kThreads / 32 ? 0 : warp / kMT * kNT;
+  float* sW3 = reinterpret_cast<float*>(smem);
+  for (int i = tid; i < 3 * kW; i += dw::kThreads) sW3[i] = W3[i];
   float sum[kNT][4];
 #pragma unroll
   for (int j = 0; j < kNT; ++j) sum[j][0] = sum[j][1] = sum[j][2] = sum[j][3] = 0.f;
   const int sr = tid >> 3, c0 = 4 * (tid & 7);             // staging: sample row, 4 float4 column groups per thread
   const int64_t n_chunks = (n_pts + dw::kK - 1) / dw::kK;
-  Dw2Rows d;
+  Dw2Rows<kW> d;
   int64_t ch = blockIdx.x;
-  if (ch < n_chunks) dw2_load<kPanel, kMask2>(d, rgb, h1_save, h2_save, h2_mask, grad_rgb, ch * dw::kK + sr, n_pts, c0);
+  if (ch < n_chunks) dw2_load<kW, kPanel, kMask2>(d, rgb, h1_save, h2_save, h2_mask, grad_rgb, ch * dw::kK + sr, n_pts, c0);
   __syncthreads();                                         // sW3 staged
   for (int buf = 0; ch < n_chunks; ch += gridDim.x, buf ^= 1) {
-    float* sA = reinterpret_cast<float*>(smem + dw::oBuf + buf * dw::kBuf);                // dZ2 [sample][unit]
-    uint2* sB = reinterpret_cast<uint2*>(smem + dw::oBuf + buf * dw::kBuf + dw::kBufA);   // H1 {hi, lo} [sample][unit]
+    float* sA = reinterpret_cast<float*>(smem + dw::oBuf(kW) + buf * dw::buf(kW));                   // dZ2 [sample][unit]
+    uint2* sB = reinterpret_cast<uint2*>(smem + dw::oBuf(kW) + buf * dw::buf(kW) + dw::buf_a(kW));   // H1 {hi, lo} [sample][unit]
     float dz3[3];
 #pragma unroll
     for (int i = 0; i < 3; ++i) dz3[i] = d.gy[i] * d.y[i] * (1.f - d.y[i]);
 #pragma unroll
-    for (int q = 0; q < 4; ++q) {
+    for (int q = 0; q < kW / 32; ++q) {
       const int c = 32 * q + c0;
       float hv[4];
       if (kMask2) {
@@ -792,32 +833,32 @@ __global__ void __launch_bounds__(dw::kThreads, 1) k_shade_dw2_tc(
       float dv[4];
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const float dh = dz3[0] * sW3[c + e] + dz3[1] * sW3[kHidden + c + e] + dz3[2] * sW3[2 * kHidden + c + e];
+        const float dh = dz3[0] * sW3[c + e] + dz3[1] * sW3[kW + c + e] + dz3[2] * sW3[2 * kW + c + e];
         dv[e] = hv[e] > 0.f ? dh : 0.f;
       }
       *reinterpret_cast<float4*>(sA + sr * kStride + c) = make_float4(dv[0], dv[1], dv[2], dv[3]);
       const float hb[4] = {d.h1[q].x, d.h1[q].y, d.h1[q].z, d.h1[q].w};
       uint32_t hi[4], lo[4];
       split4(hb, hi, lo);
-      *reinterpret_cast<uint4*>(sB + sr * dw::kStrideB + c) = make_uint4(hi[0], lo[0], hi[1], lo[1]);
-      *reinterpret_cast<uint4*>(sB + sr * dw::kStrideB + c + 2) = make_uint4(hi[2], lo[2], hi[3], lo[3]);
+      *reinterpret_cast<uint4*>(sB + sr * kStrideB + c) = make_uint4(hi[0], lo[0], hi[1], lo[1]);
+      *reinterpret_cast<uint4*>(sB + sr * kStrideB + c + 2) = make_uint4(hi[2], lo[2], hi[3], lo[3]);
     }
     __syncthreads();                                       // this buffer is complete; the other one is no longer read
     if (ch + gridDim.x < n_chunks)
-      dw2_load<kPanel, kMask2>(d, rgb, h1_save, h2_save, h2_mask, grad_rgb, (ch + gridDim.x) * dw::kK + sr, n_pts, c0);
+      dw2_load<kW, kPanel, kMask2>(d, rgb, h1_save, h2_save, h2_mask, grad_rgb, (ch + gridDim.x) * dw::kK + sr, n_pts, c0);
     float acc[kNT][4];
 #pragma unroll
     for (int j = 0; j < kNT; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
 #pragma unroll
     for (int s = 0; s < dw::kK / 8; ++s) {
-      // A[m][k] = dZ2[sample 8 s + k][unit 16 w + m]
-      const float av[4] = {sA[(8 * s + t) * kStride + 16 * warp + g], sA[(8 * s + t) * kStride + 16 * warp + g + 8],
-                           sA[(8 * s + t + 4) * kStride + 16 * warp + g], sA[(8 * s + t + 4) * kStride + 16 * warp + g + 8]};
+      // A[m][k] = dZ2[sample 8 s + k][unit 16 mt + m]
+      const float av[4] = {sA[(8 * s + t) * kStride + 16 * mt + g], sA[(8 * s + t) * kStride + 16 * mt + g + 8],
+                           sA[(8 * s + t + 4) * kStride + 16 * mt + g], sA[(8 * s + t + 4) * kStride + 16 * mt + g + 8]};
       uint32_t ah[4], al[4];
       split4(av, ah, al);
 #pragma unroll
       for (int j = 0; j < kNT; ++j) {
-        const uint2 b0 = sB[(8 * s + t) * dw::kStrideB + 8 * j + g], b1 = sB[(8 * s + t + 4) * dw::kStrideB + 8 * j + g];
+        const uint2 b0 = sB[(8 * s + t) * kStrideB + 8 * (j0 + j) + g], b1 = sB[(8 * s + t + 4) * kStrideB + 8 * (j0 + j) + g];
         mma3<kThree>(acc[j], ah, al, make_uint4(b0.x, b1.x, b0.y, b1.y));
       }
     }
@@ -828,13 +869,33 @@ __global__ void __launch_bounds__(dw::kThreads, 1) k_shade_dw2_tc(
   }
 #pragma unroll
   for (int j = 0; j < kNT; ++j) {
-    const int c = 8 * j + 2 * t, m = 16 * warp + g;
-    atomicAdd(grad_W2 + m * kHidden + c, sum[j][0]);
-    atomicAdd(grad_W2 + m * kHidden + c + 1, sum[j][1]);
-    atomicAdd(grad_W2 + (m + 8) * kHidden + c, sum[j][2]);
-    atomicAdd(grad_W2 + (m + 8) * kHidden + c + 1, sum[j][3]);
+    const int c = 8 * (j0 + j) + 2 * t, m = 16 * mt + g;
+    atomicAdd(grad_W2 + m * kW + c, sum[j][0]);
+    atomicAdd(grad_W2 + m * kW + c + 1, sum[j][1]);
+    atomicAdd(grad_W2 + (m + 8) * kW + c, sum[j][2]);
+    atomicAdd(grad_W2 + (m + 8) * kW + c + 1, sum[j][3]);
   }
 }
+
+template <bool kThree, bool kPanel, bool kMask2>
+__global__ void __launch_bounds__(dw::kThreads, 1) k_shade_dw2_tc(UBN_SHADE_DW2_PARAMS) {
+  shade_dw2_tc<kHidden, kThree, kPanel, kMask2>(UBN_SHADE_DW2_ARGS);
+}
+
+// other widths: kCtas resident CTAs per SM
+template <int kW, bool kThree, int kCtas, bool kPanel, bool kMask2>
+__global__ void __launch_bounds__(dw::kThreads, kCtas) k_shade_dw2_tc_w(UBN_SHADE_DW2_PARAMS) {
+  shade_dw2_tc<kW, kThree, kPanel, kMask2>(UBN_SHADE_DW2_ARGS);
+}
+#undef UBN_SHADE_DW2_ARGS
+#undef UBN_SHADE_DW2_PARAMS
+
+// Width 64 (DirectMPIGO, K = 9): warps per CTA and resident CTAs per SM of each launch, from the -Xptxas -v figures of DESIGN §4
+namespace w64 {
+constexpr int kFwdWarps = 8, kFwdCtas = 2;
+constexpr int kBwdWarps = 8, kBwdCtas = 1;               // 3xTF32 needs 230 registers: 2 CTAs (128) or 4 warps x 3 (168) spill
+constexpr int kDw2Ctas = 2;
+}  // namespace w64
 
 }  // namespace tc
 }  // namespace ubn
@@ -848,17 +909,23 @@ int set_smem(K kernel, uint32_t bytes) {
   return finish(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
 }
 
-unsigned unit_grid(int64_t n_pts, int warps) {
+// at most ctas CTAs per SM, and no CTA without a unit for each of its warps
+unsigned unit_grid(int64_t n_pts, int warps, int ctas = 1) {
   const int64_t n_units = (n_pts + tc::kUnit - 1) / tc::kUnit;
-  return (unsigned)std::min<int64_t>(kNumSMs, (n_units + warps - 1) / warps);
+  return (unsigned)std::min<int64_t>((int64_t)kNumSMs * ctas, (n_units + warps - 1) / warps);
 }
 
-template <int kF, bool kSave, bool kThree, int kWarps, bool kPanel>
+// kW = 128 runs the kernels that keep their own names; other widths the _w kernels with kCtas resident CTAs per SM
+template <int kF, bool kSave, bool kThree, int kWarps, bool kPanel, int kW = tc::kHidden, int kCtas = 1>
 int launch_fwd(const float* feat, const float* vb, const int64_t* ray_id, const float* W1k, const float* W2, const float* b2,
                const float* W3, const float* b3, int64_t n, float* rgb, float* h1, float* h2, uint32_t* m1, cudaStream_t st) {
-  auto k = tc::k_shade_fwd_tc<kF, kSave, kThree, kWarps, kPanel>;
-  if (int e = set_smem(k, tc::kSmemFwd)) return e;
-  k<<<unit_grid(n, kWarps), 32 * kWarps, tc::kSmemFwd, st>>>(feat, vb, ray_id, W1k, W2, b2, W3, b3, n, rgb, h1, h2, m1);
+  auto k = [] {
+    if constexpr (kW == tc::kHidden) return tc::k_shade_fwd_tc<kF, kSave, kThree, kWarps, kPanel>;
+    else return tc::k_shade_fwd_tc_w<kF, kW, kSave, kThree, kWarps, kCtas, kPanel>;
+  }();
+  constexpr uint32_t bytes = tc::fw::smem(kW);
+  if (int e = set_smem(k, bytes)) return e;
+  k<<<unit_grid(n, kWarps, kCtas), 32 * kWarps, bytes, st>>>(feat, vb, ray_id, W1k, W2, b2, W3, b3, n, rgb, h1, h2, m1);
   UBN_LAUNCH_CHECK();
   return 0;
 }
@@ -871,30 +938,40 @@ int launch_fwd_p(bool panel, const float* feat, const float* vb, const int64_t* 
                : launch_fwd<kF, kSave, kThree, kWarps, false>(feat, vb, ray_id, W1k, W2, b2, W3, b3, n, rgb, h1, h2, nullptr, st);
 }
 
-template <int kF, bool kThree, int kWarps, bool kPanel, bool kMask1, bool kDz1Out>
+template <int kF, bool kThree, int kWarps, bool kPanel, bool kMask1, bool kDz1Out, int kW = tc::kHidden, int kCtas = 1>
 int launch_bwd(const float* feat, const int64_t* ray_id, const float* W1k, const float* W2, const float* W3, const float* rgb,
                const float* h1, const float* h2, const float* grad_rgb, int64_t n, float* grad_feat, float* grad_vb, float* gW1k,
                float* gb2, float* gW3, float* gb3, uint32_t* m2, const uint32_t* m1, float* dz1, cudaStream_t st) {
   auto k = [] {
-    if constexpr (kF == tc::kFeat) return tc::k_shade_bwd_tc<kThree, kWarps, kPanel, kMask1, kDz1Out>;
-    else return tc::k_shade_bwd_tc_k<kF, kThree, kWarps, kPanel, kMask1, kDz1Out>;
+    if constexpr (kW != tc::kHidden) {
+      static_assert(!kDz1Out, "the dZ1 round trip is a width-128 A/B engine");
+      return tc::k_shade_bwd_tc_w<kF, kW, kThree, kWarps, kCtas, kPanel, kMask1>;
+    } else if constexpr (kF == tc::kFeat) {
+      return tc::k_shade_bwd_tc<kThree, kWarps, kPanel, kMask1, kDz1Out>;
+    } else {
+      return tc::k_shade_bwd_tc_k<kF, kThree, kWarps, kPanel, kMask1, kDz1Out>;
+    }
   }();
-  const uint32_t bytes = tc::bk::smem_bytes(kWarps, kF);
+  const uint32_t bytes = tc::bk::smem_bytes(kWarps, kF, kW);
   if (int e = set_smem(k, bytes)) return e;
-  k<<<unit_grid(n, kWarps), 32 * kWarps, bytes, st>>>(feat, ray_id, W1k, W2, W3, rgb, h1, h2, grad_rgb, n, grad_feat, grad_vb, gW1k,
+  k<<<unit_grid(n, kWarps, kCtas), 32 * kWarps, bytes, st>>>(feat, ray_id, W1k, W2, W3, rgb, h1, h2, grad_rgb, n, grad_feat, grad_vb, gW1k,
                                                       gb2, gW3, gb3, m2, m1, dz1);
   UBN_LAUNCH_CHECK();
   return 0;
 }
 
-template <bool kThree, bool kPanel, bool kMask2>
+template <bool kThree, bool kPanel, bool kMask2, int kW = tc::kHidden, int kCtas = 1>
 int launch_dw2(const float* W3, const float* rgb, const float* h1, const float* h2, const uint32_t* m2, const float* grad_rgb,
                int64_t n, float* gW2, cudaStream_t st) {
-  auto k = tc::k_shade_dw2_tc<kThree, kPanel, kMask2>;
-  if (int e = set_smem(k, tc::dw::kSmem)) return e;
+  auto k = [] {
+    if constexpr (kW == tc::kHidden) return tc::k_shade_dw2_tc<kThree, kPanel, kMask2>;
+    else return tc::k_shade_dw2_tc_w<kW, kThree, kCtas, kPanel, kMask2>;
+  }();
+  constexpr uint32_t bytes = tc::dw::smem(kW);
+  if (int e = set_smem(k, bytes)) return e;
   const int64_t n_chunks = (n + tc::dw::kK - 1) / tc::dw::kK;
-  const unsigned grid = (unsigned)std::min<int64_t>(kNumSMs, n_chunks);
-  k<<<grid, tc::dw::kThreads, tc::dw::kSmem, st>>>(W3, rgb, h1, h2, m2, grad_rgb, n, gW2);
+  const unsigned grid = (unsigned)std::min<int64_t>((int64_t)kNumSMs * kCtas, n_chunks);
+  k<<<grid, tc::dw::kThreads, bytes, st>>>(W3, rgb, h1, h2, m2, grad_rgb, n, gW2);
   UBN_LAUNCH_CHECK();
   return 0;
 }
@@ -949,6 +1026,44 @@ int rgbnet_bwd_tc_fused(const float* feat, const int64_t* ray_id, const float* W
   if (panel) { if (one) UBN_DW(false, true, false); else UBN_DW(true, true, false); }
   if (one) UBN_DW(false, false, false); else UBN_DW(true, false, false);
 #undef UBN_DW
+}
+
+// hidden width kW != 128: the forward writes its saves in the panel layout only, and the backward runs with both ReLU masks
+template <int kF, int kW>
+int rgbnet_fwd_tc_w(const float* feat, const float* view_bias, const int64_t* ray_id, const float* W1k, const float* W2,
+                    const float* b2, const float* W3, const float* b3, int64_t n_pts, float* rgb, float* h1_save, float* h2_save,
+                    uint32_t* h1_mask, int single_pass, void* stream) {
+  const bool save = h1_save != nullptr && h2_save != nullptr;
+  if (save && (single_pass & 4) == 0) return finish(cudaErrorInvalidValue);
+  if (n_pts <= 0) return 0;
+  const bool one = (single_pass & 1) != 0;
+  cudaStream_t st = as_stream(stream);
+  constexpr int W = tc::w64::kFwdWarps, C = tc::w64::kFwdCtas;
+#define UBN_FWD_W(SAVE, THREE, M1) \
+  return launch_fwd<kF, SAVE, THREE, W, SAVE, kW, C>(feat, view_bias, ray_id, W1k, W2, b2, W3, b3, n_pts, rgb, h1_save, h2_save, M1, st)
+  if (save) { if (one) UBN_FWD_W(true, false, h1_mask); else UBN_FWD_W(true, true, h1_mask); }
+  if (one) UBN_FWD_W(false, false, nullptr); else UBN_FWD_W(false, true, nullptr);
+#undef UBN_FWD_W
+}
+
+template <int kF, int kW>
+int rgbnet_bwd_tc_fused_w(const float* feat, const int64_t* ray_id, const float* W1k, const float* W2, const float* W3,
+                          const float* rgb, const float* h1_save, const float* h2_save, const float* grad_rgb, int64_t n_pts,
+                          float* grad_feat, float* grad_view_bias, float* grad_W1k, float* grad_W2, float* grad_b2, float* grad_W3,
+                          float* grad_b3, uint32_t* h2_mask_scratch, const uint32_t* h1_mask, int single_pass, void* stream) {
+  if ((single_pass & 4) == 0 || h1_mask == nullptr || h2_mask_scratch == nullptr) return finish(cudaErrorInvalidValue);
+  if (n_pts <= 0) return 0;
+  const bool one = (single_pass & 1) != 0;
+  cudaStream_t st = as_stream(stream);
+  constexpr int W = tc::w64::kBwdWarps, C = tc::w64::kBwdCtas, C2 = tc::w64::kDw2Ctas;
+#define UBN_BWD_W(THREE)                                                                                                        \
+  launch_bwd<kF, THREE, W, true, true, false, kW, C>(feat, ray_id, W1k, W2, W3, rgb, h1_save, h2_save, grad_rgb, n_pts, grad_feat, \
+                                                     grad_view_bias, grad_W1k, grad_b2, grad_W3, grad_b3, h2_mask_scratch, h1_mask,  \
+                                                     nullptr, st)
+  if (int e = one ? UBN_BWD_W(false) : UBN_BWD_W(true)) return e;
+#undef UBN_BWD_W
+  if (one) return launch_dw2<false, true, true, kW, C2>(W3, rgb, h1_save, h2_save, h2_mask_scratch, grad_rgb, n_pts, grad_W2, st);
+  return launch_dw2<true, true, true, kW, C2>(W3, rgb, h1_save, h2_save, h2_mask_scratch, grad_rgb, n_pts, grad_W2, st);
 }
 
 }  // namespace
@@ -1010,4 +1125,31 @@ extern "C" int ubn_rgbnet_bwd_tc_fused_k(int n_feat, const float* feat, const in
     default: return finish(cudaErrorInvalidValue);
   }
 #undef UBN_BWD_K
+}
+
+extern "C" int ubn_rgbnet_fwd_tc_kw(int n_feat, int n_hidden, const float* feat, const float* view_bias, const int64_t* ray_id,
+                                    const float* W1k, const float* W2, const float* b2, const float* W3, const float* b3, int64_t n_pts,
+                                    float* rgb, float* h1_save, float* h2_save, uint32_t* h1_mask, int single_pass, void* stream) {
+  if (n_hidden == tc::kHidden)
+    return ubn_rgbnet_fwd_tc_k(n_feat, feat, view_bias, ray_id, W1k, W2, b2, W3, b3, n_pts, rgb, h1_save, h2_save, h1_mask,
+                               single_pass, stream);
+  if (n_hidden == 64 && n_feat == 9)
+    return rgbnet_fwd_tc_w<9, 64>(feat, view_bias, ray_id, W1k, W2, b2, W3, b3, n_pts, rgb, h1_save, h2_save, h1_mask, single_pass,
+                                  stream);
+  return finish(cudaErrorInvalidValue);
+}
+
+extern "C" int ubn_rgbnet_bwd_tc_fused_kw(int n_feat, int n_hidden, const float* feat, const int64_t* ray_id, const float* W1k,
+                                          const float* W2, const float* W3, const float* rgb, const float* h1_save, const float* h2_save,
+                                          const float* grad_rgb, int64_t n_pts, float* grad_feat, float* grad_view_bias,
+                                          float* grad_W1k, float* grad_W2, float* grad_b2, float* grad_W3, float* grad_b3,
+                                          uint32_t* h2_mask_scratch, const uint32_t* h1_mask, int single_pass, void* stream) {
+  if (n_hidden == tc::kHidden)
+    return ubn_rgbnet_bwd_tc_fused_k(n_feat, feat, ray_id, W1k, W2, W3, rgb, h1_save, h2_save, grad_rgb, n_pts, grad_feat,
+                                     grad_view_bias, grad_W1k, grad_W2, grad_b2, grad_W3, grad_b3, h2_mask_scratch, h1_mask,
+                                     single_pass, stream);
+  if (n_hidden == 64 && n_feat == 9)
+    return rgbnet_bwd_tc_fused_w<9, 64>(feat, ray_id, W1k, W2, W3, rgb, h1_save, h2_save, grad_rgb, n_pts, grad_feat, grad_view_bias,
+                                        grad_W1k, grad_W2, grad_b2, grad_W3, grad_b3, h2_mask_scratch, h1_mask, single_pass, stream);
+  return finish(cudaErrorInvalidValue);
 }

@@ -1021,7 +1021,7 @@ class DirectMPIGO(nn.Module):
         step_id = torch.arange(mask_inbbox.shape[1], device=dev).view(1, -1).expand_as(mask_inbbox)[mask_inbbox]
         return ray_pts[mask_inbbox], ray_id, step_id, N_samples
 
-    _shade = _ContractedBase._shade        # sigmoid(k0), or the rgbnet on cat[k0, view embedding] (cuBLAS for LLFF's width 64)
+    _shade = _ContractedBase._shade        # sigmoid(k0), or the rgbnet on cat[k0, view embedding] (tensor cores at llff's 9 / 64)
 
     def _fused_ok(self):
         return march.ndc_supported(self.k0.grid) and self.density.grid.is_cuda
