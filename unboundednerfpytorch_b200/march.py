@@ -1,8 +1,9 @@
 """Fused ray march (autograd.Function) over the C ABI: the hot path of FourierGridModel.forward
 (FourierGrid_model.py:554-621) and DirectContractedVoxGO.forward (dcvgo.py:264-331) -- ``March`` -- and of
 DirectMPIGO.forward (dmpigo.py:251-295) -- ``NdcMarch`` -- and of DirectVoxGO.forward (dvgo.py:330-366) -- ``BoxMarch`` --
-up to and including the feature-grid read, in 3 launches forward (pass A, scan, pass B) and 2 backward.  All share the dense pass-A records, the compaction and the
-gradient-buffer plumbing below.
+up to and including the feature-grid read, in 3 launches forward (pass A, scan, pass B) and 2 backward.  All three run the one
+forward body and the one backward body below (_forward / _backward); a geometry record (_Contracted, _Ndc, _Box) binds them
+to the C entries of its sampling policy.
 """
 import functools
 import os
@@ -47,6 +48,17 @@ def tma_supported(k0_grid):
             and min(k0_grid.shape[2:]) >= 2)
 
 
+def _set_mask_fields(c, mask, mask_scale, mask_shift):
+    """The mask-cache fields every march cfg carries: the occupancy grid's size and its world -> index map."""
+    c.use_maskcache = 1 if mask is not None else 0
+    if mask is not None:
+        for a in range(3):
+            c.mask_sz[a] = int(mask.shape[a])
+            c.mask_scale[a] = float(mask_scale[a])
+            c.mask_shift[a] = float(mask_shift[a])
+    return c
+
+
 def make_cfg(scene_center, scene_radius, bg_len, contracted_norm, n_samples, act_shift, interval,
              fast_color_thres, cumdist_thres=None, mask=None, mask_scale=None, mask_shift=None):
     c = UbnMarchCfg()
@@ -68,13 +80,7 @@ def make_cfg(scene_center, scene_radius, bg_len, contracted_norm, n_samples, act
     c.fast_color_thres = float(fast_color_thres)
     c.use_cumdist = 1 if cumdist_thres is not None else 0
     c.cumdist_thres = float(cumdist_thres) if cumdist_thres is not None else 0.0
-    c.use_maskcache = 1 if mask is not None else 0
-    if mask is not None:
-        for a in range(3):
-            c.mask_sz[a] = int(mask.shape[a])
-            c.mask_scale[a] = float(mask_scale[a])
-            c.mask_shift[a] = float(mask_shift[a])
-    return c
+    return _set_mask_fields(c, mask, mask_scale, mask_shift)
 
 
 def _pass_a_buffers(N, S, dev):
@@ -82,16 +88,6 @@ def _pass_a_buffers(N, S, dev):
     f32 = dict(dtype=torch.float32, device=dev)
     return (torch.empty(N * S, **f32), torch.empty(N * S, **f32), torch.empty(N * S, **f32), torch.empty(N * S, **f32),
             torch.empty(N * S, dtype=torch.uint8, device=dev), torch.empty(N, **f32), torch.empty(N, dtype=torch.int32, device=dev))
-
-
-def _compact(lib, nkeep, N, S, dense_known, st):
-    """offsets[N+1] = exclusive scan of the per-ray survivor counts, and M = offsets[N]: known without a host sync when nothing
-    can be masked out, else the march's one device-to-host read."""
-    offsets = torch.empty(N + 1, dtype=torch.int64, device=nkeep.device)
-    scratch = torch.empty(N // 1024 + 4, dtype=torch.int64, device=nkeep.device)
-    check(lib.ubn_exclusive_scan_i32(ptr(nkeep), c_i64(N), ptr(offsets), ptr(scratch), st))
-    M = N * S if dense_known else int(offsets[N].item())
-    return offsets, M
 
 
 def _grad_target(param, meta, want, dev):
@@ -112,6 +108,126 @@ def _hand_over(param, grad, buf):
     return grad
 
 
+class _Geometry:
+    """Binds _forward / _backward to one sampling policy's C entries ubn_<entry>_{density,feature}_{fwd,bwd}, timed under the
+    same names without the ubn_ prefix.  These defaults are the NDC march's; the contracted and box marches override what
+    their entries add."""
+    entry = 'march_ndc'
+    lead = ()              # tensors every entry takes right after rays_o, rays_d
+    shift = ()             # pass A's arguments right after the density grid's desc
+
+    def steps(self, cfg):
+        return cfg.n_samples
+
+    def pass_a_tail(self, dev):
+        return ()
+
+    def survivors(self, offsets, tail, N, S):
+        return int(offsets[N].item())         # the march's one device-to-host read
+
+    def pass_b(self, lib, head, k0_grid, dens, alpha, weight, out, st):
+        """Launch pass B into out = (feat, alpha, weight, ray_id, step_id).  Returns the further outputs: (those with a gradient,
+        which the density backward takes right after g_alpha), (constants)."""
+        with _cabi.timed(self.entry + '_feature_fwd'):
+            check(getattr(lib, f'ubn_{self.entry}_feature_fwd')(*head, ptr(alpha), ptr(weight), *map(ptr, out), st))
+        return (), ()
+
+
+class _Contracted(_Geometry):
+    """Every entry takes the t table; pass B also writes raw_density, t and the inner-sphere flag, and on the render path may
+    stage the feature grid by TMA."""
+    entry = 'march'
+
+    def __init__(self, t_table, dense_known, coherent):
+        self.lead = (t_table,)
+        self.dense_known, self.coherent = dense_known, coherent
+
+    def survivors(self, offsets, tail, N, S):
+        # known without a host sync when nothing can be masked out
+        return N * S if self.dense_known else super().survivors(offsets, tail, N, S)
+
+    def pass_b(self, lib, head, k0_grid, dens, alpha, weight, out, st):
+        feat, o_alpha, o_weight, ray_id, step_id = out
+        M, dev = o_alpha.shape[0], o_alpha.device
+        o_dens = torch.empty(M, dtype=torch.float32, device=dev)
+        o_t = torch.empty(M, dtype=torch.float32, device=dev)
+        o_inner = torch.empty(M, dtype=torch.bool, device=dev)
+        # render path: bricks of the feature grid staged by TMA for 32 adjacent rays x 4 steps
+        use_tma = self.coherent and tma_supported(k0_grid) and not torch.is_grad_enabled()
+        name = 'march_feature_fwd_tma' if use_tma else 'march_feature_fwd'
+        with _cabi.timed(name):
+            check(getattr(lib, 'ubn_' + name)(*head, *map(ptr, (dens, alpha, weight, feat, o_dens, o_alpha, o_weight, ray_id, step_id,
+                                                                 o_t, o_inner)), *((ptr(TMA_STATS),) if use_tma else ()), st))
+        return (o_dens,), (o_t, o_inner)
+
+
+def _forward(ctx, geo, density_grid, k0_grid, rays_o, rays_d, mask_world, cfg, ddesc, kdesc):
+    """Pass A (dense per-sample records), the exclusive scan of the per-ray survivor counts, pass B (compacted records and the
+    feature read).  Returns (weights[M], alphainv_last[N], raw_alpha[M], *geometry outputs with a gradient, k0_feat[M,C],
+    ray_id[M] i64, step_id[M] i64, *constant geometry outputs)."""
+    dev = rays_o.device
+    rays_o = rays_o.contiguous().float()
+    rays_d = rays_d.contiguous().float()
+    N, S = rays_o.shape[0], geo.steps(cfg)
+    f32 = dict(dtype=torch.float32, device=dev)
+    records = _pass_a_buffers(N, S, dev)
+    dens, alpha, weight, T, flags, last, nkeep = records
+    tail = geo.pass_a_tail(dev)
+    with ops._Guard(rays_o) as lib:
+        st = stream_of(rays_o)
+        rays = (ptr(rays_o), ptr(rays_d), *map(ptr, geo.lead))
+        with _cabi.timed(geo.entry + '_density_fwd'):
+            check(getattr(lib, f'ubn_{geo.entry}_density_fwd')(*rays, ptr(density_grid), ddesc, *geo.shift, ptr(mask_world), cfg,
+                                                                 c_i64(N), *map(ptr, records), *map(ptr, tail), st))
+        offsets = torch.empty(N + 1, dtype=torch.int64, device=dev)
+        scratch = torch.empty(N // 1024 + 4, dtype=torch.int64, device=dev)
+        check(lib.ubn_exclusive_scan_i32(ptr(nkeep), c_i64(N), ptr(offsets), ptr(scratch), st))
+        M = geo.survivors(offsets, tail, N, S)
+        out = (torch.empty(M, k0_grid.shape[1], **f32), torch.empty(M, **f32), torch.empty(M, **f32),
+               torch.empty(M, dtype=torch.int64, device=dev), torch.empty(M, dtype=torch.int64, device=dev))
+        feat, o_alpha, o_weight, ray_id, step_id = out
+        head = (*rays, ptr(k0_grid), kdesc, cfg, c_i64(N), ptr(flags), ptr(offsets))
+        differentiable, constant = geo.pass_b(lib, head, k0_grid, dens, alpha, weight, out, st)
+    ctx.save_for_backward(rays_o, rays_d, dens, alpha, weight, T, flags, last, offsets)
+    ctx.geo, ctx.cfg, ctx.ddesc, ctx.kdesc = geo, cfg, ddesc, kdesc
+    ctx.n_extra = len(differentiable)
+    ctx.dmeta = (density_grid.shape, density_grid.stride())
+    ctx.kmeta = (k0_grid.shape, k0_grid.stride())
+    ctx.dparam, ctx.kparam = density_grid, k0_grid      # for their persistent gradient buffers (_grad_target)
+    ctx.mark_non_differentiable(ray_id, step_id, *constant)
+    return (o_weight, last, o_alpha, *differentiable, feat, ray_id, step_id, *constant)
+
+
+@torch.autograd.function.once_differentiable
+def _backward(ctx, g_weight, g_last, g_alpha, *rest):
+    """The k0 scatter, then the density reverse scan and scatter.  Gradients for (density_grid, k0_grid), None for the rest."""
+    rays_o, rays_d, dens, alpha, weight, T, flags, last, offsets = ctx.saved_tensors
+    geo = ctx.geo
+    dev = rays_o.device
+    N = rays_o.shape[0]
+    cont = lambda g: g.contiguous() if g is not None else None
+    g_extra = [cont(g) for g in rest[:ctx.n_extra]]
+    g_weight, g_last, g_alpha, g_feat = map(cont, (g_weight, g_last, g_alpha, rest[ctx.n_extra]))
+    with ops._Guard(rays_o) as lib:
+        st = stream_of(rays_o)
+        rays = (ptr(rays_o), ptr(rays_d), *map(ptr, geo.lead))
+        want_k = ctx.needs_input_grad[1] and g_feat is not None
+        want_d = ctx.needs_input_grad[0]
+        grad_d, buf_d = _grad_target(ctx.dparam, ctx.dmeta, want_d, dev)
+        grad_k, buf_k = _grad_target(ctx.kparam, ctx.kmeta, want_k, dev)
+        if want_k:
+            with _cabi.timed(geo.entry + '_feature_bwd'):
+                check(getattr(lib, f'ubn_{geo.entry}_feature_bwd')(*rays, ctx.kdesc, ctx.cfg, c_i64(N), ptr(flags), ptr(offsets),
+                                                                     ptr(g_feat), ptr(grad_k), st))
+        if want_d:
+            gd = torch.empty_like(dens)     # per-sample density gradients between the run scatter's two launches
+            with _cabi.timed(geo.entry + '_density_bwd'):
+                check(getattr(lib, f'ubn_{geo.entry}_density_bwd')(*rays, ctx.ddesc, ctx.cfg, c_i64(N), *map(ptr, (
+                    dens, alpha, weight, T, flags, last, offsets, g_weight, g_alpha, *g_extra, g_last, grad_d, gd)), st))
+    grads = (_hand_over(ctx.dparam, grad_d, buf_d), _hand_over(ctx.kparam, grad_k, buf_k))
+    return grads + (None,) * (len(ctx.needs_input_grad) - 2)
+
+
 class March(torch.autograd.Function):
     """(density_grid, k0_grid, rays) -> compacted per-survivor records.
 
@@ -122,75 +238,10 @@ class March(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, density_grid, k0_grid, rays_o, rays_d, t_table, mask_world, cfg, ddesc, kdesc, dense_known, coherent=False):
-        dev = rays_o.device
-        rays_o = rays_o.contiguous().float()
-        rays_d = rays_d.contiguous().float()
-        N, S = rays_o.shape[0], cfg.n_samples
-        f32 = dict(dtype=torch.float32, device=dev)
-        dens, alpha, weight, T, flags, last, nkeep = _pass_a_buffers(N, S, dev)
-        with ops._Guard(rays_o) as lib:
-            st = stream_of(rays_o)
-            with _cabi.timed('march_density_fwd'):
-                check(lib.ubn_march_density_fwd(ptr(rays_o), ptr(rays_d), ptr(t_table), ptr(density_grid), ddesc,
-                                                ptr(mask_world), cfg, c_i64(N), ptr(dens), ptr(alpha), ptr(weight), ptr(T),
-                                                ptr(flags), ptr(last), ptr(nkeep), st))
-            offsets, M = _compact(lib, nkeep, N, S, dense_known, st)
-            C = k0_grid.shape[1]
-            feat = torch.empty(M, C, **f32)
-            o_dens = torch.empty(M, **f32)
-            o_alpha = torch.empty(M, **f32)
-            o_weight = torch.empty(M, **f32)
-            ray_id = torch.empty(M, dtype=torch.int64, device=dev)
-            step_id = torch.empty(M, dtype=torch.int64, device=dev)
-            o_t = torch.empty(M, **f32)
-            o_inner = torch.empty(M, dtype=torch.bool, device=dev)
-            use_tma = coherent and tma_supported(k0_grid) and not torch.is_grad_enabled()
-            with _cabi.timed('march_feature_fwd_tma' if use_tma else 'march_feature_fwd'):
-                if use_tma:       # render path: bricks of the feature grid staged by TMA for 32 adjacent rays x 4 steps
-                    check(lib.ubn_march_feature_fwd_tma(ptr(rays_o), ptr(rays_d), ptr(t_table), ptr(k0_grid), kdesc, cfg, c_i64(N),
-                                                        ptr(flags), ptr(offsets), ptr(dens), ptr(alpha), ptr(weight), ptr(feat),
-                                                        ptr(o_dens), ptr(o_alpha), ptr(o_weight), ptr(ray_id), ptr(step_id),
-                                                        ptr(o_t), ptr(o_inner), ptr(TMA_STATS), st))
-                else:
-                    check(lib.ubn_march_feature_fwd(ptr(rays_o), ptr(rays_d), ptr(t_table), ptr(k0_grid), kdesc, cfg, c_i64(N),
-                                                    ptr(flags), ptr(offsets), ptr(dens), ptr(alpha), ptr(weight), ptr(feat),
-                                                    ptr(o_dens), ptr(o_alpha), ptr(o_weight), ptr(ray_id), ptr(step_id),
-                                                    ptr(o_t), ptr(o_inner), st))
-        ctx.save_for_backward(rays_o, rays_d, t_table, dens, alpha, weight, T, flags, last, offsets)
-        ctx.cfg, ctx.ddesc, ctx.kdesc = cfg, ddesc, kdesc
-        ctx.dmeta = (density_grid.shape, density_grid.stride())
-        ctx.kmeta = (k0_grid.shape, k0_grid.stride())
-        ctx.dparam, ctx.kparam = density_grid, k0_grid      # for their persistent gradient buffers (_grad_target)
-        ctx.mark_non_differentiable(ray_id, step_id, o_t, o_inner)
-        return o_weight, last, o_alpha, o_dens, feat, ray_id, step_id, o_t, o_inner
+        return _forward(ctx, _Contracted(t_table, dense_known, coherent), density_grid, k0_grid, rays_o, rays_d, mask_world, cfg,
+                        ddesc, kdesc)
 
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, g_weight, g_last, g_alpha, g_dens, g_feat, *unused):
-        rays_o, rays_d, t_table, dens, alpha, weight, T, flags, last, offsets = ctx.saved_tensors
-        dev = rays_o.device
-        N = rays_o.shape[0]
-        cont = lambda g: g.contiguous() if g is not None else None
-        g_weight, g_last, g_alpha, g_dens, g_feat = map(cont, (g_weight, g_last, g_alpha, g_dens, g_feat))
-        with ops._Guard(rays_o) as lib:
-            want_k = ctx.needs_input_grad[1] and g_feat is not None
-            want_d = ctx.needs_input_grad[0]
-            grad_d, buf_d = _grad_target(ctx.dparam, ctx.dmeta, want_d, dev)
-            grad_k, buf_k = _grad_target(ctx.kparam, ctx.kmeta, want_k, dev)
-            if want_k:
-                with _cabi.timed('march_feature_bwd'):
-                    check(lib.ubn_march_feature_bwd(ptr(rays_o), ptr(rays_d), ptr(t_table), ctx.kdesc, ctx.cfg, c_i64(N),
-                                                    ptr(flags), ptr(offsets), ptr(g_feat), ptr(grad_k), stream_of(rays_o)))
-            if want_d:
-                gd = torch.empty_like(dens)     # per-sample density gradients between the run scatter's two launches
-                with _cabi.timed('march_density_bwd'):
-                    check(lib.ubn_march_density_bwd(ptr(rays_o), ptr(rays_d), ptr(t_table), ctx.ddesc, ctx.cfg, c_i64(N),
-                                                    ptr(dens), ptr(alpha), ptr(weight), ptr(T), ptr(flags), ptr(last),
-                                                    ptr(offsets), ptr(g_weight), ptr(g_alpha), ptr(g_dens), ptr(g_last),
-                                                    ptr(grad_d), ptr(gd), stream_of(rays_o)))
-        grad_d = _hand_over(ctx.dparam, grad_d, buf_d)
-        grad_k = _hand_over(ctx.kparam, grad_k, buf_k)
-        return grad_d, grad_k, None, None, None, None, None, None, None, None, None
+    backward = staticmethod(_backward)
 
 
 def make_ndc_cfg(xyz_min, xyz_max, n_samples, interval, fast_color_thres, mask, mask_scale, mask_shift):
@@ -198,20 +249,21 @@ def make_ndc_cfg(xyz_min, xyz_max, n_samples, interval, fast_color_thres, mask, 
     for a in range(3):
         c.xyz_min[a] = float(xyz_min[a])
         c.xyz_max[a] = float(xyz_max[a])
-        c.mask_sz[a] = int(mask.shape[a])
-        c.mask_scale[a] = float(mask_scale[a])
-        c.mask_shift[a] = float(mask_shift[a])
     c.n_samples = int(n_samples)
     c.interval = float(interval)
     c.fast_color_thres = float(fast_color_thres)
-    c.use_maskcache = 1
-    return c
+    return _set_mask_fields(c, mask, mask_scale, mask_shift)
 
 
 def ndc_supported(k0_grid):
     """Grids the fused NDC feature read covers: single-slab channels-last k0 with 3 or 9 channels, >= 2 voxels per axis."""
     return (k0_grid.is_cuda and k0_grid.dim() == 5 and k0_grid.shape[0] == 1 and k0_grid.shape[1] in (3, 9)
             and k0_grid.stride(1) == 1 and min(k0_grid.shape[2:]) >= 2 and k0_grid[0, 0].numel() < 2 ** 31)
+
+
+class _Ndc(_Geometry):
+    def __init__(self, act_shift_grid, sdesc):
+        self.shift = (ptr(act_shift_grid), sdesc)
 
 
 class NdcMarch(torch.autograd.Function):
@@ -222,63 +274,9 @@ class NdcMarch(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, density_grid, k0_grid, act_shift_grid, rays_o, rays_d, mask_world, cfg, ddesc, kdesc, sdesc):
-        dev = rays_o.device
-        rays_o = rays_o.contiguous().float()
-        rays_d = rays_d.contiguous().float()
-        N, S = rays_o.shape[0], cfg.n_samples
-        f32 = dict(dtype=torch.float32, device=dev)
-        dens, alpha, weight, T, flags, last, nkeep = _pass_a_buffers(N, S, dev)
-        with ops._Guard(rays_o) as lib:
-            st = stream_of(rays_o)
-            with _cabi.timed('march_ndc_density_fwd'):
-                check(lib.ubn_march_ndc_density_fwd(ptr(rays_o), ptr(rays_d), ptr(density_grid), ddesc, ptr(act_shift_grid), sdesc,
-                                                    ptr(mask_world), cfg, c_i64(N), ptr(dens), ptr(alpha), ptr(weight), ptr(T),
-                                                    ptr(flags), ptr(last), ptr(nkeep), st))
-            offsets, M = _compact(lib, nkeep, N, S, False, st)
-            feat = torch.empty(M, k0_grid.shape[1], **f32)
-            o_alpha = torch.empty(M, **f32)
-            o_weight = torch.empty(M, **f32)
-            ray_id = torch.empty(M, dtype=torch.int64, device=dev)
-            step_id = torch.empty(M, dtype=torch.int64, device=dev)
-            with _cabi.timed('march_ndc_feature_fwd'):
-                check(lib.ubn_march_ndc_feature_fwd(ptr(rays_o), ptr(rays_d), ptr(k0_grid), kdesc, cfg, c_i64(N), ptr(flags),
-                                                    ptr(offsets), ptr(alpha), ptr(weight), ptr(feat), ptr(o_alpha), ptr(o_weight),
-                                                    ptr(ray_id), ptr(step_id), st))
-        ctx.save_for_backward(rays_o, rays_d, dens, alpha, weight, T, flags, last, offsets)
-        ctx.cfg, ctx.ddesc, ctx.kdesc = cfg, ddesc, kdesc
-        ctx.dmeta = (density_grid.shape, density_grid.stride())
-        ctx.kmeta = (k0_grid.shape, k0_grid.stride())
-        ctx.dparam, ctx.kparam = density_grid, k0_grid
-        ctx.mark_non_differentiable(ray_id, step_id)
-        return o_weight, last, o_alpha, feat, ray_id, step_id
+        return _forward(ctx, _Ndc(act_shift_grid, sdesc), density_grid, k0_grid, rays_o, rays_d, mask_world, cfg, ddesc, kdesc)
 
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, g_weight, g_last, g_alpha, g_feat, *unused):
-        rays_o, rays_d, dens, alpha, weight, T, flags, last, offsets = ctx.saved_tensors
-        dev = rays_o.device
-        N = rays_o.shape[0]
-        cont = lambda g: g.contiguous() if g is not None else None
-        g_weight, g_last, g_alpha, g_feat = map(cont, (g_weight, g_last, g_alpha, g_feat))
-        with ops._Guard(rays_o) as lib:
-            st = stream_of(rays_o)
-            want_k = ctx.needs_input_grad[1] and g_feat is not None
-            want_d = ctx.needs_input_grad[0]
-            grad_d, buf_d = _grad_target(ctx.dparam, ctx.dmeta, want_d, dev)
-            grad_k, buf_k = _grad_target(ctx.kparam, ctx.kmeta, want_k, dev)
-            if want_k:
-                with _cabi.timed('march_ndc_feature_bwd'):
-                    check(lib.ubn_march_ndc_feature_bwd(ptr(rays_o), ptr(rays_d), ctx.kdesc, ctx.cfg, c_i64(N), ptr(flags),
-                                                        ptr(offsets), ptr(g_feat), ptr(grad_k), st))
-            if want_d:
-                gd = torch.empty_like(dens)
-                with _cabi.timed('march_ndc_density_bwd'):
-                    check(lib.ubn_march_ndc_density_bwd(ptr(rays_o), ptr(rays_d), ctx.ddesc, ctx.cfg, c_i64(N), ptr(dens),
-                                                        ptr(alpha), ptr(weight), ptr(T), ptr(flags), ptr(last), ptr(offsets),
-                                                        ptr(g_weight), ptr(g_alpha), ptr(g_last), ptr(grad_d), ptr(gd), st))
-        grad_d = _hand_over(ctx.dparam, grad_d, buf_d)
-        grad_k = _hand_over(ctx.kparam, grad_k, buf_k)
-        return grad_d, grad_k, None, None, None, None, None, None, None, None
+    backward = staticmethod(_backward)
 
 
 def box_s_max(xyz_min, xyz_max, stepdist):
@@ -307,13 +305,7 @@ def make_box_cfg(xyz_min, xyz_max, near, stepdist, act_shift, interval, fast_col
     c.act_shift = float(act_shift)
     c.interval = float(interval)
     c.fast_color_thres = float(fast_color_thres)
-    c.use_maskcache = 1 if mask is not None else 0
-    if mask is not None:
-        for a in range(3):
-            c.mask_sz[a] = int(mask.shape[a])
-            c.mask_scale[a] = float(mask_scale[a])
-            c.mask_shift[a] = float(mask_shift[a])
-    return c
+    return _set_mask_fields(c, mask, mask_scale, mask_shift)
 
 
 def box_supported(density_grid, k0_grid):
@@ -326,6 +318,24 @@ def box_supported(density_grid, k0_grid):
             and (k0_grid.shape[1] != 12 or k0_grid.data_ptr() % 16 == 0))
 
 
+class _Box(_Geometry):
+    """Records of cfg.s_max steps per ray; pass A also sets an overflow word when a ray needs more."""
+    entry = 'march_box'
+
+    def steps(self, cfg):
+        return cfg.s_max
+
+    def pass_a_tail(self, dev):
+        return (torch.zeros(1, dtype=torch.int32, device=dev),)
+
+    def survivors(self, offsets, tail, N, S):
+        # the march's one device-to-host read: the survivor count and the overflow word together
+        M, over = torch.stack([offsets[N], tail[0][0].to(torch.int64)]).tolist() if N > 0 else (0, 0)
+        if over:
+            raise RuntimeError(f'box march: a ray needs more than s_max = {S} steps (bbox / stepsize / ray origin out of range)')
+        return M
+
+
 class BoxMarch(torch.autograd.Function):
     """DirectVoxGO's march: (density_grid, k0_grid, rays) -> compacted per-survivor records sorted by (ray, step).
 
@@ -334,65 +344,6 @@ class BoxMarch(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, density_grid, k0_grid, rays_o, rays_d, mask_world, cfg, ddesc, kdesc):
-        dev = rays_o.device
-        rays_o = rays_o.contiguous().float()
-        rays_d = rays_d.contiguous().float()
-        N, S = rays_o.shape[0], cfg.s_max
-        f32 = dict(dtype=torch.float32, device=dev)
-        dens, alpha, weight, T, flags, last, nkeep = _pass_a_buffers(N, S, dev)
-        overflow = torch.zeros(1, dtype=torch.int32, device=dev)
-        with ops._Guard(rays_o) as lib:
-            st = stream_of(rays_o)
-            with _cabi.timed('march_box_density_fwd'):
-                check(lib.ubn_march_box_density_fwd(ptr(rays_o), ptr(rays_d), ptr(density_grid), ddesc, ptr(mask_world), cfg,
-                                                    c_i64(N), ptr(dens), ptr(alpha), ptr(weight), ptr(T), ptr(flags), ptr(last),
-                                                    ptr(nkeep), ptr(overflow), st))
-            offsets, _ = _compact(lib, nkeep, N, S, True, st)
-            # the march's one device-to-host read: the survivor count and the overflow word together
-            M, over = torch.stack([offsets[N], overflow[0].to(torch.int64)]).tolist() if N > 0 else (0, 0)
-            if over:
-                raise RuntimeError(f'box march: a ray needs more than s_max = {S} steps (bbox / stepsize / ray origin out of range)')
-            feat = torch.empty(M, k0_grid.shape[1], **f32)
-            o_alpha = torch.empty(M, **f32)
-            o_weight = torch.empty(M, **f32)
-            ray_id = torch.empty(M, dtype=torch.int64, device=dev)
-            step_id = torch.empty(M, dtype=torch.int64, device=dev)
-            with _cabi.timed('march_box_feature_fwd'):
-                check(lib.ubn_march_box_feature_fwd(ptr(rays_o), ptr(rays_d), ptr(k0_grid), kdesc, cfg, c_i64(N), ptr(flags),
-                                                    ptr(offsets), ptr(alpha), ptr(weight), ptr(feat), ptr(o_alpha), ptr(o_weight),
-                                                    ptr(ray_id), ptr(step_id), st))
-        ctx.save_for_backward(rays_o, rays_d, dens, alpha, weight, T, flags, last, offsets)
-        ctx.cfg, ctx.ddesc, ctx.kdesc = cfg, ddesc, kdesc
-        ctx.dmeta = (density_grid.shape, density_grid.stride())
-        ctx.kmeta = (k0_grid.shape, k0_grid.stride())
-        ctx.dparam, ctx.kparam = density_grid, k0_grid
-        ctx.mark_non_differentiable(ray_id, step_id)
-        return o_weight, last, o_alpha, feat, ray_id, step_id
+        return _forward(ctx, _Box(), density_grid, k0_grid, rays_o, rays_d, mask_world, cfg, ddesc, kdesc)
 
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, g_weight, g_last, g_alpha, g_feat, *unused):
-        rays_o, rays_d, dens, alpha, weight, T, flags, last, offsets = ctx.saved_tensors
-        dev = rays_o.device
-        N = rays_o.shape[0]
-        cont = lambda g: g.contiguous() if g is not None else None
-        g_weight, g_last, g_alpha, g_feat = map(cont, (g_weight, g_last, g_alpha, g_feat))
-        with ops._Guard(rays_o) as lib:
-            st = stream_of(rays_o)
-            want_k = ctx.needs_input_grad[1] and g_feat is not None
-            want_d = ctx.needs_input_grad[0]
-            grad_d, buf_d = _grad_target(ctx.dparam, ctx.dmeta, want_d, dev)
-            grad_k, buf_k = _grad_target(ctx.kparam, ctx.kmeta, want_k, dev)
-            if want_k:
-                with _cabi.timed('march_box_feature_bwd'):
-                    check(lib.ubn_march_box_feature_bwd(ptr(rays_o), ptr(rays_d), ctx.kdesc, ctx.cfg, c_i64(N), ptr(flags),
-                                                        ptr(offsets), ptr(g_feat), ptr(grad_k), st))
-            if want_d:
-                gd = torch.empty_like(dens)
-                with _cabi.timed('march_box_density_bwd'):
-                    check(lib.ubn_march_box_density_bwd(ptr(rays_o), ptr(rays_d), ctx.ddesc, ctx.cfg, c_i64(N), ptr(dens),
-                                                        ptr(alpha), ptr(weight), ptr(T), ptr(flags), ptr(last), ptr(offsets),
-                                                        ptr(g_weight), ptr(g_alpha), ptr(g_last), ptr(grad_d), ptr(gd), st))
-        grad_d = _hand_over(ctx.dparam, grad_d, buf_d)
-        grad_k = _hand_over(ctx.kparam, grad_k, buf_k)
-        return grad_d, grad_k, None, None, None, None, None, None
+    backward = staticmethod(_backward)

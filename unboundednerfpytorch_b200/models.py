@@ -43,19 +43,29 @@ def _view_embed(viewdirs, viewfreq):
     return torch.cat([viewdirs, emb.sin(), emb.cos()], -1)
 
 
-class _ContractedBase(nn.Module):
-    """Shared machinery of the two contracted-space models."""
+class _GridModel(nn.Module):
+    """What the four models share: the host copies of the geometry the march cfgs take by value, activate_density, the TV
+    terms, the rgbnet and its shading, and the mask cache's lattice and rebuild."""
 
-    T_BOUNDARY = 2.0          # dcvgo.py:243-244; FourierGridModel overrides with 1.5
-    USE_CUMDIST = False
-    USE_MASKCACHE = False
+    _HOST_BUFFERS = ('xyz_min', 'xyz_max')        # the two bbox buffers the march cfg takes by value
+    _host_cache = None          # (mask_cache it was read from, host bbox, host mask geometry)
 
-    # ---- helpers --------------------------------------------------------------------------------
-    def _host(self):
-        if self._host_cache is None:
-            self._host_cache = dict(center=self.scene_center.detach().cpu().tolist(),
-                                    radius=self.scene_radius.detach().cpu().tolist())
+    def _host_geometry(self):
+        """The geometry the march cfgs take by value, read to the host once and again after _apply, a state-dict load or a
+        new mask_cache."""
+        if self._host_cache is None or self._host_cache[0] is not self.mask_cache:
+            mc = self.mask_cache
+            self._host_cache = (mc, tuple(getattr(self, name).detach().cpu().tolist() for name in self._HOST_BUFFERS),
+                                (mc.xyz2ijk_scale.cpu().tolist(), mc.xyz2ijk_shift.cpu().tolist()))
         return self._host_cache
+
+    def _host(self):
+        """The two _HOST_BUFFERS as host lists."""
+        return self._host_geometry()[1]
+
+    def _mask_geometry(self):
+        """(mask_scale, mask_shift): the mask cache's world -> index map as host lists."""
+        return self._host_geometry()[2]
 
     def _apply(self, fn, *a, **k):
         self._host_cache = None
@@ -65,6 +75,101 @@ class _ContractedBase(nn.Module):
         self._host_cache = None
         return super()._load_from_state_dict(*a, **k)
 
+    def _voxel_size(self):
+        return self.voxel_size
+
+    def _voxel_size_ratio(self):
+        return self.voxel_size_ratio
+
+    def _density_shift(self):
+        return self.act_shift
+
+    def activate_density(self, density, interval=None):
+        interval = interval if interval is not None else self._voxel_size_ratio()
+        shape = density.shape
+        return Raw2Alpha.apply(density.flatten().contiguous(), self._density_shift(), interval).reshape(shape)
+
+    def density_total_variation_add_grad(self, weight, dense_mode):
+        self.density.total_variation_add_grad(*self._tv_weights(self.density, weight, dense_mode))
+
+    def k0_total_variation_add_grad(self, weight, dense_mode):
+        self.k0.total_variation_add_grad(*self._tv_weights(self.k0, weight, dense_mode))
+
+    def tv_terms(self, weight_density=0., weight_k0=0., dense_mode=True):
+        """{grid parameter: (wx, wy, wz, dense_mode)} with the weights of the two methods above -- the form
+        dist.reduce_tv_step consumes to pipeline all-reduce / TV / Adam slab by slab."""
+        return {grid.grid: self._tv_weights(grid, weight, dense_mode)
+                for grid, weight in ((self.density, weight_density), (self.k0, weight_k0)) if weight > 0}
+
+    def _add_rgbnet(self, feat_dim, viewbase_pe, width, depth):
+        """The view-frequency buffer, then the rgbnet on cat[feat_dim features, view embedding]."""
+        self.register_buffer('viewfreq', torch.FloatTensor([(2 ** i) for i in range(viewbase_pe)]))
+        self.rgbnet = _make_rgbnet(3 + 3 * viewbase_pe * 2 + feat_dim, width, depth)
+
+    def _shade(self, k0, viewdirs, ray_id):
+        if self.rgbnet is None:
+            return torch.sigmoid(k0)
+        emb = _view_embed(viewdirs, self.viewfreq).flatten(0, -2)
+        if shade_mod.supported(self.rgbnet, k0.shape[-1]):
+            return shade_mod.shade(self.rgbnet, k0, emb, ray_id)          # fused on-chip MLP (csrc/shade.cu)
+        return torch.sigmoid(self.rgbnet(torch.cat([k0, emb[ray_id]], -1)))   # other widths / depths: torch (cuBLAS)
+
+    def _mask_lattice(self, world_size):
+        """[X, Y, Z, 3]: linspace(xyz_min, xyz_max, world_size) per axis, the points a mask cache is built on."""
+        ws = [int(v) for v in world_size]
+        axes = [torch.linspace(float(self.xyz_min[a]), float(self.xyz_max[a]), ws[a], device=self.xyz_min.device) for a in range(3)]
+        return torch.stack(torch.meshgrid(*axes, indexing='ij'), -1)
+
+    def _set_mask_cache(self, mask):
+        self.mask_cache = G.MaskGrid(path=None, mask=mask, xyz_min=self.xyz_min, xyz_max=self.xyz_max).to(mask.device)
+
+    @torch.no_grad()
+    def update_occupancy_cache(self):
+        """mask_cache.mask &= max_pool3d(Raw2Alpha(density(mask lattice))) > fast_color_thres (FourierGrid_model.py:441-456,
+        dcvgo.py:214-226, dvgo.py:236-246, dmpigo.py:174-187: DirectMPIGO's shift is 0, without its act_shift grid, as there).
+        Two kernels: ops.lattice_alpha generates the lattice points in registers; ops.maxpool3_gt_and_ pools, thresholds and
+        ANDs (4 B + 1 B per cell)."""
+        from . import ops
+        mn, mx = self.density._bounds()
+        alpha = ops.lattice_alpha(self.density.grid.data, mn, mx, self.density.num_freqs, self.xyz_min.tolist(),
+                                  self.xyz_max.tolist(), self.mask_cache.mask.shape, host_scalar(self._density_shift()),
+                                  float(self._voxel_size_ratio()))
+        ops.maxpool3_gt_and_(self.mask_cache.mask, alpha, self.fast_color_thres)
+
+    @torch.no_grad()
+    def _rebuild_mask_cache(self, world_size, density):
+        """After a rescale: mask(lattice) & (max_pool3d(alpha(density)) > fast_color_thres) on the new lattice."""
+        xyz = self._mask_lattice(world_size)
+        alpha = F.max_pool3d(self.activate_density(density.contiguous()), kernel_size=3, padding=1, stride=1)[0, 0]
+        self._set_mask_cache(self.mask_cache(xyz) & (alpha > self.fast_color_thres))
+
+
+class _CoarseGeo:
+    """hit_coarse_geo, for the models whose reference has it (FourierGridModel, DirectVoxGO)."""
+
+    def hit_coarse_geo(self, rays_o, rays_d, near, far, stepsize, **render_kwargs):
+        """FourierGrid_model.py:495-507, dvgo.py:292-304: does a ray hit the occupancy mask?"""
+        from . import ops
+        shape = rays_o.shape[:-1]
+        rays_o = rays_o.reshape(-1, 3).contiguous()
+        rays_d = rays_d.reshape(-1, 3).contiguous()
+        ray_pts, mask_outbbox, ray_id = ops.sample_pts_on_rays(rays_o, rays_d, self.xyz_min, self.xyz_max, near, 1e9,
+                                                               stepsize * float(self._voxel_size()))[:3]
+        mask_inbbox = ~mask_outbbox
+        hit = torch.zeros([len(rays_o)], dtype=torch.bool, device=rays_o.device)
+        hit[ray_id[mask_inbbox][self.mask_cache(ray_pts[mask_inbbox])]] = 1
+        return hit.reshape(shape)
+
+
+class _ContractedBase(_GridModel):
+    """Shared machinery of the two contracted-space models."""
+
+    T_BOUNDARY = 2.0          # dcvgo.py:243-244; FourierGridModel overrides with 1.5
+    USE_CUMDIST = False
+    USE_MASKCACHE = False
+    _HOST_BUFFERS = ('scene_center', 'scene_radius')
+
+    # ---- helpers --------------------------------------------------------------------------------
     def _init_scene(self, xyz_min, xyz_max, bg_len, fast_color_thres, contracted_norm):
         xyz_min = torch.as_tensor(np.asarray(xyz_min), dtype=torch.float32)
         xyz_max = torch.as_tensor(np.asarray(xyz_max), dtype=torch.float32)
@@ -81,16 +186,10 @@ class _ContractedBase(nn.Module):
             self.fast_color_thres = fast_color_thres
         self.bg_len = bg_len
         self.contracted_norm = contracted_norm
-        self._host_cache = None
 
     def _maybe_update_thres(self, global_step):
         if isinstance(self._fast_color_thres, dict) and global_step in self._fast_color_thres:
             self.fast_color_thres = self._fast_color_thres[global_step]
-
-    def activate_density(self, density, interval=None):
-        interval = interval if interval is not None else self._voxel_size_ratio()
-        shape = density.shape
-        return Raw2Alpha.apply(density.flatten().contiguous(), self.act_shift, interval).reshape(shape)
 
     def _sample_dense(self, ori_rays_o, ori_rays_d, stepsize):
         """Dense [N,S,3] contracted points with torch elementwise ops (dcvgo.py:239-262,
@@ -123,18 +222,13 @@ class _ContractedBase(nn.Module):
         dev = rays_o.device
         t_table = march.t_schedule(self._world_len(), stepsize, self.bg_len, self.T_BOUNDARY, dev)
         interval = stepsize * float(self._voxel_size_ratio())
-        host = self._host()
+        center, radius = self._host()
+        mscale, mshift = self._mask_geometry()
         mask = self.mask_cache.mask if self.USE_MASKCACHE else None
         cum = None
         if self.USE_CUMDIST:
             cum = (2 + 2 * self.bg_len) / self._world_len() * stepsize * 0.95
-        mscale = mshift = None
-        if mask is not None:
-            if getattr(self, '_mask_host', None) is None or self._mask_host[0] is not self.mask_cache:
-                self._mask_host = (self.mask_cache, self.mask_cache.xyz2ijk_scale.cpu().tolist(),
-                                   self.mask_cache.xyz2ijk_shift.cpu().tolist())
-            mscale, mshift = self._mask_host[1], self._mask_host[2]
-        cfg = march.make_cfg(host['center'], host['radius'], self.bg_len, self.contracted_norm, t_table.numel(),
+        cfg = march.make_cfg(center, radius, self.bg_len, self.contracted_norm, t_table.numel(),
                              host_scalar(self.act_shift), interval, self.fast_color_thres,
                              cumdist_thres=cum, mask=mask, mask_scale=mscale, mask_shift=mshift)
         dmn, dmx = self.density._bounds()
@@ -146,46 +240,9 @@ class _ContractedBase(nn.Module):
                                 dense_known, coherent)
         return out, t_table
 
-    def _shade(self, k0, viewdirs, ray_id):
-        if self.rgbnet is None:
-            return torch.sigmoid(k0)
-        emb = _view_embed(viewdirs, self.viewfreq).flatten(0, -2)
-        if shade_mod.supported(self.rgbnet, k0.shape[-1]):
-            return shade_mod.shade(self.rgbnet, k0, emb, ray_id)          # fused on-chip MLP (csrc/shade.cu)
-        return torch.sigmoid(self.rgbnet(torch.cat([k0, emb[ray_id]], -1)))   # other widths / depths: torch (cuBLAS)
-
-    def density_total_variation_add_grad(self, weight, dense_mode):
-        w = weight * self._tv_world_max(self.density) / 128
-        self.density.total_variation_add_grad(w, w, w, dense_mode)
-
-    def k0_total_variation_add_grad(self, weight, dense_mode):
-        w = weight * self._tv_world_max(self.k0) / 128
-        self.k0.total_variation_add_grad(w, w, w, dense_mode)
-
-    def tv_terms(self, weight_density=0., weight_k0=0., dense_mode=True):
-        """{grid parameter: (wx, wy, wz, dense_mode)} with the weights of the two methods above -- the form
-        dist.reduce_tv_step consumes to pipeline all-reduce / TV / Adam slab by slab."""
-        out = {}
-        for grid, weight in ((self.density, weight_density), (self.k0, weight_k0)):
-            if weight > 0:
-                w = weight * self._tv_world_max(grid) / 128
-                out[grid.grid] = (w, w, w, dense_mode)
-        return out
-
-    @staticmethod
-    def _tv_world_max(g):
-        return float(max(g.grid.shape[2:]))
-
-
-@torch.no_grad()
-def _occupancy_update(model, density, mask_cache, interval):
-    """mask &= max_pool3d(Raw2Alpha(density(lattice of the mask grid))) > fast_color_thres  (two launches, 4 B + 1 B per cell)."""
-    from . import ops
-    from .functional import host_scalar
-    mn, mx = density._bounds()
-    alpha = ops.lattice_alpha(density.grid.data, mn, mx, density.num_freqs, model.xyz_min.tolist(), model.xyz_max.tolist(),
-                              mask_cache.mask.shape, host_scalar(model.act_shift), interval)
-    ops.maxpool3_gt_and_(mask_cache.mask, alpha, model.fast_color_thres)
+    def _tv_weights(self, grid, weight, dense_mode):
+        w = weight * float(max(grid.grid.shape[2:])) / 128         # each grid's own largest dimension
+        return (w, w, w, dense_mode)
 
 
 @torch.no_grad()
@@ -196,15 +253,7 @@ def _scale_dense_model(model, num_voxels):
     model.density.scale_volume_grid(model.world_size)
     model.k0.scale_volume_grid(model.world_size)
     if np.prod(model.world_size.tolist()) <= 256 ** 3:
-        dev = model.density.grid.device
-        ws = [int(v) for v in model.world_size]
-        axes = [torch.linspace(float(model.xyz_min[a]), float(model.xyz_max[a]), ws[a], device=dev) for a in range(3)]
-        xyz = torch.stack(torch.meshgrid(*axes, indexing='ij'), -1)
-        alpha = F.max_pool3d(model.activate_density(model.density.get_dense_grid().contiguous()), kernel_size=3,
-                             padding=1, stride=1)[0, 0]
-        model.mask_cache = G.MaskGrid(path=None, mask=model.mask_cache(xyz) & (alpha > model.fast_color_thres),
-                                      xyz_min=model.xyz_min, xyz_max=model.xyz_max).to(dev)
-        model._mask_host = None
+        model._rebuild_mask_cache(model.world_size, model.density.get_dense_grid())
 
 
 @torch.no_grad()
@@ -234,7 +283,7 @@ def _count_views(density, world_size, voxel_size, rays_o_tr, rays_d_tr, imsz, ne
 
 
 # ======================================================================================================
-class FourierGridModel(_ContractedBase):
+class FourierGridModel(_CoarseGeo, _ContractedBase):
     """FourierGrid/FourierGrid_model.py:134-681."""
 
     T_BOUNDARY = 1.5          # FourierGrid_model.py:526
@@ -277,8 +326,7 @@ class FourierGridModel(_ContractedBase):
             self.k0 = G.FourierGrid(channels=rgbnet_dim, world_size=self.world_size_rgb, xyz_min=self.xyz_min,
                                     xyz_max=self.xyz_max, use_nerf_pos=True, fourier_freq_num=fourier_freq_num,
                                     config=k0_config)
-            self.register_buffer('viewfreq', torch.FloatTensor([(2 ** i) for i in range(viewbase_pe)]))
-            self.rgbnet = _make_rgbnet(3 + 3 * viewbase_pe * 2 + rgbnet_dim, rgbnet_width, rgbnet_depth)
+            self._add_rgbnet(rgbnet_dim, viewbase_pe, rgbnet_width, rgbnet_depth)
         self.vd = None      # view-direction grid variant (num_voxels_viewdir > 0) is not on the benchmarked path
         if num_voxels_viewdir is not None and num_voxels_viewdir > 0:
             raise NotImplementedError('num_voxels_viewdir > 0 (view-direction grid) is outside the hot-path scope')
@@ -300,6 +348,9 @@ class FourierGridModel(_ContractedBase):
 
     def _world_len(self):
         return self.world_len_density
+
+    def _voxel_size(self):
+        return self.voxel_size_density
 
     def _voxel_size_ratio(self):
         return self.voxel_size_ratio_density
@@ -325,24 +376,7 @@ class FourierGridModel(_ContractedBase):
         self.k0.scale_volume_grid(self.world_size_rgb)
         self.world_size = self.world_size_density
         if np.prod(self.world_size_density.tolist()) <= 256 ** 3:
-            self._rebuild_mask_cache(self.world_size_density)
-
-    @torch.no_grad()
-    def _rebuild_mask_cache(self, world_size):
-        dev = self.density.grid.device
-        ws = [int(v) for v in world_size]
-        axes = [torch.linspace(float(self.xyz_min[a]), float(self.xyz_max[a]), ws[a], device=dev) for a in range(3)]
-        xyz = torch.stack(torch.meshgrid(*axes, indexing='ij'), -1)
-        dense = self.density.get_dense_grid()
-        alpha = F.max_pool3d(self.activate_density(dense.contiguous()), kernel_size=3, padding=1, stride=1)[0, 0]
-        self.mask_cache = G.MaskGrid(path=None, mask=self.mask_cache(xyz) & (alpha > self.fast_color_thres),
-                                     xyz_min=self.xyz_min, xyz_max=self.xyz_max).to(dev)
-
-    @torch.no_grad()
-    def update_occupancy_cache(self):
-        """FourierGrid_model.py:441-456: mask_cache.mask &= max_pool3d(alpha(density(mask lattice))) > fast_color_thres, as two
-        kernels (ops.lattice_alpha generates the lattice points in registers; ops.maxpool3_gt_and_ pools, thresholds and ANDs)."""
-        _occupancy_update(self, self.density, self.mask_cache, float(self.voxel_size_ratio_density))
+            self._rebuild_mask_cache(self.world_size_density, self.density.get_dense_grid())
 
     @torch.no_grad()
     def maskout_near_cam_vox(self, cam_o, near_clip):
@@ -364,19 +398,6 @@ class FourierGridModel(_ContractedBase):
         return _count_views(self.density, self.world_size_density, self.voxel_size_density, rays_o_tr, rays_d_tr, imsz, near,
                             stepsize, downrate, irregular_shape)
 
-    def hit_coarse_geo(self, rays_o, rays_d, near, far, stepsize, **render_kwargs):
-        """FourierGrid_model.py:495-507: does a ray hit the occupancy mask?"""
-        from . import ops
-        shape = rays_o.shape[:-1]
-        rays_o = rays_o.reshape(-1, 3).contiguous()
-        rays_d = rays_d.reshape(-1, 3).contiguous()
-        ray_pts, mask_outbbox, ray_id = ops.sample_pts_on_rays(rays_o, rays_d, self.xyz_min, self.xyz_max, near, 1e9,
-                                                               stepsize * float(self.voxel_size_density))[:3]
-        mask_inbbox = ~mask_outbbox
-        hit = torch.zeros([len(rays_o)], dtype=torch.bool, device=rays_o.device)
-        hit[ray_id[mask_inbbox][self.mask_cache(ray_pts[mask_inbbox])]] = 1
-        return hit.reshape(shape)
-
     def sample_ray(self, ori_rays_o, ori_rays_d, stepsize, is_train=False, **render_kwargs):
         """FourierGrid_model.py:509-552 return tuple (ray_pts, indexs, inner_mask, t, rays_d_extend)."""
         ray_pts, inner_mask, t = self._sample_dense(ori_rays_o, ori_rays_d, stepsize)
@@ -391,17 +412,7 @@ class FourierGridModel(_ContractedBase):
         (weights, alphainv_last, alpha, density, k0, ray_id, step_id, t, inner), t_table = self._march(
             rays_o, rays_d, render_kwargs['stepsize'])
         rgb = self._shade(k0, viewdirs, ray_id)
-        rgb_marched = composite_rgb(weights, rgb, ray_id, N)
-        if render_kwargs.get('rand_bkgd', False):
-            rgb_marched = rgb_marched + alphainv_last.unsqueeze(-1) * torch.rand_like(rgb_marched)
-        s = 1 - 1 / (1 + t)
-        ret = {'alphainv_last': alphainv_last, 'weights': weights, 'rgb_marched': rgb_marched, 'raw_density': density,
-               'raw_alpha': alpha, 'raw_rgb': rgb, 'ray_id': ray_id, 'step_id': step_id, 'n_max': t_table.numel(),
-               't': t, 's': s}
-        if render_kwargs.get('render_depth', False):
-            with torch.no_grad():
-                ret['depth'] = segment_sum(weights * s, ray_id, N)
-        return ret
+        return self._finish(N, weights, alphainv_last, density, alpha, rgb, ray_id, step_id, t, t_table.numel(), render_kwargs)
 
     def forward_ops(self, rays_o, rays_d, viewdirs, global_step=None, is_train=False, **render_kwargs):
         """Op-by-op composition in the reference's order (FourierGrid_model.py:566-672)."""
@@ -433,8 +444,11 @@ class FourierGridModel(_ContractedBase):
             t, density, alpha = t.reshape(-1), density.reshape(-1), alpha.reshape(-1)
         k0 = self.k0(ray_pts)
         rgb = self._shade(k0, viewdirs, ray_id)
+        return self._finish(N, weights, alphainv_last, density, alpha, rgb, ray_id, step_id, t, n_max, render_kwargs)
+
+    def _finish(self, N, weights, alphainv_last, density, alpha, rgb, ray_id, step_id, t, n_max, render_kwargs):
         rgb_marched = composite_rgb(weights, rgb, ray_id, N)
-        if render_kwargs.get('rand_bkgd', False):
+        if render_kwargs.get('rand_bkgd', False):           # FourierGrid_model.py:646: a random background only, never bg
             rgb_marched = rgb_marched + alphainv_last.unsqueeze(-1) * torch.rand_like(rgb_marched)
         s = 1 - 1 / (1 + t)
         ret = {'alphainv_last': alphainv_last, 'weights': weights, 'rgb_marched': rgb_marched, 'raw_density': density,
@@ -476,8 +490,7 @@ class DirectContractedVoxGO(_ContractedBase):
             self.rgbnet = None
         else:
             self.k0_dim = rgbnet_dim
-            self.register_buffer('viewfreq', torch.FloatTensor([(2 ** i) for i in range(viewbase_pe)]))
-            self.rgbnet = _make_rgbnet(3 + 3 * viewbase_pe * 2 + rgbnet_dim, rgbnet_width, rgbnet_depth)
+            self._add_rgbnet(rgbnet_dim, viewbase_pe, rgbnet_width, rgbnet_depth)
         self.k0 = G.DenseGrid(channels=self.k0_dim, world_size=self.world_size, xyz_min=self.xyz_min, xyz_max=self.xyz_max)
         if mask_cache_world_size is None:
             mask_cache_world_size = self.world_size
@@ -494,9 +507,6 @@ class DirectContractedVoxGO(_ContractedBase):
     def _world_len(self):
         return self.world_len
 
-    def _voxel_size_ratio(self):
-        return self.voxel_size_ratio
-
     def get_kwargs(self):
         return {
             'xyz_min': self.xyz_min.cpu().numpy(), 'xyz_max': self.xyz_max.cpu().numpy(),
@@ -509,12 +519,6 @@ class DirectContractedVoxGO(_ContractedBase):
 
     def scale_volume_grid(self, num_voxels):
         _scale_dense_model(self, num_voxels)
-
-    @torch.no_grad()
-    def update_occupancy_cache(self):
-        """dcvgo.py:214-226 (same composition as FourierGrid_model.py:441-456)."""
-        _occupancy_update(self, self.density, self.mask_cache, float(self.voxel_size_ratio))
-        self._mask_host = None
 
     def sample_ray(self, ori_rays_o, ori_rays_d, stepsize, is_train=False, **render_kwargs):
         """dcvgo.py:228-262 return tuple (ray_pts, inner_mask, t)."""
@@ -589,7 +593,7 @@ class DirectContractedVoxGO(_ContractedBase):
 
 
 # ======================================================================================================
-class DirectVoxGO(nn.Module):
+class DirectVoxGO(_CoarseGeo, _GridModel):
     """Bounded-scene model (FourierGrid/dvgo.py:26-425): ragged AABB sampling (sample_pts_on_rays) instead of the contracted
     schedule; depth = sum w * step_id.  ``forward`` runs the fused box march (march.BoxMarch: pass A, scan, pass B; one host read
     of the survivor count) with the rgb from ``_shade`` -- the tensor-core rgbnet when shade.supported (the default fine config:
@@ -628,15 +632,12 @@ class DirectVoxGO(nn.Module):
             self.k0_dim, self.rgbnet = 3, None
         else:
             self.k0_dim = rgbnet_dim
-            self.register_buffer('viewfreq', torch.FloatTensor([(2 ** i) for i in range(viewbase_pe)]))
-            dim0 = 3 + 3 * viewbase_pe * 2 + (rgbnet_dim if rgbnet_direct else rgbnet_dim - 3)
-            self.rgbnet = _make_rgbnet(dim0, rgbnet_width, rgbnet_depth)
+            self._add_rgbnet(rgbnet_dim if rgbnet_direct else rgbnet_dim - 3, viewbase_pe, rgbnet_width, rgbnet_depth)
         self.k0 = G.DenseGrid(channels=self.k0_dim, world_size=self.world_size, xyz_min=self.xyz_min, xyz_max=self.xyz_max)
         self.mask_cache_path, self.mask_cache_thres = mask_cache_path, mask_cache_thres
         if mask_cache_world_size is None:
             mask_cache_world_size = self.world_size
         self._pending_mask = None
-        self._mask_host = None
         self.mask_cache = G.MaskGrid(path=None, mask=torch.ones([int(v) for v in mask_cache_world_size], dtype=torch.bool),
                                      xyz_min=self.xyz_min, xyz_max=self.xyz_max)
         if mask_cache_path:
@@ -648,33 +649,20 @@ class DirectVoxGO(nn.Module):
     @torch.no_grad()
     def _resolve_mask_cache(self):
         path, thres, ws = self._pending_mask
-        dev = self.xyz_min.device
-        coarse = G.MaskGrid(path=path, mask_cache_thres=thres).to(dev)
-        axes = [torch.linspace(float(self.xyz_min[a]), float(self.xyz_max[a]), ws[a], device=dev) for a in range(3)]
-        xyz = torch.stack(torch.meshgrid(*axes, indexing='ij'), -1)
-        self.mask_cache = G.MaskGrid(path=None, mask=coarse(xyz), xyz_min=self.xyz_min, xyz_max=self.xyz_max).to(dev)
+        coarse = G.MaskGrid(path=path, mask_cache_thres=thres).to(self.xyz_min.device)
+        self._set_mask_cache(coarse(self._mask_lattice(ws)))
         self._pending_mask = None
-        self._mask_host = None
 
     def _apply(self, fn, *a, **k):
-        self._mask_host = None
         out = super()._apply(fn, *a, **k)
         if self._pending_mask is not None and self.xyz_min.is_cuda:
             self._resolve_mask_cache()
         return out
 
     def _load_from_state_dict(self, state_dict, prefix, *a, **k):
-        self._mask_host = None
         if prefix + 'mask_cache.mask' in state_dict:
             self._pending_mask = None
         return super()._load_from_state_dict(state_dict, prefix, *a, **k)
-
-    def _mask_geometry(self):
-        if self._mask_host is None or self._mask_host[0] is not self.mask_cache:
-            self._mask_host = (self.mask_cache, self.mask_cache.xyz2ijk_scale.cpu().tolist(),
-                               self.mask_cache.xyz2ijk_shift.cpu().tolist(), self.xyz_min.cpu().tolist(),
-                               self.xyz_max.cpu().tolist())
-        return self._mask_host[1:]
 
     def _set_grid_resolution(self, num_voxels):
         self.num_voxels = num_voxels
@@ -697,12 +685,6 @@ class DirectVoxGO(nn.Module):
         """dvgo.py:213-234 (the pg_scale steps of the fine stage)."""
         _scale_dense_model(self, num_voxels)
 
-    @torch.no_grad()
-    def update_occupancy_cache(self):
-        """dvgo.py:236-246: mask &= max_pool3d(Raw2Alpha(density(mask lattice))) > fast_color_thres (ops.lattice_alpha +
-        ops.maxpool3_gt_and_)."""
-        _occupancy_update(self, self.density, self.mask_cache, float(self.voxel_size_ratio))
-
     def voxel_count_views(self, rays_o_tr, rays_d_tr, imsz, near, far, stepsize, downrate=1, irregular_shape=False):
         """dvgo.py:248-277 (see _count_views): feeds MaskedAdam.set_pervoxel_lr and the coarse stage's mask update."""
         return _count_views(self.density, self.world_size, self.voxel_size, rays_o_tr, rays_d_tr, imsz, near, stepsize, downrate,
@@ -717,27 +699,9 @@ class DirectVoxGO(nn.Module):
         cams = cam_o.to(self.density.grid.device).reshape(-1, 3)
         ops.maskout_near_cam_(self.density.grid.data[0][0], cams, near_clip, -100.0, lattice=(lo, hi))
 
-    def activate_density(self, density, interval=None):
-        interval = interval if interval is not None else self.voxel_size_ratio
-        shape = density.shape
-        return Raw2Alpha.apply(density.flatten().contiguous(), self.act_shift, interval).reshape(shape)
-
-    def density_total_variation_add_grad(self, weight, dense_mode):
-        w = weight * float(self.world_size.max()) / 128
-        self.density.total_variation_add_grad(w, w, w, dense_mode)
-
-    def k0_total_variation_add_grad(self, weight, dense_mode):
-        w = weight * float(self.world_size.max()) / 128
-        self.k0.total_variation_add_grad(w, w, w, dense_mode)
-
-    def tv_terms(self, weight_density=0., weight_k0=0., dense_mode=True):
-        """{grid parameter: (wx, wy, wz, dense_mode)} for dist.reduce_tv_step (same weights as the two methods above)."""
-        out = {}
-        for grid, weight in ((self.density, weight_density), (self.k0, weight_k0)):
-            if weight > 0:
-                w = weight * float(self.world_size.max()) / 128
-                out[grid.grid] = (w, w, w, dense_mode)
-        return out
+    def _tv_weights(self, grid, weight, dense_mode):
+        w = weight * float(self.world_size.max()) / 128          # dvgo.py: the model's world size, for both grids
+        return (w, w, w, dense_mode)
 
     def sample_ray(self, rays_o, rays_d, near, far, stepsize, **render_kwargs):
         """dvgo.py:306-328."""
@@ -749,19 +713,6 @@ class DirectVoxGO(nn.Module):
         mask_inbbox = ~mask_outbbox
         return ray_pts[mask_inbbox], ray_id[mask_inbbox], step_id[mask_inbbox]
 
-    def hit_coarse_geo(self, rays_o, rays_d, near, far, stepsize, **render_kwargs):
-        """dvgo.py:292-304."""
-        from . import ops
-        shape = rays_o.shape[:-1]
-        rays_o = rays_o.reshape(-1, 3).contiguous()
-        rays_d = rays_d.reshape(-1, 3).contiguous()
-        ray_pts, mask_outbbox, ray_id = ops.sample_pts_on_rays(rays_o, rays_d, self.xyz_min, self.xyz_max, near, 1e9,
-                                                               stepsize * float(self.voxel_size))[:3]
-        mask_inbbox = ~mask_outbbox
-        hit = torch.zeros([len(rays_o)], dtype=torch.bool, device=rays_o.device)
-        hit[ray_id[mask_inbbox][self.mask_cache(ray_pts[mask_inbbox])]] = 1
-        return hit.reshape(shape)
-
     # ---- rendering ------------------------------------------------------------------------------------------------------------
     def _stepdist(self, stepsize):
         # what sample_ray hands ubn_sample_pts_* (the same fp32 value reaches the march); host_scalar caches the read per tensor,
@@ -771,10 +722,12 @@ class DirectVoxGO(nn.Module):
     def _fused_ok(self, stepsize):
         if not march.box_supported(self.density.grid, self.k0.grid):
             return False
-        _, _, lo, hi = self._mask_geometry()
+        lo, hi = self._host()
         return march.box_s_max(lo, hi, self._stepdist(stepsize)) <= march.BOX_S_MAX_LIMIT
 
-    _shade = _ContractedBase._shade        # sigmoid(k0), or the rgbnet on cat[k0, view embedding] (tensor cores when supported)
+    def _mask_geometry(self):
+        """(mask_scale, mask_shift, xyz_min, xyz_max) as host lists: all the box march cfg takes by value."""
+        return (*super()._mask_geometry(), *self._host())
 
     def forward(self, rays_o, rays_d, viewdirs, global_step=None, **render_kwargs):
         """dvgo.py:330-397 on the fused box march (see the class docstring); same keys as the reference's ret_dict."""
@@ -798,14 +751,7 @@ class DirectVoxGO(nn.Module):
         else:
             emb = _view_embed(viewdirs, self.viewfreq).flatten(0, -2)[ray_id]
             rgb = torch.sigmoid(self.rgbnet(torch.cat([k0[:, 3:], emb], -1)) + k0[:, :3])
-        rgb_marched = composite_rgb(weights, rgb, ray_id, N)
-        rgb_marched = rgb_marched + alphainv_last.unsqueeze(-1) * render_kwargs['bg']
-        ret = {'alphainv_last': alphainv_last, 'weights': weights, 'rgb_marched': rgb_marched, 'raw_alpha': alpha,
-               'raw_rgb': rgb, 'ray_id': ray_id}
-        if render_kwargs.get('render_depth', False):
-            with torch.no_grad():
-                ret['depth'] = segment_sum(weights * step_id, ray_id, N)
-        return ret
+        return self._finish(N, weights, alphainv_last, alpha, rgb, ray_id, step_id, render_kwargs)
 
     def forward_ops(self, rays_o, rays_d, viewdirs, global_step=None, **render_kwargs):
         """Op-by-op composition in the reference's order (dvgo.py:330-397): ragged sample_pts_on_rays, boolean-mask compactions,
@@ -834,8 +780,11 @@ class DirectVoxGO(nn.Module):
             emb = _view_embed(viewdirs, self.viewfreq).flatten(0, -2)[ray_id]
             logit = self.rgbnet(torch.cat([k0_view, emb], -1))
             rgb = torch.sigmoid(logit if self.rgbnet_direct else logit + k0[:, :3])
+        return self._finish(N, weights, alphainv_last, alpha, rgb, ray_id, step_id, render_kwargs)
+
+    def _finish(self, N, weights, alphainv_last, alpha, rgb, ray_id, step_id, render_kwargs):
         rgb_marched = composite_rgb(weights, rgb, ray_id, N)
-        rgb_marched = rgb_marched + alphainv_last.unsqueeze(-1) * render_kwargs['bg']
+        rgb_marched = rgb_marched + alphainv_last.unsqueeze(-1) * render_kwargs['bg']       # dvgo.py:406: always bg
         ret = {'alphainv_last': alphainv_last, 'weights': weights, 'rgb_marched': rgb_marched, 'raw_alpha': alpha,
                'raw_rgb': rgb, 'ray_id': ray_id}
         if render_kwargs.get('render_depth', False):
@@ -845,7 +794,7 @@ class DirectVoxGO(nn.Module):
 
 
 # ======================================================================================================
-class DirectMPIGO(nn.Module):
+class DirectMPIGO(_GridModel):
     """Forward-facing model in NDC space (FourierGrid/dmpigo.py:18-340): a DenseGrid density with a frozen per-plane bias
     ``act_shift`` ([1,1,1,1,mpi_depth] DenseGrid), a DenseGrid k0 (3 channels, or rgbnet_dim features + rgbnet), a mask cache,
     NDC samples o + d * i/(S-1) inside the bbox.  ``forward`` runs the fused NDC march (march.NdcMarch); ``forward_ops``
@@ -882,8 +831,7 @@ class DirectMPIGO(nn.Module):
         else:
             self.k0_dim = rgbnet_dim
             self.k0 = G.DenseGrid(channels=rgbnet_dim, world_size=self.world_size, xyz_min=self.xyz_min, xyz_max=self.xyz_max)
-            self.register_buffer('viewfreq', torch.FloatTensor([(2 ** i) for i in range(viewbase_pe)]))
-            self.rgbnet = _make_rgbnet(3 + 3 * viewbase_pe * 2 + rgbnet_dim, rgbnet_width, rgbnet_depth)
+            self._add_rgbnet(rgbnet_dim, viewbase_pe, rgbnet_width, rgbnet_depth)
         self.mask_cache_path, self.mask_cache_thres = mask_cache_path, mask_cache_thres
         if mask_cache_world_size is None:
             mask_cache_world_size = self.world_size
@@ -892,8 +840,6 @@ class DirectMPIGO(nn.Module):
                                       'and assign model.mask_cache instead')
         self.mask_cache = G.MaskGrid(path=None, mask=torch.ones([int(v) for v in mask_cache_world_size], dtype=torch.bool),
                                      xyz_min=self.xyz_min, xyz_max=self.xyz_max)
-        self._host_cache = None
-        self._mask_host = None
 
     def _set_grid_resolution(self, num_voxels, mpi_depth):
         """dmpigo.py:120-130: X, Y from the voxel budget per plane (fp32 sqrt, truncated to long), Z = mpi_depth."""
@@ -915,26 +861,6 @@ class DirectMPIGO(nn.Module):
             'density_config': self.density_config, 'k0_config': self.k0_config, **self.rgbnet_kwargs,
         }
 
-    # ---- host-side caches (bbox and mask-cache geometry go to the kernels by value) ----------------------------------------
-    def _apply(self, fn, *a, **k):
-        self._host_cache = self._mask_host = None
-        return super()._apply(fn, *a, **k)
-
-    def _load_from_state_dict(self, *a, **k):
-        self._host_cache = self._mask_host = None
-        return super()._load_from_state_dict(*a, **k)
-
-    def _host(self):
-        if self._host_cache is None:
-            self._host_cache = (self.xyz_min.detach().cpu().tolist(), self.xyz_max.detach().cpu().tolist())
-        return self._host_cache
-
-    def _mask_geometry(self):
-        if self._mask_host is None or self._mask_host[0] is not self.mask_cache:
-            self._mask_host = (self.mask_cache, self.mask_cache.xyz2ijk_scale.cpu().tolist(),
-                               self.mask_cache.xyz2ijk_shift.cpu().tolist())
-        return self._mask_host[1], self._mask_host[2]
-
     # ---- grid maintenance -----------------------------------------------------------------------------------------------
     @torch.no_grad()
     def scale_volume_grid(self, num_voxels, mpi_depth):
@@ -943,25 +869,7 @@ class DirectMPIGO(nn.Module):
         self.density.scale_volume_grid(self.world_size)
         self.k0.scale_volume_grid(self.world_size)
         if np.prod(self.world_size.tolist()) <= 256 ** 3:
-            dev = self.density.grid.device
-            ws = [int(v) for v in self.world_size]
-            axes = [torch.linspace(float(self.xyz_min[a]), float(self.xyz_max[a]), ws[a], device=dev) for a in range(3)]
-            xyz = torch.stack(torch.meshgrid(*axes, indexing='ij'), -1)
-            dens = (self.density.get_dense_grid() + self.act_shift.grid).contiguous()
-            alpha = F.max_pool3d(self.activate_density(dens), kernel_size=3, padding=1, stride=1)[0, 0]
-            self.mask_cache = G.MaskGrid(path=None, mask=self.mask_cache(xyz) & (alpha > self.fast_color_thres),
-                                         xyz_min=self.xyz_min, xyz_max=self.xyz_max).to(dev)
-
-    @torch.no_grad()
-    def update_occupancy_cache(self):
-        """dmpigo.py:174-187: mask &= max_pool3d(Raw2Alpha(density(lattice), shift 0)) > fast_color_thres -- WITHOUT act_shift,
-        as the reference does (two launches: ops.lattice_alpha, ops.maxpool3_gt_and_)."""
-        from . import ops
-        mn, mx = self.density._bounds()
-        lo, hi = self._host()
-        alpha = ops.lattice_alpha(self.density.grid.data, mn, mx, 0, lo, hi, self.mask_cache.mask.shape, 0.0,
-                                  float(self.voxel_size_ratio))
-        ops.maxpool3_gt_and_(self.mask_cache.mask, alpha, self.fast_color_thres)
+            self._rebuild_mask_cache(self.world_size, self.density.get_dense_grid() + self.act_shift.grid)
 
     @torch.no_grad()
     def update_occupancy_cache_lt_nviews(self, rays_o_tr, rays_d_tr, imsz, render_kwargs, maskout_lt_nviews):
@@ -979,31 +887,16 @@ class DirectMPIGO(nn.Module):
             count += (ones.grad > 1)
         self.mask_cache.mask &= (count >= maskout_lt_nviews)[0, 0]
 
-    def density_total_variation_add_grad(self, weight, dense_mode):
-        wxy, wxy_, wz, _ = self._tv_weights(weight, dense_mode)
-        self.density.total_variation_add_grad(wxy, wxy_, wz, dense_mode)
-
-    def k0_total_variation_add_grad(self, weight, dense_mode):
-        wxy, wxy_, wz, _ = self._tv_weights(weight, dense_mode)
-        self.k0.total_variation_add_grad(wxy, wxy_, wz, dense_mode)
-
-    def _tv_weights(self, weight, dense_mode):
+    def _tv_weights(self, grid, weight, dense_mode):
         """dmpigo.py:209-217: (wxy, wxy, wz) with wxy = weight * max(world_size[:2]) / 128 (an fp32 tensor expression there)
-        and wz = weight * mpi_depth / 128."""
+        and wz = weight * mpi_depth / 128, for both grids."""
         wxy = float(weight * self.world_size[:2].max() / 128)
         wz = weight * self.mpi_depth / 128
         return (wxy, wxy, wz, dense_mode)
 
-    def tv_terms(self, weight_density=0., weight_k0=0., dense_mode=True):
-        """{grid parameter: (wx, wy, wz, dense_mode)} for dist.reduce_tv_step (same weights as the two methods above)."""
-        return {grid.grid: self._tv_weights(weight, dense_mode)
-                for grid, weight in ((self.density, weight_density), (self.k0, weight_k0)) if weight > 0}
-
     # ---- rendering ------------------------------------------------------------------------------------------------------
-    def activate_density(self, density, interval=None):
-        interval = interval if interval is not None else self.voxel_size_ratio
-        shape = density.shape
-        return Raw2Alpha.apply(density.flatten().contiguous(), 0., interval).reshape(shape)
+    def _density_shift(self):
+        return 0.           # the act_shift grid is added to the density before the activation
 
     def _n_samples(self, stepsize):
         return int((self.mpi_depth - 1) / stepsize) + 1
@@ -1020,8 +913,6 @@ class DirectMPIGO(nn.Module):
         ray_id = torch.arange(mask_inbbox.shape[0], device=dev).view(-1, 1).expand_as(mask_inbbox)[mask_inbbox]
         step_id = torch.arange(mask_inbbox.shape[1], device=dev).view(1, -1).expand_as(mask_inbbox)[mask_inbbox]
         return ray_pts[mask_inbbox], ray_id, step_id, N_samples
-
-    _shade = _ContractedBase._shade        # sigmoid(k0), or the rgbnet on cat[k0, view embedding] (tensor cores at llff's 9 / 64)
 
     def _fused_ok(self):
         return march.ndc_supported(self.k0.grid) and self.density.grid.is_cuda
