@@ -551,6 +551,11 @@ int ubn_rgbnet_bwd_tc_fused_kw(int n_feat, int n_hidden, const float* feat, cons
                                const float* grad_rgb, int64_t n_pts, float* grad_feat, float* grad_view_bias, float* grad_W1k,
                                float* grad_W2, float* grad_b2, float* grad_W3, float* grad_b3, uint32_t* h2_mask_scratch,
                                const uint32_t* h1_mask, int single_pass, void* stream);
+/* Which kernel computes grad_W2 in the width-128 fused backward with panel saves (bit 2) and h2_mask_scratch: 1 (the default) =
+ * warpgroup MMA (wgmma) with a producer warpgroup staging H1 in shared memory; 0 = the mma.sync kernel.  Same products and the
+ * same per-chunk fp32 running sums, so the same results up to the tensor cores' accumulation order.  Process-wide like
+ * ubn_set_feature_kernel.  Returns cudaErrorInvalidValue for other values. */
+int ubn_set_dw2_engine(int engine);
 
 #if defined(__GNUC__)
 #pragma GCC visibility pop

@@ -18,9 +18,12 @@ Prints one JSON line:
 * max_err        -- every gradient (k0, W1, b1, W2, b2, W3, b3) at the timed size against an fp64 evaluation, as a fraction of
                     the largest element of the fp64 gradient (samples whose fp64 pre-activations come within 1e-5 of zero are
                     dropped for this check, as in tests/test_gpu_models.py);
+* dw2            -- with --dw2 mma,wgmma (width 128): the dW2 engines timed alternately in this one run, --rounds times each
+                    (a torch.profiler pass per round), with the rates of the fastest round and max_err for each engine;
 * gpu / power_limit_w -- where it ran, read in the same run.
 
     python scripts/bench_rgbnet.py [--shape truck|llff] [--iters 20] [--warmup 3] [--profile DIR] [--no-check]
+                                   [--dw2 mma,wgmma] [--rounds 3]
 """
 import argparse
 import json
@@ -41,6 +44,7 @@ LLFF_SURVIVORS = 412_419     # outputs.survivors of scripts/bench_mpi.py at its 
 HMMA_PER_SAMPLE = {'k_shade_fwd_tc': 864 / 16,      # layer 1 (2 k-steps) + layer 2 (16 k-steps), 16 column tiles, 3 passes
                    'k_shade_bwd_tc': 1120 / 16,     # dH1 768 + dX 96 + dW1k/view bias 96 + dW3 96 + E 64, per 16-sample unit
                    'k_shade_dw2_tc': 1536 / 32,     # 8 warps x 4 k-steps x 16 column tiles x 3 passes per 32-sample chunk
+                   'k_shade_dw2_wgmma': 1536 / 32,  # the same products as 2 warpgroups x 4 k-steps x 3 wgmma.m64n128k8
                    # width 64, 9 features
                    'k_shade_fwd_tc_w': 240 / 16,    # layer 1 (2 k-steps) + layer 2 (8 k-steps), 8 column tiles, 3 passes
                    'k_shade_bwd_tc_w': 368 / 16,    # dH1 192 + dX 48 + dW1k/view bias 48 + dW3 48 + E 32, per 16-sample unit
@@ -49,10 +53,13 @@ HMMA_PER_SAMPLE = {'k_shade_fwd_tc': 864 / 16,      # layer 1 (2 k-steps) + laye
 BYTES_PER_SAMPLE = {'k_shade_fwd_tc': 48 + 8 + 12 + 512 + 512 + 16,          # feat, ray_id, rgb, H1 + H2 saves, H1 masks
                     'k_shade_bwd_tc': 512 + 48 + 12 + 12 + 8 + 16 + 48 + 16,  # H2, feat, rgb, grad_rgb, ray_id, H1 masks; grad_feat, H2 masks
                     'k_shade_dw2_tc': 512 + 16 + 12 + 12,                     # H1, H2 masks, rgb, grad_rgb
+                    'k_shade_dw2_wgmma': 512 + 16 + 12 + 12,
                     'k_shade_fwd_tc_w': 36 + 8 + 12 + 256 + 256 + 8,          # the same at width 64 with 9 features
                     'k_shade_bwd_tc_w': 256 + 36 + 12 + 12 + 8 + 8 + 36 + 8,
                     'k_shade_dw2_tc_w': 256 + 8 + 12 + 12}
 # shape -> feature columns, hidden width, view-embedding columns, kernel-name suffix, default samples and rays
+# --dw2 engine name -> ubn_set_dw2_engine value and the kernel it runs at width 128
+DW2_ENGINES = {'mma': (0, 'k_shade_dw2_tc'), 'wgmma': (1, 'k_shade_dw2_wgmma')}
 SHAPES = {'truck': dict(K=12, W=128, E=27, sfx='', samples=4_194_304, rays=8192),
           'llff': dict(K=9, W=64, E=3, sfx='_w', samples=LLFF_SURVIVORS, rays=None)}
 
@@ -99,6 +106,24 @@ def _rates(name, ms, M):
                 hbm_gbs=round(byt / ms / 1e6, 1), share_of_hbm_datasheet=round(byt / ms * 1e3 / HBM_PEAK, 3))
 
 
+def _kernel_ms(shade, inputs, iters, names, trace=None):
+    """per-kernel mean device time (ms) over iters steps, from a torch.profiler pass of its own"""
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(iters):
+            _step(shade, *inputs)
+        torch.cuda.synchronize()
+    if trace:
+        prof.export_chrome_trace(trace)
+    kms = {}
+    for ev in prof.key_averages():
+        for kname in names:
+            if kname + '<' in ev.key:
+                t = getattr(ev, 'device_time_total', None) or getattr(ev, 'cuda_time_total', 0.0)
+                kms[kname] = kms.get(kname, 0.0) + t / 1e3 / iters
+    return kms
+
+
 def _check(shade, net, k0, emb, ray_id, gr, chunk=200_000):
     """max |grad - grad_fp64| / max |grad_fp64| for k0 and every parameter, at the full size, ReLU-ambiguous samples dropped"""
     from unboundednerfpytorch_b200 import models
@@ -136,6 +161,8 @@ def main():
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--profile', default=None, help='also run a torch.profiler pass and write its trace under this directory')
     ap.add_argument('--no-check', action='store_true')
+    ap.add_argument('--dw2', default=None, help='comma list of dW2 engines (mma, wgmma) to time alternately, width 128 only')
+    ap.add_argument('--rounds', type=int, default=3, help='rounds of the --dw2 alternation')
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit('bench_rgbnet.py needs a GPU')
@@ -147,7 +174,10 @@ def main():
     net, k0, emb, ray_id, gr = _inputs(M, args.rays or sh['rays'], sh['K'], sh['W'], sh['E'])
     assert shade.supported(net, sh['K'])
     k0.requires_grad_(True)
-    fwd_k, bwd_k, dw2_k = (f'k_shade_{n}_tc{sh["sfx"]}' for n in ('fwd', 'bwd', 'dw2'))
+    fwd_k, bwd_k = (f'k_shade_{n}_tc{sh["sfx"]}' for n in ('fwd', 'bwd'))
+    dw2_k = DW2_ENGINES['wgmma'][1] if sh['W'] == 128 else 'k_shade_dw2_tc_w'
+    engines = args.dw2.split(',') if args.dw2 else []
+    assert all(e in DW2_ENGINES for e in engines) and (not engines or sh['W'] == 128), '--dw2 takes mma / wgmma at width 128'
     res = dict(metric=f'rgbnet forward + backward, {args.shape} shape', gpu=name, power_limit_w=power, samples=M,
                rays=emb.shape[0], features=sh['K'], width=sh['W'], mode=shade.MODE, bwd_mode=shade.BWD_MODE)
     for _ in range(args.warmup):
@@ -165,22 +195,34 @@ def main():
     res['rates']['backward_pair'] = dict(ms=round(bwd, 3), tflops_hmma_equiv=round(pair_flop / bwd / 1e9, 1),
                                          share_of_tf32_datasheet=round(pair_flop / bwd / 1e9 / (TF32_PEAK / 1e12), 3))
     if args.profile:
-        from torch.profiler import ProfilerActivity, profile
         os.makedirs(args.profile, exist_ok=True)
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            for _ in range(args.iters):
-                _step(shade, net, k0, emb, ray_id, gr)
-            torch.cuda.synchronize()
-        prof.export_chrome_trace(os.path.join(args.profile, 'bench_rgbnet.pt.trace.json'))
-        kms = {}
-        for ev in prof.key_averages():
-            for kname in (fwd_k, bwd_k, dw2_k):
-                if kname + '<' in ev.key:
-                    t = getattr(ev, 'device_time_total', None) or getattr(ev, 'cuda_time_total', 0.0)
-                    kms[kname] = kms.get(kname, 0.0) + t / 1e3 / args.iters
+        kms = _kernel_ms(shade, (net, k0, emb, ray_id, gr), args.iters, (fwd_k, bwd_k, dw2_k),
+                         os.path.join(args.profile, 'bench_rgbnet.pt.trace.json'))
         res['kernels_ms'] = {k: round(v, 3) for k, v in kms.items()}
         for k, v in kms.items():
             res['rates'][k] = _rates(k, v, M)
+    if engines:
+        from unboundednerfpytorch_b200 import ops
+        runs = {e: [] for e in engines}
+        try:
+            for _ in range(args.rounds):
+                for e in engines:
+                    value, kname = DW2_ENGINES[e]
+                    ops.set_dw2_engine(value)
+                    for _ in range(args.warmup):
+                        _step(shade, net, k0, emb, ray_id, gr)
+                    torch.cuda.synchronize()
+                    runs[e].append(_kernel_ms(shade, (net, k0, emb, ray_id, gr), args.iters, (kname,))[kname])
+            res['dw2'] = {}
+            for e in engines:
+                value, kname = DW2_ENGINES[e]
+                res['dw2'][e] = dict(kernel=kname, ms_rounds=[round(v, 3) for v in runs[e]], **_rates(kname, min(runs[e]), M))
+                if not args.no_check:
+                    ops.set_dw2_engine(value)
+                    err, _ = _check(shade, net, k0.detach(), emb, ray_id, gr)
+                    res['dw2'][e]['max_err_of_scale'] = {k: float(f'{v:.3g}') for k, v in err.items()}
+        finally:
+            ops.set_dw2_engine(1)
     if not args.no_check:
         err, n = _check(shade, net, k0.detach(), emb, ray_id, gr)
         res['max_err_of_scale'] = {k: float(f'{v:.3g}') for k, v in err.items()}

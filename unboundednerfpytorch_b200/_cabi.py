@@ -77,6 +77,7 @@ _SIGNATURES = {
     'ubn_rgbnet_bwd_tc_fused_k': [c_int] + [c_p] * 9 + [c_i64] + [c_p] * 9 + [c_int, c_p],
     'ubn_rgbnet_fwd_tc_kw': [c_int, c_int] + [c_p] * 8 + [c_i64] + [c_p] * 4 + [c_int, c_p],
     'ubn_rgbnet_bwd_tc_fused_kw': [c_int, c_int] + [c_p] * 9 + [c_i64] + [c_p] * 9 + [c_int, c_p],
+    'ubn_set_dw2_engine': [c_int],
     'ubn_total_variation_add_grad': [c_p, c_p, c_f, c_f, c_f, c_i64, c_i64, c_i64, c_i64, c_i64, c_int, c_p],
     'ubn_adam_upd': [c_p, c_p, c_p, c_p, c_p, c_i64, c_int, c_f, c_f, c_f, c_f, c_int, c_p],
     'ubn_tv_adam_fused': [c_p, c_p, c_p, c_p, c_f, c_f, c_f, c_i64, c_i64, c_i64, c_i64, c_i64, c_int, c_int,

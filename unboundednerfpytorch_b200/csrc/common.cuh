@@ -31,6 +31,23 @@ __host__ __device__ __forceinline__ T ceil_div(T a, T b) { return (a + b - 1) / 
 // grid size for a plain elementwise kernel: one thread per element, capped only by int range
 inline unsigned blocks_for(int64_t n, int threads) { return (unsigned)((n + threads - 1) / threads); }
 
+// ---- shared-memory mbarriers (the TMA brick loads of render_tma.cu, the dW2 pipeline of shade_tc.cu) ------------------------
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra DONE_%=;\n\tbra WAIT_%=;\n\t"
+      "DONE_%=:\n\t}\n" ::"r"(bar),
+      "r"(parity)
+      : "memory");
+}
+
 // NDC sample i of n on a forward-facing ray (render_utils_kernel.cu:260-263): p = o + d * (i / (n - 1)), the step as an IEEE
 // float division and each coordinate as one fma, the form nvcc gives the reference's `o + d * dist`.  Shared by
 // ubn_sample_ndc_pts_on_rays and the fused NDC march, so both produce the same bits.

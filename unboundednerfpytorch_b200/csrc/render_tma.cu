@@ -36,20 +36,8 @@ constexpr uint32_t kBoxBytes = kBox * kBox * kBox * kChan * 4;   // 24 576
 constexpr int kWarps = 4;
 constexpr uint32_t kSmemBytes = kWarps * kBoxBytes + kWarps * 8 + 128;   // + mbarriers (+ slack for 128-byte alignment)
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra DONE_%=;\n\tbra WAIT_%=;\n\t"
-      "DONE_%=:\n\t}\n" ::"r"(bar),
-      "r"(parity)
-      : "memory");
 }
 // 4-D tiled TMA load: coordinates in tensor-map order (innermost first) = {channel, z, y, x}
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int c3) {

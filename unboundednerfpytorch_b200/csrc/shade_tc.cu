@@ -887,6 +887,239 @@ template <int kW, bool kThree, int kCtas, bool kPanel, bool kMask2>
 __global__ void __launch_bounds__(dw::kThreads, kCtas) k_shade_dw2_tc_w(UBN_SHADE_DW2_PARAMS) {
   shade_dw2_tc<kW, kThree, kPanel, kMask2>(UBN_SHADE_DW2_ARGS);
 }
+
+// ---- backward, launch 2 on warpgroup MMA (width 128, panel saves, H2 masks) ---------------------------------------------
+// The same split-K GEMM, chunks and numerical policy as shade_dw2_tc, on wgmma.m64n128k8 (TF32): B = H1 is read by the tensor
+// cores straight from shared memory, so no warp loads B fragments into registers.  One persistent CTA per SM, three warpgroups:
+//   * warpgroup 0 (producer) copies each 32-sample chunk into raw shared-memory slots with cp.async (kRaw - 1 chunks in
+//     flight, no registers held for them), then splits H1 into hi / lo and writes it transposed into two K-major
+//     [128 units][32 samples] tiles in the 128-byte-swizzle layout of the wgmma descriptor (TF32 wgmma takes K-major
+//     operands only; the panel save is unit-minor), plus the chunk's dz3 and H2 mask words, into a ring of kStages stages
+//     guarded by full / empty mbarriers;
+//   * warpgroups 1 and 2 (consumers) own dW2 rows 64 c .. 64 c + 63 each.  A = dZ2^T is rebuilt in registers from dz3, W3
+//     and the masks as shade_dw2_tc builds it, split into hi / lo, and every k-step issues the three mma3 products (al.Bh,
+//     ah.Bl, ah.Bh; ah.Bh alone at single_pass).  The accumulator restarts every chunk and is added into an fp32 running sum.
+namespace wg {
+constexpr int kThreads = 384;
+constexpr int kStages = 4;
+constexpr int kProducerRegs = 80, kConsumerRegs = 208;          // 128 * 80 + 256 * 208 <= 384 * 168 (launch allotment)
+constexpr uint32_t kTile = kHidden * dw::kK * 4;                // one [128][32] fp32 B tile: 16 KB
+constexpr uint32_t kExtra = 1024;                               // dz3 [3][32] and H2 mask words [4][32] (keeps 1 KB alignment)
+__host__ __device__ constexpr uint32_t stage_bytes(bool three) { return (three ? 2 : 1) * kTile + kExtra; }
+// the producer's raw slots: chunks still in flight from global memory (cp.async), kRaw - 1 ahead of the one it converts
+constexpr int kRaw = 3;
+constexpr uint32_t kRawH1 = 8 * 128 * 16;                       // float4 [8][128 threads]
+constexpr uint32_t kRawSlot = kRawH1 + 2 * 6 * 32 * 4;          // + rgb, grad_rgb (warp 0) and mask words (warp 1)
+__host__ __device__ constexpr uint32_t oRaw(bool three) { return kStages * stage_bytes(three); }
+__host__ __device__ constexpr uint32_t oBar(bool three) { return oRaw(three) + kRaw * kRawSlot; }
+// + full and empty barriers, + slack to align the base to the 1 KB the swizzle pattern repeats at
+__host__ __device__ constexpr uint32_t smem(bool three) { return oBar(three) + 2 * kStages * 8 + 1024; }
+}  // namespace wg
+
+// byte offset of (unit n, sample k) in a K-major [128][32] fp32 tile with the 128-byte swizzle: 16-byte group k / 4 of row n
+// lands at group (k / 4) ^ (n % 8)
+__device__ __forceinline__ uint32_t sw128_off(int n, int k) { return n * 128 + ((((k >> 2) ^ n) & 7) << 4) + (k & 3) * 4; }
+
+// shared-memory matrix descriptor of a K-major operand in the 128-byte-swizzle layout: 8-row groups 1024 B apart
+__device__ __forceinline__ uint64_t sw128_desc(uint32_t addr) {
+  return (uint64_t)((addr & 0x3FFFF) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
+}
+
+// d (64 x 128, fp32, accumulator layout) = (kScaleD ? d : 0) + A (64 x 8, registers, mma.m16n8k8 A layout per warp) . B (desc)
+template <int kScaleD>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], const uint32_t (&a)[4], uint64_t desc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, "
+      "%26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, "
+      "%51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),
+        "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),
+        "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
+        "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc), "n"(kScaleD));
+}
+
+// 16- and 4-byte asynchronous copies global -> shared; ok = false writes zeros and reads nothing
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool ok) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(ok ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async4(uint32_t dst, const void* src, bool ok) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(ok ? 4 : 0) : "memory");
+}
+
+// Producer thread tid (warp pw) copies its share of chunk ch into a raw slot: sample row lane of H1 unit quads pw + 4 j as
+// float4 [j][tid] (the coalesced 16-byte panel loads of dw2_load), warp 0 also rgb and grad_rgb, warp 1 the four mask words
+// ([pw][6][32] words after the H1 part).  Rows >= n_pts are zeros.  Always commits one cp.async group.
+__device__ __forceinline__ void dw2_raw_issue(uint8_t* slot, const float* __restrict__ rgb, const float* __restrict__ h1_save,
+                                              const uint32_t* __restrict__ h2_mask, const float* __restrict__ grad_rgb,
+                                              int64_t ch, int64_t n_chunks, int64_t n_pts, int tid) {
+  const int pw = tid >> 5, lane = tid & 31;
+  if (ch < n_chunks) {
+    const int64_t r = ch * dw::kK + lane;
+    const bool ok = r < n_pts;
+    const float* src = h1_save + (ok ? save_idx<true, kHidden>(r, 4 * pw) : 0);
+    const uint32_t dst = smem_u32(slot) + tid * 16;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) cp_async16(dst + j * 128 * 16, ok ? src + j * 4 * kPanelRows * 4 : h1_save, ok);
+    const uint32_t xd = smem_u32(slot + wg::kRawH1) + (pw * 6 * 32 + lane) * 4;
+    if (pw == 0) {
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+        cp_async4(xd + i * 128, ok ? rgb + r * 3 + i : rgb, ok);
+        cp_async4(xd + (3 + i) * 128, ok ? grad_rgb + r * 3 + i : grad_rgb, ok);
+      }
+    } else if (pw == 1) {
+#pragma unroll
+      for (int c = 0; c < kHidden / 32; ++c) cp_async4(xd + c * 128, ok ? h2_mask + mask_idx<kHidden>(r, c) : h2_mask, ok);
+    }
+  }
+  asm volatile("cp.async.commit_group;" ::: "memory");
+}
+
+// the same thread's share from the raw slot into a stage: H1 split into hi / lo and transposed into the swizzled tiles,
+// dz3 [3][32] and the mask words [4][32] after them
+template <bool kThree>
+__device__ __forceinline__ void dw2_stage_put(const uint8_t* slot, uint8_t* stage, int tid) {
+  const int pw = tid >> 5, lane = tid & 31;
+  const float4* h1 = reinterpret_cast<const float4*>(slot);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int q = pw + 4 * j;
+    const float4 h = h1[j * 128 + tid];
+    const float v[4] = {h.x, h.y, h.z, h.w};
+    uint32_t hi[4], lo[4];
+    split4(v, hi, lo);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const uint32_t off = sw128_off(4 * q + e, lane);
+      *reinterpret_cast<uint32_t*>(stage + off) = hi[e];
+      if (kThree) *reinterpret_cast<uint32_t*>(stage + wg::kTile + off) = lo[e];
+    }
+  }
+  const float* x = reinterpret_cast<const float*>(slot + wg::kRawH1) + pw * 6 * 32 + lane;
+  float* sx = reinterpret_cast<float*>(stage + (kThree ? 2 : 1) * wg::kTile) + lane;
+  if (pw == 0) {
+#pragma unroll
+    for (int i = 0; i < 3; ++i) sx[i * 32] = x[(3 + i) * 32] * x[i * 32] * (1.f - x[i * 32]);
+  } else if (pw == 1) {
+#pragma unroll
+    for (int c = 0; c < kHidden / 32; ++c) sx[(3 + c) * 32] = x[c * 32];
+  }
+}
+
+template <bool kThree>
+__global__ void __launch_bounds__(wg::kThreads, 1) k_shade_dw2_wgmma(const float* __restrict__ W3, const float* __restrict__ rgb,
+                                                                      const float* __restrict__ h1_save,
+                                                                      const uint32_t* __restrict__ h2_mask,
+                                                                      const float* __restrict__ grad_rgb, int64_t n_pts,
+                                                                      float* __restrict__ grad_W2) {
+  constexpr int kW = kHidden;
+  constexpr uint32_t kStage = wg::stage_bytes(kThree);
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  const int tid = threadIdx.x, lane = tid & 31;
+  const uint32_t full0 = smem_u32(smem + wg::oBar(kThree)), empty0 = full0 + 8 * wg::kStages;
+  if (tid == 0) {
+    for (int s = 0; s < wg::kStages; ++s) {
+      mbar_init(full0 + 8 * s, 128);
+      mbar_init(empty0 + 8 * s, 256);
+    }
+  }
+  __syncthreads();
+  const int64_t n_chunks = (n_pts + dw::kK - 1) / dw::kK, step = gridDim.x;
+
+  if (tid < 128) {                                          // producer
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(wg::kProducerRegs));
+    uint8_t* raw = smem + wg::oRaw(kThree);
+    const int64_t ch0 = blockIdx.x;
+    for (int k = 0; k < wg::kRaw - 1; ++k)
+      dw2_raw_issue(raw + k * wg::kRawSlot, rgb, h1_save, h2_mask, grad_rgb, ch0 + k * step, n_chunks, n_pts, tid);
+    int i = 0;
+    for (int64_t ch = ch0; ch < n_chunks; ch += step, ++i) {
+      // the slot refilled here was read into the stage at the previous chunk
+      dw2_raw_issue(raw + (i + wg::kRaw - 1) % wg::kRaw * wg::kRawSlot, rgb, h1_save, h2_mask, grad_rgb,
+                    ch + (wg::kRaw - 1) * step, n_chunks, n_pts, tid);
+      asm volatile("cp.async.wait_group %0;" ::"n"(wg::kRaw - 1) : "memory");   // this chunk's copies have landed
+      const int s = i % wg::kStages;
+      mbar_wait(empty0 + 8 * s, ((i / wg::kStages) & 1) ^ 1);
+      dw2_stage_put<kThree>(raw + i % wg::kRaw * wg::kRawSlot, smem + s * kStage, tid);
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the generic-proxy stores, before wgmma reads them
+      mbar_arrive(full0 + 8 * s);
+    }
+    return;
+  }
+
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(wg::kConsumerRegs));
+  const int ct = tid - 128, g = lane >> 2, t = lane & 3;
+  const int m0 = 64 * (ct >> 7) + 16 * ((ct >> 5) & 3) + g;     // this thread's rows m0 and m0 + 8 (same 32-unit mask word)
+  float w3[3][2];
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    w3[i][0] = W3[i * kW + m0];
+    w3[i][1] = W3[i * kW + m0 + 8];
+  }
+  float acc[64], sum[64];
+#pragma unroll
+  for (int e = 0; e < 64; ++e) acc[e] = sum[e] = 0.f;
+  int i = 0;
+  for (int64_t ch = blockIdx.x; ch < n_chunks; ch += step, ++i) {
+    const int s = i % wg::kStages;
+    mbar_wait(full0 + 8 * s, (i / wg::kStages) & 1);
+    uint8_t* stage = smem + s * kStage;
+    const float* sx = reinterpret_cast<const float*>(stage + (kThree ? 2 : 1) * wg::kTile);
+    // A[m][k] = dZ2[sample 8 ks + k][unit m], a0 = (m0, t), a1 = (m0 + 8, t), a2 = (m0, t + 4), a3 = (m0 + 8, t + 4)
+    uint32_t ah[4][4], al[4][4];
+#pragma unroll
+    for (int ks = 0; ks < dw::kK / 8; ++ks) {
+      float av[4];
+#pragma unroll
+      for (int q = 0; q < 2; ++q) {
+        const int k = 8 * ks + t + 4 * q;
+        const float dz3[3] = {sx[k], sx[32 + k], sx[64 + k]};
+        const uint32_t w = __float_as_uint(sx[(3 + (m0 >> 5)) * 32 + k]) >> (m0 & 31);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float dh = dz3[0] * w3[0][h] + dz3[1] * w3[1][h] + dz3[2] * w3[2][h];
+          av[2 * q + h] = ((w >> (8 * h)) & 1u) ? dh : 0.f;
+        }
+      }
+      split4(av, ah[ks], al[ks]);
+    }
+    const uint32_t b = smem_u32(stage);
+    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+    for (int ks = 0; ks < dw::kK / 8; ++ks) {
+      const uint64_t bh = sw128_desc(b + 32 * ks);
+      if (kThree) {
+        if (ks == 0) wgmma_tf32<0>(acc, al[ks], bh);
+        else wgmma_tf32<1>(acc, al[ks], bh);
+        wgmma_tf32<1>(acc, ah[ks], sw128_desc(b + wg::kTile + 32 * ks));
+        wgmma_tf32<1>(acc, ah[ks], bh);
+      } else if (ks == 0) {
+        wgmma_tf32<0>(acc, ah[ks], bh);
+      } else {
+        wgmma_tf32<1>(acc, ah[ks], bh);
+      }
+    }
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+#pragma unroll
+    for (int e = 0; e < 64; ++e) asm volatile("" : "+f"(acc[e])::"memory");   // no read of acc above the wait
+    mbar_arrive(empty0 + 8 * s);
+#pragma unroll
+    for (int e = 0; e < 64; ++e) sum[e] += acc[e];
+  }
+  // accumulator element 4 j + e: row m0 + 8 (e / 2), column 8 j + 2 t + e % 2
+#pragma unroll
+  for (int j = 0; j < 16; ++j)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) atomicAdd(grad_W2 + (m0 + 8 * (e >> 1)) * kW + 8 * j + 2 * t + (e & 1), sum[4 * j + e]);
+}
 #undef UBN_SHADE_DW2_ARGS
 #undef UBN_SHADE_DW2_PARAMS
 
@@ -976,6 +1209,21 @@ int launch_dw2(const float* W3, const float* rgb, const float* h1, const float* 
   return 0;
 }
 
+// which engine computes dW2 at width 128 with panel saves and H2 masks: 1 = k_shade_dw2_wgmma (default), 0 = k_shade_dw2_tc
+int g_dw2_engine = 1;
+
+template <bool kThree>
+int launch_dw2_wgmma(const float* W3, const float* rgb, const float* h1, const uint32_t* m2, const float* grad_rgb, int64_t n,
+                     float* gW2, cudaStream_t st) {
+  auto k = tc::k_shade_dw2_wgmma<kThree>;
+  constexpr uint32_t bytes = tc::wg::smem(kThree);
+  if (int e = set_smem(k, bytes)) return e;
+  const int64_t n_chunks = (n + tc::dw::kK - 1) / tc::dw::kK;
+  k<<<(unsigned)std::min<int64_t>(kNumSMs, n_chunks), tc::wg::kThreads, bytes, st>>>(W3, rgb, h1, m2, grad_rgb, n, gW2);
+  UBN_LAUNCH_CHECK();
+  return 0;
+}
+
 template <int kF>
 int rgbnet_fwd_tc(const float* feat, const float* view_bias, const int64_t* ray_id, const float* W1k, const float* W2, const float* b2,
                   const float* W3, const float* b3, int64_t n_pts, float* rgb, float* h1_save, float* h2_save, uint32_t* h1_mask,
@@ -1022,6 +1270,10 @@ int rgbnet_bwd_tc_fused(const float* feat, const int64_t* ray_id, const float* W
 #undef UBN_BWD
   if (e) return e;
 #define UBN_DW(THREE, P, M2) return launch_dw2<THREE, P, M2>(W3, rgb, h1_save, h2_save, m2, grad_rgb, n_pts, grad_W2, st)
+  if (mask2 && g_dw2_engine == 1) {
+    if (one) return launch_dw2_wgmma<false>(W3, rgb, h1_save, m2, grad_rgb, n_pts, grad_W2, st);
+    return launch_dw2_wgmma<true>(W3, rgb, h1_save, m2, grad_rgb, n_pts, grad_W2, st);
+  }
   if (mask2) { if (one) UBN_DW(false, true, true); else UBN_DW(true, true, true); }
   if (panel) { if (one) UBN_DW(false, true, false); else UBN_DW(true, true, false); }
   if (one) UBN_DW(false, false, false); else UBN_DW(true, false, false);
@@ -1067,6 +1319,12 @@ int rgbnet_bwd_tc_fused_w(const float* feat, const int64_t* ray_id, const float*
 }
 
 }  // namespace
+
+extern "C" int ubn_set_dw2_engine(int engine) {
+  if (engine < 0 || engine > 1) return finish(cudaErrorInvalidValue);
+  g_dw2_engine = engine;
+  return 0;
+}
 
 extern "C" int ubn_rgbnet_fwd_tc(const float* feat, const float* view_bias, const int64_t* ray_id, const float* W1k,
                                  const float* W2, const float* b2, const float* W3, const float* b3, int64_t n_pts,

@@ -461,6 +461,13 @@ def get_density_scatter():
     return int(load().ubn_get_density_scatter())
 
 
+def set_dw2_engine(engine):
+    """grad_W2 of the width-128 rgbnet backward with ReLU masks: 1 = warpgroup MMA (default), 0 = mma.sync
+    (ubn_set_dw2_engine).  Process-wide."""
+    from ._cabi import load
+    check(load().ubn_set_dw2_engine(c_int(int(engine))))
+
+
 def cumdist_thres(dist, thres):
     _chk(dist, 'dist')
     mask = torch.empty(dist.shape, dtype=torch.bool, device=dist.device)
