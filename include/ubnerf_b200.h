@@ -557,6 +557,42 @@ int ubn_rgbnet_bwd_tc_fused_kw(int n_feat, int n_hidden, const float* feat, cons
  * ubn_set_feature_kernel.  Returns cudaErrorInvalidValue for other values. */
 int ubn_set_dw2_engine(int engine);
 
+/* ---- TensoRFGrid: the vector-matrix (VM) factorised grid (FourierGrid/grid.py:90-201) ------------------------------------------
+ * Six factors, in this order everywhere: 0 xy_plane [1,Rxy,X,Y], 1 xz_plane [1,R,X,Z], 2 yz_plane [1,R,Y,Z], 3 x_vec [1,R,X,1],
+ * 4 y_vec [1,R,Y,1], 5 z_vec [1,Rxy,Z,1], and, for C > 1, f_vec [R+R+Rxy, C] (row-major).  Factor f element (r, a, b) sits at
+ * factor[r * stride_r[f] + a * stride_a[f] + b * stride_b[f]] (vectors: a = the node, b = 0), so the reference-contiguous layout and
+ * the channels-last one (a corner's R components contiguous: stride_r == 1) are both described; the kernels take 128-bit loads and
+ * reductions when every factor is channels-last with R, Rxy multiples of 4 and 16-byte aligned bases.  Gradient buffers have the
+ * strides of their factors.  A point p reads the factors at ind = (p - xyz_min) / (xyz_max - xyz_min) * 2 - 1 (no axis flip) with
+ * F.grid_sample(bilinear, align_corners=True, zero padding) arithmetic, corners in ATen's order nw, ne, sw, se; feat =
+ * [xy.z, xz.y, yz.x] (3R products); out = sum(feat) for C = 1, feat . f_vec for C > 1.  C must be 1, 3 or 12; R + R + Rxy <= 96. */
+typedef struct UbnTensorfDesc {
+  int32_t X, Y, Z, R, Rxy, C;
+  int64_t stride_r[6], stride_a[6], stride_b[6];
+  float xyz_min[3], xyz_max[3];
+} UbnTensorfDesc;
+
+/* CTAs of the backward's persistent launch: the f_vec partial sums of the scratch below hold one [R+R+Rxy, C] block per CTA. */
+#define UBN_TENSORF_BWD_MAX_CTAS 528
+
+/* TensoRFGrid.forward: out[M, C] (fully written) for the points xyz[M, 3].  f_vec is ignored (may be NULL) when C == 1. */
+int ubn_tensorf_fwd(const float* const* factors, const float* f_vec, const UbnTensorfDesc* desc, const float* xyz, int64_t M,
+                    float* out, void* stream);
+/* Adjoint of ubn_tensorf_fwd for grad_out[M, C]: ADDED into grads[6] (the factor gradients) and grad_f_vec (C > 1).  Plane
+ * gradients are reduced straight into grads; the vector gradients go through vec_copies (1..64) replicated copies in scratch
+ * (copy = blockIdx % vec_copies), summed in a fixed order by a closing launch.  grad_f_vec = feat^T . grad_out is summed as
+ * per-128-sample partials added into one fp32 running sum per CTA, the CTAs' sums added in CTA order by the closing launch.
+ * scratch: device floats, at least vec_copies * (X*R + Y*R + Z*Rxy) + UBN_TENSORF_BWD_MAX_CTAS * (R+R+Rxy) * C, 16-byte aligned. */
+int ubn_tensorf_bwd(const float* const* factors, const float* f_vec, const UbnTensorfDesc* desc, const float* xyz, int64_t M,
+                    const float* grad_out, float* const* grads, float* grad_f_vec, int vec_copies, float* scratch, void* stream);
+/* TensoRFGrid.total_variation_add_grad: grads[f] += the gradient of the reference's smooth-L1 TV sum over the planes' two axes and
+ * the vectors' length, weighted wx / wy / wz by the world axis each factor axis spans, divided by 6.  One launch for all six. */
+int ubn_tensorf_tv_add_grad(const float* const* factors, float* const* grads, const UbnTensorfDesc* desc, float wx, float wy,
+                            float wz, void* stream);
+/* TensoRFGrid.get_dense_grid: out [1, C, X, Y, Z] (contiguous, fully written) = the node products (no interpolation), summed for
+ * C == 1, projected by f_vec for C > 1. */
+int ubn_tensorf_dense(const float* const* factors, const float* f_vec, const UbnTensorfDesc* desc, float* out, void* stream);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

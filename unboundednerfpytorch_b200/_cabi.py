@@ -25,6 +25,15 @@ class UbnGridDesc(ctypes.Structure):
                 ('xyz_min', c_f * 3), ('xyz_max', c_f * 3)]
 
 
+class UbnTensorfDesc(ctypes.Structure):
+    _fields_ = [('X', c_i32), ('Y', c_i32), ('Z', c_i32), ('R', c_i32), ('Rxy', c_i32), ('C', c_i32),
+                ('stride_r', c_i64 * 6), ('stride_a', c_i64 * 6), ('stride_b', c_i64 * 6),
+                ('xyz_min', c_f * 3), ('xyz_max', c_f * 3)]
+
+
+TENSORF_BWD_MAX_CTAS = 528   # UBN_TENSORF_BWD_MAX_CTAS of include/ubnerf_b200.h
+
+
 class UbnMarchCfg(ctypes.Structure):
     _fields_ = [('scene_center', c_f * 3), ('scene_radius', c_f * 3),
                 ('contract_B', c_f), ('contract_A', c_f),
@@ -133,6 +142,10 @@ _SIGNATURES = {
                                   c_p, c_p, c_p, c_p, c_p],
     'ubn_march_box_density_bwd': [c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnBoxMarchCfg), c_i64,
                                   c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
+    'ubn_tensorf_fwd': [c_p, c_p, ctypes.POINTER(UbnTensorfDesc), c_p, c_i64, c_p, c_p],
+    'ubn_tensorf_bwd': [c_p, c_p, ctypes.POINTER(UbnTensorfDesc), c_p, c_i64, c_p, c_p, c_p, c_int, c_p, c_p],
+    'ubn_tensorf_tv_add_grad': [c_p, c_p, ctypes.POINTER(UbnTensorfDesc), c_f, c_f, c_f, c_p],
+    'ubn_tensorf_dense': [c_p, c_p, ctypes.POINTER(UbnTensorfDesc), c_p, c_p],
 }
 _RESTYPE = {'ubn_last_error_string': ctypes.c_char_p, 'ubn_launch_count': c_i64, 'ubn_reset_launch_count': None}
 

@@ -264,7 +264,7 @@ def _count_views(density, world_size, voxel_size, rays_o_tr, rays_d_tr, imsz, ne
     the count.  far is 1e9 as the reference sets it."""
     from . import ops
     far = 1e9
-    dev = density.grid.device
+    dev = density.xyz_min.device
     ws = [int(v) for v in world_size]
     n_samples = int(np.linalg.norm(np.array(ws) + 1) / stepsize) + 1
     step = float(stepsize * voxel_size)
@@ -599,7 +599,9 @@ class DirectVoxGO(_CoarseGeo, _GridModel):
     of the survivor count) with the rgb from ``_shade`` -- the tensor-core rgbnet when shade.supported (the default fine config:
     rgbnet_dim 12, rgbnet_direct, width 128) -- for a single-slab density and a 3- or 12-channel channels-last k0.  With
     rgbnet_direct=False the march is fused and the torch epilogue sigmoid(rgbnet(cat[k0[:, 3:], emb]) + k0[:, :3]) stays.
-    ``forward_ops`` composes the drop-in ops in the reference's order (the cross-check and the path for other grids).
+    ``forward_ops`` composes the drop-in ops in the reference's order (the cross-check and the path for other grids).  With a
+    TensoRFGrid density or k0 (``density_type`` / ``k0_type``, built through ``grid.create_grid`` as dvgo.py does) ``forward`` runs
+    that composition on the TensoRF kernels and shades with ``_shade``, since the fused march reads dense grids only.
 
     The coarse-to-fine schedule of run_train.py works: maskout_near_cam_vox, voxel_count_views (per-voxel lr), scale_volume_grid,
     update_occupancy_cache, and ``mask_cache_path``.  The latter builds the fine mask as the reference does (dvgo.py:138-152):
@@ -624,7 +626,8 @@ class DirectVoxGO(_CoarseGeo, _GridModel):
         self.register_buffer('act_shift', torch.FloatTensor([np.log(1 / (1 - alpha_init) - 1)]))
         self._set_grid_resolution(num_voxels)
         self.density_type, self.density_config, self.k0_type, self.k0_config = density_type, density_config, k0_type, k0_config
-        self.density = G.DenseGrid(channels=1, world_size=self.world_size, xyz_min=self.xyz_min, xyz_max=self.xyz_max)
+        self.density = G.create_grid(density_type, channels=1, world_size=self.world_size, xyz_min=self.xyz_min,
+                                     xyz_max=self.xyz_max, config=self.density_config)
         self.rgbnet_kwargs = dict(rgbnet_dim=rgbnet_dim, rgbnet_direct=rgbnet_direct, rgbnet_full_implicit=rgbnet_full_implicit,
                                   rgbnet_depth=rgbnet_depth, rgbnet_width=rgbnet_width, viewbase_pe=viewbase_pe)
         self.rgbnet_direct = rgbnet_direct
@@ -633,7 +636,8 @@ class DirectVoxGO(_CoarseGeo, _GridModel):
         else:
             self.k0_dim = rgbnet_dim
             self._add_rgbnet(rgbnet_dim if rgbnet_direct else rgbnet_dim - 3, viewbase_pe, rgbnet_width, rgbnet_depth)
-        self.k0 = G.DenseGrid(channels=self.k0_dim, world_size=self.world_size, xyz_min=self.xyz_min, xyz_max=self.xyz_max)
+        self.k0 = G.create_grid(k0_type, channels=self.k0_dim, world_size=self.world_size, xyz_min=self.xyz_min,
+                                xyz_max=self.xyz_max, config=self.k0_config)
         self.mask_cache_path, self.mask_cache_thres = mask_cache_path, mask_cache_thres
         if mask_cache_world_size is None:
             mask_cache_world_size = self.world_size
@@ -691,10 +695,25 @@ class DirectVoxGO(_CoarseGeo, _GridModel):
                             irregular_shape)
 
     @torch.no_grad()
+    def update_occupancy_cache(self):
+        """dvgo.py:236-245.  A TensoRF density is read at the mask lattice through its own forward, then pooled and ANDed as for
+        the dense grids."""
+        if not self._tensorf():
+            return super().update_occupancy_cache()
+        from . import ops
+        density = self.density(self._mask_lattice(self.mask_cache.mask.shape))
+        alpha = self.activate_density(density).contiguous()
+        ops.maxpool3_gt_and_(self.mask_cache.mask, alpha, self.fast_color_thres)
+
+    @torch.no_grad()
     def maskout_near_cam_vox(self, cam_o, near_clip):
         """dvgo.py:185-198: density = -100 at the points of the world lattice linspace(xyz_min, xyz_max, world_size) that are
         within near_clip of a camera position (one kernel: every voxel scans the camera list)."""
         from . import ops
+        if isinstance(self.density, G.TensoRFGrid):
+            # dvgo.py:197 writes density.grid, which a TensoRFGrid does not have (the reference fails there as well); the
+            # shipped TensoRF config runs it only in the DenseGrid coarse stage
+            raise NotImplementedError('maskout_near_cam_vox needs a DenseGrid density (a TensoRFGrid has no voxel lattice)')
         lo, hi = self.xyz_min.cpu().tolist(), self.xyz_max.cpu().tolist()
         cams = cam_o.to(self.density.grid.device).reshape(-1, 3)
         ops.maskout_near_cam_(self.density.grid.data[0][0], cams, near_clip, -100.0, lattice=(lo, hi))
@@ -719,8 +738,11 @@ class DirectVoxGO(_CoarseGeo, _GridModel):
         # so a device-side voxel_size (after scale_volume_grid on a CUDA model) costs one sync per rescale, not per step
         return stepsize * host_scalar(self.voxel_size)
 
+    def _tensorf(self):
+        return isinstance(self.density, G.TensoRFGrid) or isinstance(self.k0, G.TensoRFGrid)
+
     def _fused_ok(self, stepsize):
-        if not march.box_supported(self.density.grid, self.k0.grid):
+        if self._tensorf() or not march.box_supported(self.density.grid, self.k0.grid):
             return False
         lo, hi = self._host()
         return march.box_s_max(lo, hi, self._stepdist(stepsize)) <= march.BOX_S_MAX_LIMIT
@@ -733,6 +755,9 @@ class DirectVoxGO(_CoarseGeo, _GridModel):
         """dvgo.py:330-397 on the fused box march (see the class docstring); same keys as the reference's ret_dict."""
         assert len(rays_o.shape) == 2 and rays_o.shape[-1] == 3, 'Only suuport point queries in [N, 3] format'
         stepsize = render_kwargs['stepsize']
+        if self._tensorf():
+            # the fused march reads dense grids only: the op-by-op composition with the TensoRF kernels, shaded as the march is
+            return self._compose(rays_o, rays_d, viewdirs, self._shade_k0, render_kwargs)
         if not (rays_o.is_cuda and self._fused_ok(stepsize)):
             return self.forward_ops(rays_o, rays_d, viewdirs, global_step=global_step, **render_kwargs)
         if self._pending_mask is not None:
@@ -746,17 +771,34 @@ class DirectVoxGO(_CoarseGeo, _GridModel):
         kdesc = G.grid_desc(self.k0.grid, *self.k0._bounds(), 0)
         weights, alphainv_last, alpha, k0, ray_id, step_id = march.BoxMarch.apply(
             self.density.grid, self.k0.grid, rays_o, rays_d, self.mask_cache.mask, cfg, ddesc, kdesc)
-        if self.rgbnet is None or self.rgbnet_direct:
-            rgb = self._shade(k0, viewdirs, ray_id)
-        else:
-            emb = _view_embed(viewdirs, self.viewfreq).flatten(0, -2)[ray_id]
-            rgb = torch.sigmoid(self.rgbnet(torch.cat([k0[:, 3:], emb], -1)) + k0[:, :3])
+        rgb = self._shade_k0(k0, viewdirs, ray_id)
         return self._finish(N, weights, alphainv_last, alpha, rgb, ray_id, step_id, render_kwargs)
+
+    def _shade_k0(self, k0, viewdirs, ray_id):
+        """rgb of the samples as forward computes it: _shade (the tensor-core rgbnet where shade.supported); with
+        rgbnet_direct=False the torch epilogue sigmoid(rgbnet(cat[k0[:, 3:], emb]) + k0[:, :3])."""
+        if self.rgbnet is None or self.rgbnet_direct:
+            return self._shade(k0, viewdirs, ray_id)
+        emb = _view_embed(viewdirs, self.viewfreq).flatten(0, -2)[ray_id]
+        return torch.sigmoid(self.rgbnet(torch.cat([k0[:, 3:], emb], -1)) + k0[:, :3])
+
+    def _shade_torch(self, k0, viewdirs, ray_id):
+        """rgb of the samples with the rgbnet in torch, as dvgo.py:373-397 writes it."""
+        if self.rgbnet is None:
+            return torch.sigmoid(k0)
+        k0_view = k0 if self.rgbnet_direct else k0[:, 3:]
+        emb = _view_embed(viewdirs, self.viewfreq).flatten(0, -2)[ray_id]
+        logit = self.rgbnet(torch.cat([k0_view, emb], -1))
+        return torch.sigmoid(logit if self.rgbnet_direct else logit + k0[:, :3])
 
     def forward_ops(self, rays_o, rays_d, viewdirs, global_step=None, **render_kwargs):
         """Op-by-op composition in the reference's order (dvgo.py:330-397): ragged sample_pts_on_rays, boolean-mask compactions,
         grid reads with their autograd, the rgbnet in torch."""
         assert len(rays_o.shape) == 2 and rays_o.shape[-1] == 3, 'Only suuport point queries in [N, 3] format'
+        return self._compose(rays_o, rays_d, viewdirs, self._shade_torch, render_kwargs)
+
+    def _compose(self, rays_o, rays_d, viewdirs, shade, render_kwargs):
+        """The body of forward_ops with the shading step ``shade(k0, viewdirs, ray_id) -> rgb`` as a parameter."""
         N, dev = len(rays_o), rays_o.device
         ray_pts, ray_id, step_id = self.sample_ray(rays_o=rays_o, rays_d=rays_d, **render_kwargs)
         interval = render_kwargs['stepsize'] * self.voxel_size_ratio
@@ -773,13 +815,7 @@ class DirectVoxGO(_CoarseGeo, _GridModel):
             mask = (weights > self.fast_color_thres)
             weights, alpha, ray_pts, ray_id, step_id = weights[mask], alpha[mask], ray_pts[mask], ray_id[mask], step_id[mask]
         k0 = self.k0(ray_pts)
-        if self.rgbnet is None:
-            rgb = torch.sigmoid(k0)
-        else:
-            k0_view = k0 if self.rgbnet_direct else k0[:, 3:]
-            emb = _view_embed(viewdirs, self.viewfreq).flatten(0, -2)[ray_id]
-            logit = self.rgbnet(torch.cat([k0_view, emb], -1))
-            rgb = torch.sigmoid(logit if self.rgbnet_direct else logit + k0[:, :3])
+        rgb = shade(k0, viewdirs, ray_id)
         return self._finish(N, weights, alphainv_last, alpha, rgb, ray_id, step_id, render_kwargs)
 
     def _finish(self, N, weights, alphainv_last, alpha, rgb, ray_id, step_id, render_kwargs):
