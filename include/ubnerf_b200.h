@@ -593,6 +593,32 @@ int ubn_tensorf_tv_add_grad(const float* const* factors, float* const* grads, co
  * C == 1, projected by f_vec for C > 1. */
 int ubn_tensorf_dense(const float* const* factors, const float* f_vec, const UbnTensorfDesc* desc, float* out, void* stream);
 
+/* ---- scene bounds (FourierGrid/bbox_compute.py) ------------------------------------------------------------------------------
+ * Each call widens bounds = device float[6] (xyz_min then xyz_max; pass +inf / -inf to start empty) IN PLACE: bounds[a] =
+ * min(bounds[a], min of the points' axis a), bounds[3+a] likewise with max.  A NaN coordinate makes that bound NaN (torch.minimum
+ * / amin propagate NaN).  Min and max are order independent: results are exact and deterministic. */
+
+/* compute_bbox_by_cam_frustrm's ray branches (:10-45, :96-110) over n_views views of the 'center' rays of get_rays_of_a_view
+ * (same bits as ubn_get_rays_of_a_view).  hw: device int32 [n_views, 2] (H, W); K: device [n_views, 9]; c2w: device
+ * [n_views, 12] (c2w[:3, :4]); max_pixels: the largest H * W (host).  inward = 1: the points rays_o + rays_d * near
+ * (unbounded-inward / nerfpp, near = near_clip); inward = 0: rays_o + dir * near and rays_o + dir * far with dir = rays_d when
+ * ndc, viewdirs otherwise.  No ray is written. */
+int ubn_frustum_bounds(const int* hw, const float* K, const float* c2w, int64_t n_views, int64_t max_pixels, int ndc, int inverse_y,
+                       int flip_x, int flip_y, int inward, float near, float far, float* bounds, void* stream);
+/* compute_bbox_by_coarse_geo's lattice (:144-149): xyz[X*Y*Z, 3] (k fastest) = lattice_min * (1 - t) + lattice_max * t with
+ * t = torch.linspace(0, 1, n) per axis; lattice_min / lattice_max: HOST float[3]. */
+int ubn_lattice_points(const float* lattice_min, const float* lattice_max, int64_t X, int64_t Y, int64_t Z, float* xyz,
+                       void* stream);
+/* compute_bbox_by_coarse_geo (:150-160) fused: the points of ubn_lattice_points whose alpha = Raw2Alpha(density(point), act_shift,
+ * interval) exceeds thres widen bounds, and their number is ADDED to *count (device int64).  density = the C = 1 grid `desc`,
+ * read as ubn_grid_sample_fwd reads it; Raw2Alpha as ubn_raw2alpha.  No point, density or alpha tensor is written. */
+int ubn_lattice_bounds(const float* grid, const UbnGridDesc* desc, const float* lattice_min, const float* lattice_max, int64_t X,
+                       int64_t Y, int64_t Z, float act_shift, float interval, float thres, float* bounds, int64_t* count,
+                       void* stream);
+/* The same reduction over a precomputed alpha[X*Y*Z] (device), for densities the fused read does not cover (TensoRFGrid). */
+int ubn_lattice_bounds_alpha(const float* alpha, const float* lattice_min, const float* lattice_max, int64_t X, int64_t Y,
+                             int64_t Z, float thres, float* bounds, int64_t* count, void* stream);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

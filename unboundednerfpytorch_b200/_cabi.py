@@ -146,6 +146,10 @@ _SIGNATURES = {
     'ubn_tensorf_bwd': [c_p, c_p, ctypes.POINTER(UbnTensorfDesc), c_p, c_i64, c_p, c_p, c_p, c_int, c_p, c_p],
     'ubn_tensorf_tv_add_grad': [c_p, c_p, ctypes.POINTER(UbnTensorfDesc), c_f, c_f, c_f, c_p],
     'ubn_tensorf_dense': [c_p, c_p, ctypes.POINTER(UbnTensorfDesc), c_p, c_p],
+    'ubn_frustum_bounds': [c_p, c_p, c_p, c_i64, c_i64, c_int, c_int, c_int, c_int, c_int, c_f, c_f, c_p, c_p],
+    'ubn_lattice_points': [c_p, c_p, c_i64, c_i64, c_i64, c_p, c_p],
+    'ubn_lattice_bounds': [c_p, ctypes.POINTER(UbnGridDesc), c_p, c_p, c_i64, c_i64, c_i64, c_f, c_f, c_f, c_p, c_p, c_p],
+    'ubn_lattice_bounds_alpha': [c_p, c_p, c_p, c_i64, c_i64, c_i64, c_f, c_p, c_p, c_p],
 }
 _RESTYPE = {'ubn_last_error_string': ctypes.c_char_p, 'ubn_launch_count': c_i64, 'ubn_reset_launch_count': None}
 

@@ -31,6 +31,23 @@ __host__ __device__ __forceinline__ T ceil_div(T a, T b) { return (a + b - 1) / 
 // grid size for a plain elementwise kernel: one thread per element, capped only by int range
 inline unsigned blocks_for(int64_t n, int threads) { return (unsigned)((n + threads - 1) / threads); }
 
+// torch.linspace(start, end, n)[i] as ATen's CUDA kernel evaluates it (RangeFactories.cu): step = (end - start) / (n - 1), then
+// start + step * i below the midpoint and end - step * (n - 1 - i) from it on, both contracted to one fma by nvcc.  Shared by the
+// lattice kernels of grid_utils.cu and bounds.cu.
+__device__ __forceinline__ float linspace_at(float start, float end, int n, int i) {
+  if (n <= 1) return start;
+  const float step = __fdiv_rn(__fsub_rn(end, start), (float)(n - 1));
+  return (i < n / 2) ? fmaf(step, (float)i, start) : fmaf(-step, (float)(n - i - 1), end);
+}
+
+// Raw2Alpha of one density (render_utils_kernel.cu:431-458): alpha = 1 - (1 + exp(d + shift))^-interval.  Shared by
+// ubn_raw2alpha (alpha_ops.cu) and the coarse-geometry bounds (bounds.cu), so both produce the same bits.
+__device__ __forceinline__ void raw2alpha_one(float d, float shift, float interval, float* e_out, float* a_out) {
+  const float e = expf(d + shift);  // can be inf
+  *e_out = e;
+  *a_out = 1 - powf(1 + e, -interval);
+}
+
 // ---- shared-memory mbarriers (the TMA brick loads of render_tma.cu, the dW2 pipeline of shade_tc.cu) ------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 

@@ -7,18 +7,12 @@
 // an activation, a max_pool3d and a boolean AND for the occupancy update; a [N,S,3] point tensor plus a full autograd backward
 // per 10 000 rays for the view count.  Here every utility is one or two kernels that generate lattice / sample coordinates in
 // registers.  Lattice coordinates follow torch.linspace's CUDA kernel (start + step * i below the midpoint, end - step * (n-1-i)
-// above; both FMA-contracted by nvcc) so that threshold decisions agree with the reference's tensors.
+// above; both FMA-contracted by nvcc; linspace_at, common.cuh) so that threshold decisions agree with the reference's tensors.
 #include <algorithm>
 
 #include "march_common.cuh"
 
 namespace ubn {
-
-__device__ __forceinline__ float linspace_at(float start, float end, int n, int i) {
-  if (n <= 1) return start;
-  const float step = __fdiv_rn(__fsub_rn(end, start), (float)(n - 1));
-  return (i < n / 2) ? fmaf(step, (float)i, start) : fmaf(-step, (float)(n - i - 1), end);
-}
 
 // alpha = Raw2Alpha(density(lattice point)) on an [mX, mY, mZ] lattice spanning [lo, hi] inclusive
 __global__ void __launch_bounds__(256) k_lattice_alpha(GridView g, float lox, float loy, float loz, float hix, float hiy, float hiz,

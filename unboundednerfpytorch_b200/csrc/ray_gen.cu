@@ -4,18 +4,9 @@
 // Replaces FourierGrid/dvgo.py:492-555 (get_rays + ndc_rays + get_rays_of_a_view: ~20 torch kernels per view and a
 // [H,W,3,3] intermediate) and the four index kernels of run_train.py:204-212 (target / rays_o / rays_d / viewdirs
 // = *_tr[sel_i]).  Outputs only: 36 B written per pixel, nothing read but 21 scalars.
-#include "common.cuh"
+#include "ray_gen.cuh"
 
 namespace ubn {
-
-struct ViewParams {
-  float fx, fy, cx, cy;     // K[0][0], K[1][1], K[0][2], K[1][2]
-  float r[3][3], t[3];      // c2w[:3,:3], c2w[:3,3]
-  int H, W;
-  int ndc, inverse_y, flip_x, flip_y;
-  float pix;                // 0.5 for mode 'center', 0 for 'lefttop' / 'random' (random offsets come in `jitter`)
-  float sw, sh;             // ndc scales -1/(W/(2 focal)), -1/(H/(2 focal)), evaluated in double on the host like Python does
-};
 
 __global__ void __launch_bounds__(256) k_rays_of_a_view(ViewParams v, const float* __restrict__ jitter,
                                                         float* __restrict__ rays_o, float* __restrict__ rays_d,
@@ -24,43 +15,10 @@ __global__ void __launch_bounds__(256) k_rays_of_a_view(ViewParams v, const floa
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= n) return;
   const int row = (int)(p / v.W), col = (int)(p - (int64_t)row * v.W);
-  // i, j are built BEFORE the flips (dvgo.py:497-513): the flipped image takes the value of the mirrored pixel
-  const int sc = v.flip_x ? v.W - 1 - col : col;
-  const int sr = v.flip_y ? v.H - 1 - row : row;
-  float i = (float)sc + v.pix, j = (float)sr + v.pix;
-  if (jitter) {   // mode 'random' (dvgo.py:503-505): i + rand_like(i), j + rand_like(j) drawn BEFORE the flips, and i is
-                  // flipped along x only, j along y only; jitter = [2,H,W] (plane 0 for i, plane 1 for j)
-    i = (float)sc + jitter[(int64_t)row * v.W + sc];
-    j = (float)sr + jitter[n + (int64_t)sr * v.W + col];
-  }
-  float d0 = __fdiv_rn(__fsub_rn(i, v.cx), v.fx);
-  float d1 = __fdiv_rn(__fsub_rn(j, v.cy), v.fy);
-  float d2 = 1.f;
-  if (!v.inverse_y) { d1 = -d1; d2 = -1.f; }
-  float rd[3];
-#pragma unroll
-  for (int k = 0; k < 3; ++k)   // torch.sum(dirs[..., None, :] * c2w[:3,:3], -1): products first, then a 3-term sum
-    rd[k] = __fadd_rn(__fadd_rn(__fmul_rn(d0, v.r[k][0]), __fmul_rn(d1, v.r[k][1])), __fmul_rn(d2, v.r[k][2]));
-  const float nrm = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(rd[0], rd[0]), __fmul_rn(rd[1], rd[1])), __fmul_rn(rd[2], rd[2])));
-  float ro[3] = {v.t[0], v.t[1], v.t[2]};
-  float* vd = viewdirs + 3 * p;
-  vd[0] = __fdiv_rn(rd[0], nrm); vd[1] = __fdiv_rn(rd[1], nrm); vd[2] = __fdiv_rn(rd[2], nrm);
-  if (v.ndc) {   // ndc_rays(H, W, focal = K[0][0], near = 1, ...)  dvgo.py:532-550
-    const float near = 1.f;
-    const float tt = __fdiv_rn(-__fadd_rn(near, ro[2]), rd[2]);
-    ro[0] = __fadd_rn(ro[0], __fmul_rn(tt, rd[0]));
-    ro[1] = __fadd_rn(ro[1], __fmul_rn(tt, rd[1]));
-    ro[2] = __fadd_rn(ro[2], __fmul_rn(tt, rd[2]));
-    const float sw = v.sw, sh = v.sh;
-    const float o0 = __fdiv_rn(__fmul_rn(sw, ro[0]), ro[2]);
-    const float o1 = __fdiv_rn(__fmul_rn(sh, ro[1]), ro[2]);
-    const float o2 = __fadd_rn(1.f, __fdiv_rn(2.f * near, ro[2]));
-    const float e0 = __fmul_rn(sw, __fsub_rn(__fdiv_rn(rd[0], rd[2]), __fdiv_rn(ro[0], ro[2])));
-    const float e1 = __fmul_rn(sh, __fsub_rn(__fdiv_rn(rd[1], rd[2]), __fdiv_rn(ro[1], ro[2])));
-    const float e2 = __fdiv_rn(-2.f * near, ro[2]);
-    ro[0] = o0; ro[1] = o1; ro[2] = o2;
-    rd[0] = e0; rd[1] = e1; rd[2] = e2;
-  }
+  float ro[3], rd[3], vd[3];
+  pixel_ray(v, row, col, jitter, ro, rd, vd);
+  float* w = viewdirs + 3 * p;
+  w[0] = vd[0]; w[1] = vd[1]; w[2] = vd[2];
   float* o = rays_o + 3 * p;
   float* d = rays_d + 3 * p;
   o[0] = ro[0]; o[1] = ro[1]; o[2] = ro[2];
@@ -107,8 +65,7 @@ int ubn_get_rays_of_a_view(int H, int W, const float* K_host, const float* c2w_h
   }
   v.H = H; v.W = W; v.ndc = ndc; v.inverse_y = inverse_y; v.flip_x = flip_x; v.flip_y = flip_y;
   v.pix = mode == 1 ? 0.5f : 0.f;
-  v.sw = (float)(-1.0 / (W / (2.0 * (double)v.fx)));
-  v.sh = (float)(-1.0 / (H / (2.0 * (double)v.fx)));
+  ndc_scales(H, W, v.fx, v.sw, v.sh);
   const int64_t n = (int64_t)H * W;
   k_rays_of_a_view<<<blocks_for(n, 256), 256, 0, as_stream(stream)>>>(v, mode == 2 ? jitter : nullptr, rays_o, rays_d, viewdirs);
   UBN_LAUNCH_CHECK();

@@ -24,6 +24,12 @@ from . import shade as shade_mod
 from .functional import Alphas2Weights, Raw2Alpha, composite_rgb, host_scalar, segment_sum
 
 
+def _host_array(v):
+    """A bbox argument as a host array: lists, NumPy arrays and tensors on any device (compute_bbox_by_cam_frustrm /
+    compute_bbox_by_coarse_geo return CUDA tensors, which run_train.py passes straight to the model constructors)."""
+    return np.asarray(v.detach().cpu() if torch.is_tensor(v) else v)
+
+
 def _cube_root_size(xyz_min, xyz_max, num_voxels):
     return ((xyz_max - xyz_min).prod() / num_voxels).pow(1 / 3)
 
@@ -171,8 +177,8 @@ class _ContractedBase(_GridModel):
 
     # ---- helpers --------------------------------------------------------------------------------
     def _init_scene(self, xyz_min, xyz_max, bg_len, fast_color_thres, contracted_norm):
-        xyz_min = torch.as_tensor(np.asarray(xyz_min), dtype=torch.float32)
-        xyz_max = torch.as_tensor(np.asarray(xyz_max), dtype=torch.float32)
+        xyz_min = torch.as_tensor(_host_array(xyz_min), dtype=torch.float32)
+        xyz_max = torch.as_tensor(_host_array(xyz_max), dtype=torch.float32)
         assert len(((xyz_max - xyz_min) * 100000).long().unique()), 'scene bbox must be a cube'
         self.register_buffer('scene_center', (xyz_min + xyz_max) * 0.5)
         self.register_buffer('scene_radius', (xyz_max - xyz_min) * 0.5)
@@ -617,8 +623,8 @@ class DirectVoxGO(_CoarseGeo, _GridModel):
         super().__init__()
         if rgbnet_full_implicit:
             raise NotImplementedError('rgbnet_full_implicit is outside the hot-path scope')
-        self.register_buffer('xyz_min', torch.as_tensor(np.asarray(xyz_min), dtype=torch.float32))
-        self.register_buffer('xyz_max', torch.as_tensor(np.asarray(xyz_max), dtype=torch.float32))
+        self.register_buffer('xyz_min', torch.as_tensor(_host_array(xyz_min), dtype=torch.float32))
+        self.register_buffer('xyz_max', torch.as_tensor(_host_array(xyz_max), dtype=torch.float32))
         self.fast_color_thres = fast_color_thres
         self.num_voxels_base = num_voxels_base
         self.voxel_size_base = _cube_root_size(self.xyz_min, self.xyz_max, num_voxels_base)
@@ -842,8 +848,8 @@ class DirectMPIGO(_GridModel):
         super().__init__()
         if density_type != 'DenseGrid' or k0_type != 'DenseGrid':
             raise NotImplementedError('only DenseGrid is on the hot path (TensoRFGrid is out of scope)')
-        self.register_buffer('xyz_min', torch.as_tensor(np.asarray(xyz_min), dtype=torch.float32).clone())
-        self.register_buffer('xyz_max', torch.as_tensor(np.asarray(xyz_max), dtype=torch.float32).clone())
+        self.register_buffer('xyz_min', torch.as_tensor(_host_array(xyz_min), dtype=torch.float32).clone())
+        self.register_buffer('xyz_max', torch.as_tensor(_host_array(xyz_max), dtype=torch.float32).clone())
         self.fast_color_thres = fast_color_thres
         self._set_grid_resolution(num_voxels, mpi_depth)
         self.density_type, self.density_config = density_type, density_config
