@@ -593,6 +593,33 @@ int ubn_tensorf_tv_add_grad(const float* const* factors, float* const* grads, co
  * C == 1, projected by f_vec for C > 1. */
 int ubn_tensorf_dense(const float* const* factors, const float* f_vec, const UbnTensorfDesc* desc, float* out, void* stream);
 
+/* ---- the fused box march with TensoRF grids (DirectVoxGO.forward, dvgo.py:330-366, with density_type / k0_type 'TensoRFGrid';
+ *      grid.py:111-129 / 174-201 for the read).  Same records, flags, scan and thresholds as ubn_march_box_density_fwd; the density
+ *      is the TensoRF read of ubn_tensorf_fwd (C = 1) at the same box point, so every output is bit-identical to sample_pts_on_rays
+ *      + mask cache + TensoRFGrid + Raw2Alpha + Alphas2Weights composed op by op. ---- */
+/* Pass A with a TensoRF density: desc->C == 1, factors and desc as for ubn_tensorf_fwd; everything else as
+ * ubn_march_box_density_fwd.  Samples outside the mask cache are not read. */
+int ubn_march_box_tensorf_density_fwd(const float* rays_o, const float* rays_d, const float* const* factors, const UbnTensorfDesc* desc,
+                                      const uint8_t* mask_world, const UbnBoxMarchCfg* cfg, int64_t n_rays, float* density,
+                                      float* alpha, float* weight, float* T, uint8_t* flags, float* alphainv_last, int32_t* n_keep,
+                                      int32_t* overflow, void* stream);
+/* Backward of the above: the reverse scan of ubn_march_box_density_bwd leaves every sample's density gradient in gd_scratch
+ * [n_rays * s_max]; a second launch walks each ray's own n_steps, recomputes the point of every record with a nonzero gradient and
+ * ADDS the adjoint of the read into grads[6] as ubn_tensorf_bwd does (planes reduced directly, vectors through vec_copies (1..64)
+ * replicated copies in vec_scratch -- at least vec_copies * (X*R + Y*R + Z*Rxy) floats, 16-byte aligned -- summed in copy order
+ * by a closing launch). */
+int ubn_march_box_tensorf_density_bwd(const float* rays_o, const float* rays_d, const float* const* factors, const UbnTensorfDesc* desc,
+                                      const UbnBoxMarchCfg* cfg, int64_t n_rays, const float* density, const float* alpha,
+                                      const float* weight, const float* T, const uint8_t* flags, const float* alphainv_last,
+                                      const int64_t* offsets, const float* g_weight, const float* g_alpha, const float* g_last,
+                                      float* const* grads, int vec_copies, float* gd_scratch, float* vec_scratch, void* stream);
+/* Pass B for a k0 read elsewhere (the k0 of a TensoRF model, read by its own forward on these points): the compacted records of
+ * ubn_march_box_feature_fwd (out_alpha / out_weight may be NULL) and, instead of the feature read, each survivor's point
+ * xyz[M, 3] -- the point sample_pts_on_rays gives that step (render_utils_kernel.cu:185-190). */
+int ubn_march_box_points_fwd(const float* rays_o, const float* rays_d, const UbnBoxMarchCfg* cfg, int64_t n_rays, const uint8_t* flags,
+                             const int64_t* offsets, const float* alpha, const float* weight, float* xyz, float* out_alpha,
+                             float* out_weight, int64_t* ray_id, int64_t* step_id, void* stream);
+
 /* ---- scene bounds (FourierGrid/bbox_compute.py) ------------------------------------------------------------------------------
  * Each call widens bounds = device float[6] (xyz_min then xyz_max; pass +inf / -inf to start empty) IN PLACE: bounds[a] =
  * min(bounds[a], min of the points' axis a), bounds[3+a] likewise with max.  A NaN coordinate makes that bound NaN (torch.minimum

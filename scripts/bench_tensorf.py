@@ -4,11 +4,12 @@
 
 The step is run_train.py:251-288 with bench_dvgo.py's loss weights (entropy_last 1e-3, rgbper 1e-2) and MaskedAdam skipping zero gradients on density and k0, on bench_dvgo.py's object-in-box scene: 384^3 voxel
 budget, density n_comp 8, 12-channel k0 with n_comp 24, width-128 rgbnet, 8192 rays, stepsize 0.5, fast_color_thres 1e-4.
-Legs, alternated in --rounds rounds in this one process: this library's step, and the reference's GPU path (its unmodified
+Legs, alternated in --rounds rounds in this one process: this library's step (forward on the fused box march), the same step
+through the op-by-op composition (DirectVoxGO._compose with the same shading), and the reference's GPU path (its unmodified
 dvgo.py / grid.py / masked_adam.py over its own CUDA build in oracle/_ref; an "unavailable" record when that is absent).
-Reported: step times, CUDA-event times of tensorf_fwd / tensorf_bwd per grid, their algorithmic bytes and FLOPs (from shapes,
-below), the survivor counts, the backward's time at each replicated vector-gradient copy count, and the card's name and power
-limit read in the same run."""
+Reported: step times, CUDA-event times of the march and tensorf kernels, the algorithmic bytes and FLOPs of tensorf_fwd /
+tensorf_bwd (from shapes, below), the survivor counts, the backward's time at each replicated vector-gradient copy count, and
+the card's name and power limit read in the same run."""
 import argparse
 import contextlib
 import io
@@ -129,15 +130,19 @@ def main():
     out['survivors'] = {'density_samples': n_dens, 'k0_samples': int(ret['ray_id'].numel())}
 
     ours = lambda: _time(lambda i: _step(m, m.forward, opt, ro, rd, vd, target, i), args.steps, args.warmup)  # noqa: E731
+    compose_fwd = lambda a, b, c, global_step=None, **rk: m._compose(a, b, c, m._shade_k0, rk)  # noqa: E731
+    compose = lambda: _time(lambda i: _step(m, compose_fwd, opt, ro, rd, vd, target, i), args.steps, args.warmup)  # noqa: E731
     ref_run, why = _reference_leg(state, ro, rd, vd, target, args)
-    legs = {'ours': [], 'reference_gpu': []}
+    legs = {'ours': [], 'compose': [], 'reference_gpu': []}
     for _ in range(args.rounds):
         legs['ours'].append(round(ours(), 3))
+        legs['compose'].append(round(compose(), 3))
         if ref_run is not None:
             legs['reference_gpu'].append(round(ref_run(), 3))
     out['step_ms'] = {k: (v if v else why) for k, v in legs.items()}
     if ref_run is not None:
         out['speedup_median'] = round(float(np.median(legs['reference_gpu']) / np.median(legs['ours'])), 2)
+    out['fused_over_compose_median'] = round(float(np.median(legs['compose']) / np.median(legs['ours'])), 3)
 
     # per-kernel CUDA-event times at each replicated vector-gradient copy count
     per_k = {}
@@ -147,7 +152,7 @@ def main():
         _time(lambda i: _step(m, m.forward, opt, ro, rd, vd, target, i), args.steps, args.warmup)
         s = _cabi.TIMER.summary()
         _cabi.TIMER = None
-        per_k.setdefault(K, []).append({k: round(v[0], 4) for k, v in s.items() if k.startswith('tensorf_bwd')})
+        per_k.setdefault(K, []).append({k: round(v[0], 4) for k, v in s.items() if k.startswith(('tensorf_', 'march_box'))})
     out['kernel_ms_by_vec_copies'] = per_k
     traffic = {'density (c1)': _traffic(m.density, n_dens), 'k0 (c12)': _traffic(m.k0, out['survivors']['k0_samples'])}
     out['algorithmic'] = traffic

@@ -146,6 +146,11 @@ _SIGNATURES = {
     'ubn_tensorf_bwd': [c_p, c_p, ctypes.POINTER(UbnTensorfDesc), c_p, c_i64, c_p, c_p, c_p, c_int, c_p, c_p],
     'ubn_tensorf_tv_add_grad': [c_p, c_p, ctypes.POINTER(UbnTensorfDesc), c_f, c_f, c_f, c_p],
     'ubn_tensorf_dense': [c_p, c_p, ctypes.POINTER(UbnTensorfDesc), c_p, c_p],
+    'ubn_march_box_tensorf_density_fwd': [c_p, c_p, c_p, ctypes.POINTER(UbnTensorfDesc), c_p, ctypes.POINTER(UbnBoxMarchCfg), c_i64,
+                                          c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
+    'ubn_march_box_tensorf_density_bwd': [c_p, c_p, c_p, ctypes.POINTER(UbnTensorfDesc), ctypes.POINTER(UbnBoxMarchCfg), c_i64,
+                                          c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_int, c_p, c_p, c_p],
+    'ubn_march_box_points_fwd': [c_p, c_p, ctypes.POINTER(UbnBoxMarchCfg), c_i64, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
     'ubn_frustum_bounds': [c_p, c_p, c_p, c_i64, c_i64, c_int, c_int, c_int, c_int, c_int, c_f, c_f, c_p, c_p],
     'ubn_lattice_points': [c_p, c_p, c_i64, c_i64, c_i64, c_p, c_p],
     'ubn_lattice_bounds': [c_p, ctypes.POINTER(UbnGridDesc), c_p, c_p, c_i64, c_i64, c_i64, c_f, c_f, c_f, c_p, c_p, c_p],

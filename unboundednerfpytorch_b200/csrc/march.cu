@@ -22,6 +22,7 @@
 #include <type_traits>
 
 #include "march_common.cuh"
+#include "tensorf.cuh"
 
 namespace ubn {
 
@@ -30,15 +31,17 @@ __device__ __forceinline__ float grid_density(const GridView& g, float x, float 
 // ------------------------------------------------------------------------------------------------
 // pass A forward
 // ------------------------------------------------------------------------------------------------
-// kP > 0: compile-time slab count + contiguous single-channel grid -> grid_density_fast (march_common.cuh); kP = 0: generic layout.
-// Smp: the sampling policy (ContractedSampler / NdcSampler, march_common.cuh).
+// kP > 0: compile-time slab count + contiguous single-channel grid -> grid_density_fast (march_common.cuh); kP = 0: generic layout;
+// kP < 0: the TensoRF density tf (C = 1) instead of g, read as ubn_tensorf_fwd reads it (tensorf.cuh's tf_read) with W = -kP
+// components per load (4: 128-bit records, tf_records4).  Smp: the sampling policy (ContractedSampler / NdcSampler / BoxSampler,
+// march_common.cuh).
 template <class Smp, int kP>
 __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_fwd(
     const float* __restrict__ rays_o, const float* __restrict__ rays_d, const float* __restrict__ t_table,
     GridView g, const uint8_t* __restrict__ mask_world, MarchParams p, int64_t n_rays,
     float* __restrict__ o_density, float* __restrict__ o_alpha, float* __restrict__ o_weight,
     float* __restrict__ o_T, uint8_t* __restrict__ o_flags, float* __restrict__ o_last,
-    int32_t* __restrict__ o_nkeep) {
+    int32_t* __restrict__ o_nkeep, TfView tf) {
   const int lane = threadIdx.x & 31;
   const int64_t ray = (int64_t)blockIdx.x * kMarchWarps + (threadIdx.x >> 5);
   if (ray >= n_rays) return;
@@ -97,7 +100,12 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_fwd(
 
     float dens = 0.f, alpha = 0.f;
     if (queried) {
-      dens = kP > 0 ? grid_density_fast<(kP > 0 ? kP : 1)>(g, x, y, z) : grid_density(g, x, y, z);
+      if constexpr (kP < 0) {
+        const float c[3] = {tf_coord(tf, 0, x), tf_coord(tf, 1, y), tf_coord(tf, 2, z)};
+        tf_read<1, -kP>(tf, c, nullptr, &dens);
+      } else {
+        dens = kP > 0 ? grid_density_fast<(kP > 0 ? kP : 1)>(g, x, y, z) : grid_density(g, x, y, z);
+      }
       dens = Smp::density(p, dens, x, y, z);
       const float e = expf(dens + p.shift);
       alpha = 1 - powf(1 + e, -p.interval);
@@ -439,6 +447,29 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_scatter(
   if (rb.v >= 0) flush(rb, slab_b);
 }
 
+// Launch 2 of the TensoRF density's backward.  Launch 1 (k_march_density_bwd<BoxSampler, 1, true>, the dense grid's launch 1) left
+// every sample's density gradient in gd_in[ray * S + s].  Warp = ray, lane = every 32nd step of the ray's own n_steps: a record
+// with a nonzero gradient recomputes its point from (ray, step) and runs the per-sample adjoint of ubn_tensorf_bwd (tensorf.cuh's
+// tf_sample_bwd): plane gradients reduced straight into grads, vector gradients into copy blockIdx % vec_copies.
+template <int W>
+__global__ void __launch_bounds__(32 * kMarchWarps) k_march_box_tensorf_scatter(
+    const float* __restrict__ rays_o, const float* __restrict__ rays_d, TfView t, MarchParams p, int64_t n_rays,
+    const float* __restrict__ gd_in, TfGrads gr, float* __restrict__ vcopies, int64_t copy_len, int vec_copies) {
+  const int64_t ray = (int64_t)blockIdx.x * kMarchWarps + (threadIdx.x >> 5);
+  if (ray >= n_rays) return;
+  const Ray r = BoxSampler::load(rays_o + 3 * ray, rays_d + 3 * ray, p);
+  float* vc = vcopies + (int64_t)(blockIdx.x % vec_copies) * copy_len;
+  for (int s = threadIdx.x & 31; s < r.n; s += 32) {
+    const float gd = gd_in[ray * p.S + s];
+    if (gd == 0.f) continue;
+    float x, y, z;
+    bool inner;
+    BoxSampler::point(r, nullptr, s, p, x, y, z, inner);
+    const float c[3] = {tf_coord(t, 0, x), tf_coord(t, 1, y), tf_coord(t, 2, z)};
+    tf_sample_bwd<1, W>(t, c, &gd, nullptr, nullptr, 0, gr, vc);
+  }
+}
+
 // the fast density paths need: contiguous single channel, >= 2 voxels per axis, 32-bit offsets inside a slab, and an 8-byte aligned
 // buffer (the pair reductions align on the ADDRESS, so odd-sized slabs -- 153^3 -- are fine: the +0 half of a pair may fall on the
 // last voxel of the previous slab, never before the buffer)
@@ -475,7 +506,7 @@ static int launch_density_fwd(const float* rays_o, const float* rays_d, const fl
                               float* weight, float* T, uint8_t* flags, float* alphainv_last, int32_t* n_keep, cudaStream_t st) {
 #define UBN_DFWD(P)                                                                                              \
   k_march_density_fwd<Smp, P><<<blocks_for(n_rays, kMarchWarps), 32 * kMarchWarps, 0, st>>>(                   \
-      rays_o, rays_d, t_table, g, mask_world, p, n_rays, density, alpha, weight, T, flags, alphainv_last, n_keep)
+      rays_o, rays_d, t_table, g, mask_world, p, n_rays, density, alpha, weight, T, flags, alphainv_last, n_keep, TfView{})
   if constexpr (std::is_same<Smp, BoxSampler>::value) {      // DVGO's density: one contiguous slab, the fast path only
     if (density_fast_slabs(g) != 1) return finish(cudaErrorInvalidValue);
     UBN_DFWD(1);
@@ -721,6 +752,63 @@ int ubn_march_box_density_bwd(const float* rays_o, const float* rays_d, const Ub
   return launch_density_bwd<BoxSampler>(rays_o, rays_d, nullptr, g, p, n_rays, density, alpha, weight, T, flags, alphainv_last,
                                         offsets, g_weight, g_alpha, nullptr, g_last, grad_density_grid, gd_scratch,
                                         as_stream(stream));
+}
+
+int ubn_march_box_tensorf_density_fwd(const float* rays_o, const float* rays_d, const float* const* factors, const UbnTensorfDesc* desc,
+                                      const uint8_t* mask_world, const UbnBoxMarchCfg* cfg, int64_t n_rays, float* density,
+                                      float* alpha, float* weight, float* T, uint8_t* flags, float* alphainv_last, int32_t* n_keep,
+                                      int32_t* overflow, void* stream) {
+  if (n_rays <= 0) return 0;
+  TfView t;
+  if (!make_tf_view(factors, desc, t) || t.C != 1 || !box_cfg_ok(cfg) || !overflow) return finish(cudaErrorInvalidValue);
+  const MarchParams p = make_box_params(cfg, overflow);
+  if (p.use_mask && !mask_world) return finish(cudaErrorInvalidValue);
+  const unsigned blocks = blocks_for(n_rays, kMarchWarps);
+  const cudaStream_t st = as_stream(stream);
+  const GridView none{};
+  if (tf_records4(t, nullptr))
+    k_march_density_fwd<BoxSampler, -4><<<blocks, 32 * kMarchWarps, 0, st>>>(rays_o, rays_d, nullptr, none, mask_world, p, n_rays,
+                                                                            density, alpha, weight, T, flags, alphainv_last, n_keep, t);
+  else
+    k_march_density_fwd<BoxSampler, -1><<<blocks, 32 * kMarchWarps, 0, st>>>(rays_o, rays_d, nullptr, none, mask_world, p, n_rays,
+                                                                            density, alpha, weight, T, flags, alphainv_last, n_keep, t);
+  UBN_LAUNCH_CHECK();
+  return 0;
+}
+
+int ubn_march_box_tensorf_density_bwd(const float* rays_o, const float* rays_d, const float* const* factors, const UbnTensorfDesc* desc,
+                                      const UbnBoxMarchCfg* cfg, int64_t n_rays, const float* density, const float* alpha,
+                                      const float* weight, const float* T, const uint8_t* flags, const float* alphainv_last,
+                                      const int64_t* offsets, const float* g_weight, const float* g_alpha, const float* g_last,
+                                      float* const* grads, int vec_copies, float* gd_scratch, float* vec_scratch, void* stream) {
+  if (n_rays <= 0) return 0;
+  TfView t;
+  TfGrads gr;
+  if (!make_tf_view(factors, desc, t) || t.C != 1 || !make_tf_grads(grads, gr) || !box_cfg_ok(cfg) || !gd_scratch || !vec_scratch ||
+      !aligned16(vec_scratch) || vec_copies < 1 || vec_copies > 64)
+    return finish(cudaErrorInvalidValue);
+  const MarchParams p = make_box_params(cfg, nullptr);
+  const cudaStream_t st = as_stream(stream);
+  const unsigned blocks = blocks_for(n_rays, kMarchWarps);
+  const int64_t copy_len = tf_copy_len(t);
+  const cudaError_t e = cudaMemsetAsync(vec_scratch, 0, (size_t)vec_copies * copy_len * sizeof(float), st);
+  if (e != cudaSuccess) return finish(e);
+  GridView g{};     // launch 1 reads only the slab count
+  g.P = 1;
+  k_march_density_bwd<BoxSampler, 1, true><<<blocks, 32 * kMarchWarps, 0, st>>>(
+      rays_o, rays_d, nullptr, g, p, n_rays, density, alpha, weight, T, flags, alphainv_last, offsets, g_weight, g_alpha, nullptr,
+      g_last, nullptr, gd_scratch);
+  UBN_LAUNCH_CHECK();
+  if (tf_records4(t, grads))
+    k_march_box_tensorf_scatter<4><<<blocks, 32 * kMarchWarps, 0, st>>>(rays_o, rays_d, t, p, n_rays, gd_scratch, gr, vec_scratch,
+                                                                        copy_len, vec_copies);
+  else
+    k_march_box_tensorf_scatter<1><<<blocks, 32 * kMarchWarps, 0, st>>>(rays_o, rays_d, t, p, n_rays, gd_scratch, gr, vec_scratch,
+                                                                        copy_len, vec_copies);
+  UBN_LAUNCH_CHECK();
+  k_tensorf_bwd_finish<<<blocks_for(copy_len, 256), 256, 0, st>>>(t, gr, vec_scratch, copy_len, vec_copies, nullptr, 0, 0, nullptr);
+  UBN_LAUNCH_CHECK();
+  return 0;
 }
 
 }  // extern "C"

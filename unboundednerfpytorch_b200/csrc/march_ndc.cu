@@ -113,6 +113,44 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_ndc_feature(
   }
 }
 
+// Pass B of the box march for a k0 read elsewhere (the k0 of a TensoRF model, read by its own forward): the compacted records
+// alpha, weight, ray_id, step_id and the survivor's point xyz[M, 3] -- box_point, the point ubn_sample_pts_* give the same step --
+// in place of the feature read.
+__global__ void __launch_bounds__(32 * kMarchWarps) k_march_box_points(
+    const float* __restrict__ rays_o, const float* __restrict__ rays_d, MarchParams p, int64_t n_rays,
+    const uint8_t* __restrict__ flags, const int64_t* __restrict__ offsets, const float* __restrict__ alpha,
+    const float* __restrict__ weight, float* __restrict__ xyz, float* __restrict__ o_alpha, float* __restrict__ o_weight,
+    int64_t* __restrict__ o_ray_id, int64_t* __restrict__ o_step_id) {
+  const int lane = threadIdx.x & 31;
+  const int64_t ray = (int64_t)blockIdx.x * kMarchWarps + (threadIdx.x >> 5);
+  if (ray >= n_rays) return;
+  int64_t out_base = offsets[ray];
+  const int64_t out_end = offsets[ray + 1];
+  if (out_base == out_end) return;
+  const Ray r = BoxSampler::load(rays_o + 3 * ray, rays_d + 3 * ray, p);
+  for (int base = 0; base < r.n && out_base < out_end; base += 32) {
+    const int s = base + lane;
+    const uint8_t f = (s < r.n) ? flags[ray * p.S + s] : 0;
+    const bool keep = (f & UBN_FLAG_KEEP) != 0;
+    const unsigned km = __ballot_sync(0xffffffffu, keep);
+    if (keep) {
+      const int64_t row = out_base + __popc(km & ((1u << lane) - 1));
+      float x, y, z;
+      bool inner;
+      BoxSampler::point(r, nullptr, s, p, x, y, z, inner);
+      xyz[3 * row] = x;
+      xyz[3 * row + 1] = y;
+      xyz[3 * row + 2] = z;
+      const int64_t i = ray * p.S + s;
+      if (o_alpha) o_alpha[row] = alpha[i];
+      if (o_weight) o_weight[row] = weight[i];
+      o_ray_id[row] = ray;
+      o_step_id[row] = s;
+    }
+    out_base += __popc(km);
+  }
+}
+
 // single slab, channels-last, C in {3, 9}, >= 2 voxels per axis (pre-clamped cells), 32-bit voxel index (make_cell), 4-byte aligned
 static bool ndc_feature_grid_ok(const GridView& g) {
   return g.P == 1 && g.sc == 1 && g.sv == g.C && (g.C == 3 || g.C == 9) && g.X >= 2 && g.Y >= 2 && g.Z >= 2 &&
@@ -200,6 +238,18 @@ int ubn_march_box_feature_bwd(const float* rays_o, const float* rays_d, const Ub
   return launch_ndc_feature<BoxSampler, true>(rays_o, rays_d, g, p, n_rays, flags, offsets, nullptr, nullptr,
                                               const_cast<float*>(grad_feat), grad_k0, nullptr, nullptr, nullptr, nullptr,
                                               as_stream(stream));
+}
+
+int ubn_march_box_points_fwd(const float* rays_o, const float* rays_d, const UbnBoxMarchCfg* cfg, int64_t n_rays, const uint8_t* flags,
+                             const int64_t* offsets, const float* alpha, const float* weight, float* xyz, float* out_alpha,
+                             float* out_weight, int64_t* ray_id, int64_t* step_id, void* stream) {
+  if (n_rays <= 0) return 0;
+  if (cfg->s_max < 1 || (out_alpha && !alpha) || (out_weight && !weight)) return finish(cudaErrorInvalidValue);
+  const MarchParams p = make_box_params(cfg, nullptr);
+  k_march_box_points<<<blocks_for(n_rays, kMarchWarps), 32 * kMarchWarps, 0, as_stream(stream)>>>(
+      rays_o, rays_d, p, n_rays, flags, offsets, alpha, weight, xyz, out_alpha, out_weight, ray_id, step_id);
+  UBN_LAUNCH_CHECK();
+  return 0;
 }
 
 }  // extern "C"

@@ -1,9 +1,9 @@
 """Fused ray march (autograd.Function) over the C ABI: the hot path of FourierGridModel.forward
 (FourierGrid_model.py:554-621) and DirectContractedVoxGO.forward (dcvgo.py:264-331) -- ``March`` -- and of
-DirectMPIGO.forward (dmpigo.py:251-295) -- ``NdcMarch`` -- and of DirectVoxGO.forward (dvgo.py:330-366) -- ``BoxMarch`` --
-up to and including the feature-grid read, in 3 launches forward (pass A, scan, pass B) and 2 backward.  All three run the one
-forward body and the one backward body below (_forward / _backward); a geometry record (_Contracted, _Ndc, _Box) binds them
-to the C entries of its sampling policy.
+DirectMPIGO.forward (dmpigo.py:251-295) -- ``NdcMarch`` -- and of DirectVoxGO.forward (dvgo.py:330-366) -- ``BoxMarch``, and
+``BoxTensorfMarch`` with TensoRF grids -- up to and including the feature-grid read, in 3 launches forward (pass A, scan, pass B)
+and 2 backward.  All of them run the one forward body and the one backward body below (_forward / _backward); a geometry record
+(_Contracted, _Ndc, _Box, _BoxTensorf) binds them to the C entries of its sampling policy and density.
 """
 import functools
 import os
@@ -12,8 +12,8 @@ import numpy as np
 import torch
 
 from . import _cabi, ops
-from ._cabi import UbnMarchCfg, UbnNdcMarchCfg, c_i64, check, ptr, stream_of
-from .grid import grid_desc
+from ._cabi import UbnMarchCfg, UbnNdcMarchCfg, c_i64, c_int, check, ptr, stream_of
+from .grid import _factor_array, grid_desc
 
 
 @functools.lru_cache(maxsize=64)
@@ -132,6 +132,23 @@ class _Geometry:
             check(getattr(lib, f'ubn_{self.entry}_feature_fwd')(*head, ptr(alpha), ptr(weight), *map(ptr, out), st))
         return (), ()
 
+    def saved_density(self, density):
+        """Density tensors the backward reads (saved with save_for_backward, so an in-place change before it raises): none."""
+        return ()
+
+    def density_fwd(self, lib, rays, density, ddesc, mask_world, cfg, N, records, tail, st):
+        """Pass A on the density tensors (one grid here)."""
+        with _cabi.timed(self.entry + '_density_fwd'):
+            check(getattr(lib, f'ubn_{self.entry}_density_fwd')(*rays, ptr(density[0]), ddesc, *self.shift, ptr(mask_world), cfg,
+                                                                  c_i64(N), *map(ptr, records), *map(ptr, tail), st))
+
+    def density_bwd(self, lib, ctx, rays, N, args, grads, gd, st):
+        """The density's reverse scan and scatter, adding into grads (one per density tensor); args = the pass A records, the
+        offsets and the output gradients, in the C entry's order."""
+        with _cabi.timed(self.entry + '_density_bwd'):
+            check(getattr(lib, f'ubn_{self.entry}_density_bwd')(*rays, ctx.ddesc, ctx.cfg, c_i64(N), *map(ptr, (*args, grads[0], gd)),
+                                                                  st))
+
 
 class _Contracted(_Geometry):
     """Every entry takes the t table; pass B also writes raw_density, t and the inner-sphere flag, and on the render path may
@@ -161,10 +178,12 @@ class _Contracted(_Geometry):
         return (o_dens,), (o_t, o_inner)
 
 
-def _forward(ctx, geo, density_grid, k0_grid, rays_o, rays_d, mask_world, cfg, ddesc, kdesc):
+def _forward(ctx, geo, density, k0_grid, rays_o, rays_d, mask_world, cfg, ddesc, kdesc, d_at=(0,), k_at=1):
     """Pass A (dense per-sample records), the exclusive scan of the per-ray survivor counts, pass B (compacted records and the
-    feature read).  Returns (weights[M], alphainv_last[N], raw_alpha[M], *geometry outputs with a gradient, k0_feat[M,C],
-    ray_id[M] i64, step_id[M] i64, *constant geometry outputs)."""
+    feature read).  density: the density tensors (a grid, or the six TensoRF factors), at the Function's inputs d_at; k0_grid at
+    input k_at, or None (k_at None) when pass B writes the survivor points instead of reading a k0.  Returns (weights[M], alphainv_last[N],
+    raw_alpha[M], *geometry outputs with a gradient, k0_feat[M,C] (or points[M,3]), ray_id[M] i64, step_id[M] i64, *constant
+    geometry outputs)."""
     dev = rays_o.device
     rays_o = rays_o.contiguous().float()
     rays_d = rays_d.contiguous().float()
@@ -176,32 +195,32 @@ def _forward(ctx, geo, density_grid, k0_grid, rays_o, rays_d, mask_world, cfg, d
     with ops._Guard(rays_o) as lib:
         st = stream_of(rays_o)
         rays = (ptr(rays_o), ptr(rays_d), *map(ptr, geo.lead))
-        with _cabi.timed(geo.entry + '_density_fwd'):
-            check(getattr(lib, f'ubn_{geo.entry}_density_fwd')(*rays, ptr(density_grid), ddesc, *geo.shift, ptr(mask_world), cfg,
-                                                                 c_i64(N), *map(ptr, records), *map(ptr, tail), st))
+        geo.density_fwd(lib, rays, density, ddesc, mask_world, cfg, N, records, tail, st)
         offsets = torch.empty(N + 1, dtype=torch.int64, device=dev)
         scratch = torch.empty(N // 1024 + 4, dtype=torch.int64, device=dev)
         check(lib.ubn_exclusive_scan_i32(ptr(nkeep), c_i64(N), ptr(offsets), ptr(scratch), st))
         M = geo.survivors(offsets, tail, N, S)
-        out = (torch.empty(M, k0_grid.shape[1], **f32), torch.empty(M, **f32), torch.empty(M, **f32),
+        out = (torch.empty(M, k0_grid.shape[1] if k0_grid is not None else 3, **f32), torch.empty(M, **f32), torch.empty(M, **f32),
                torch.empty(M, dtype=torch.int64, device=dev), torch.empty(M, dtype=torch.int64, device=dev))
         feat, o_alpha, o_weight, ray_id, step_id = out
         head = (*rays, ptr(k0_grid), kdesc, cfg, c_i64(N), ptr(flags), ptr(offsets))
         differentiable, constant = geo.pass_b(lib, head, k0_grid, dens, alpha, weight, out, st)
-    ctx.save_for_backward(rays_o, rays_d, dens, alpha, weight, T, flags, last, offsets)
+    ctx.save_for_backward(rays_o, rays_d, dens, alpha, weight, T, flags, last, offsets, *geo.saved_density(density))
     ctx.geo, ctx.cfg, ctx.ddesc, ctx.kdesc = geo, cfg, ddesc, kdesc
     ctx.n_extra = len(differentiable)
-    ctx.dmeta = (density_grid.shape, density_grid.stride())
-    ctx.kmeta = (k0_grid.shape, k0_grid.stride())
-    ctx.dparam, ctx.kparam = density_grid, k0_grid      # for their persistent gradient buffers (_grad_target)
-    ctx.mark_non_differentiable(ray_id, step_id, *constant)
+    ctx.dmeta = [(t.shape, t.stride()) for t in density]
+    ctx.kmeta = (k0_grid.shape, k0_grid.stride()) if k0_grid is not None else None
+    ctx.dparam, ctx.kparam = density, k0_grid      # for their persistent gradient buffers (_grad_target)
+    ctx.d_at, ctx.k_at = d_at, k_at
+    ctx.mark_non_differentiable(ray_id, step_id, *constant, *((feat,) if k0_grid is None else ()))
     return (o_weight, last, o_alpha, *differentiable, feat, ray_id, step_id, *constant)
 
 
 @torch.autograd.function.once_differentiable
 def _backward(ctx, g_weight, g_last, g_alpha, *rest):
-    """The k0 scatter, then the density reverse scan and scatter.  Gradients for (density_grid, k0_grid), None for the rest."""
-    rays_o, rays_d, dens, alpha, weight, T, flags, last, offsets = ctx.saved_tensors
+    """The k0 scatter, then the density reverse scan and scatter.  Gradients for the density tensors and k0_grid, None for the
+    rest."""
+    rays_o, rays_d, dens, alpha, weight, T, flags, last, offsets = ctx.saved_tensors[:9]
     geo = ctx.geo
     dev = rays_o.device
     N = rays_o.shape[0]
@@ -211,21 +230,24 @@ def _backward(ctx, g_weight, g_last, g_alpha, *rest):
     with ops._Guard(rays_o) as lib:
         st = stream_of(rays_o)
         rays = (ptr(rays_o), ptr(rays_d), *map(ptr, geo.lead))
-        want_k = ctx.needs_input_grad[1] and g_feat is not None
-        want_d = ctx.needs_input_grad[0]
-        grad_d, buf_d = _grad_target(ctx.dparam, ctx.dmeta, want_d, dev)
+        want_k = ctx.k_at is not None and ctx.needs_input_grad[ctx.k_at] and g_feat is not None
+        want_d = any(ctx.needs_input_grad[i] for i in ctx.d_at)
+        targets_d = [_grad_target(p, m, want_d, dev) for p, m in zip(ctx.dparam, ctx.dmeta)]
         grad_k, buf_k = _grad_target(ctx.kparam, ctx.kmeta, want_k, dev)
         if want_k:
             with _cabi.timed(geo.entry + '_feature_bwd'):
                 check(getattr(lib, f'ubn_{geo.entry}_feature_bwd')(*rays, ctx.kdesc, ctx.cfg, c_i64(N), ptr(flags), ptr(offsets),
                                                                      ptr(g_feat), ptr(grad_k), st))
         if want_d:
-            gd = torch.empty_like(dens)     # per-sample density gradients between the run scatter's two launches
-            with _cabi.timed(geo.entry + '_density_bwd'):
-                check(getattr(lib, f'ubn_{geo.entry}_density_bwd')(*rays, ctx.ddesc, ctx.cfg, c_i64(N), *map(ptr, (
-                    dens, alpha, weight, T, flags, last, offsets, g_weight, g_alpha, *g_extra, g_last, grad_d, gd)), st))
-    grads = (_hand_over(ctx.dparam, grad_d, buf_d), _hand_over(ctx.kparam, grad_k, buf_k))
-    return grads + (None,) * (len(ctx.needs_input_grad) - 2)
+            gd = torch.empty_like(dens)     # per-sample density gradients between the backward's two launches
+            geo.density_bwd(lib, ctx, rays, N, (dens, alpha, weight, T, flags, last, offsets, g_weight, g_alpha, *g_extra, g_last),
+                            [g for g, _ in targets_d], gd, st)
+    grads = [None] * len(ctx.needs_input_grad)
+    for i, p, (g, buf) in zip(ctx.d_at, ctx.dparam, targets_d):
+        grads[i] = _hand_over(p, g, buf)
+    if ctx.k_at is not None:
+        grads[ctx.k_at] = _hand_over(ctx.kparam, grad_k, buf_k)
+    return tuple(grads)
 
 
 class March(torch.autograd.Function):
@@ -238,7 +260,7 @@ class March(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, density_grid, k0_grid, rays_o, rays_d, t_table, mask_world, cfg, ddesc, kdesc, dense_known, coherent=False):
-        return _forward(ctx, _Contracted(t_table, dense_known, coherent), density_grid, k0_grid, rays_o, rays_d, mask_world, cfg,
+        return _forward(ctx, _Contracted(t_table, dense_known, coherent), (density_grid,), k0_grid, rays_o, rays_d, mask_world, cfg,
                         ddesc, kdesc)
 
     backward = staticmethod(_backward)
@@ -274,7 +296,7 @@ class NdcMarch(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, density_grid, k0_grid, act_shift_grid, rays_o, rays_d, mask_world, cfg, ddesc, kdesc, sdesc):
-        return _forward(ctx, _Ndc(act_shift_grid, sdesc), density_grid, k0_grid, rays_o, rays_d, mask_world, cfg, ddesc, kdesc)
+        return _forward(ctx, _Ndc(act_shift_grid, sdesc), (density_grid,), k0_grid, rays_o, rays_d, mask_world, cfg, ddesc, kdesc)
 
     backward = staticmethod(_backward)
 
@@ -309,13 +331,8 @@ def make_box_cfg(xyz_min, xyz_max, near, stepdist, act_shift, interval, fast_col
 
 
 def box_supported(density_grid, k0_grid):
-    """Grids the fused box march covers: a contiguous single-slab density grid and a single-slab channels-last k0 with 3 or 12
-    channels (16-byte aligned records for 12), >= 2 voxels per axis, 32-bit voxel offsets."""
-    return (density_grid.is_cuda and k0_grid.is_cuda and density_grid.dim() == 5 and density_grid.shape[:2] == (1, 1)
-            and density_grid.is_contiguous() and min(density_grid.shape[2:]) >= 2 and density_grid.numel() < 2 ** 31
-            and k0_grid.dim() == 5 and k0_grid.shape[0] == 1 and k0_grid.shape[1] in (3, 12) and k0_grid.stride(1) == 1
-            and k0_grid.stride(4) == k0_grid.shape[1] and min(k0_grid.shape[2:]) >= 2 and k0_grid[0, 0].numel() < 2 ** 31
-            and (k0_grid.shape[1] != 12 or k0_grid.data_ptr() % 16 == 0))
+    """Grids the fused box march covers: box_density_supported and box_k0_supported."""
+    return box_density_supported(density_grid) and box_k0_supported(k0_grid)
 
 
 class _Box(_Geometry):
@@ -344,6 +361,73 @@ class BoxMarch(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, density_grid, k0_grid, rays_o, rays_d, mask_world, cfg, ddesc, kdesc):
-        return _forward(ctx, _Box(), density_grid, k0_grid, rays_o, rays_d, mask_world, cfg, ddesc, kdesc)
+        return _forward(ctx, _Box(), (density_grid,), k0_grid, rays_o, rays_d, mask_world, cfg, ddesc, kdesc)
+
+    backward = staticmethod(_backward)
+
+
+def box_density_supported(density_grid):
+    """Density grids the box march's pass A reads: contiguous single slab, one channel, >= 2 voxels per axis, 32-bit offsets."""
+    return (density_grid.is_cuda and density_grid.dim() == 5 and density_grid.shape[:2] == (1, 1) and density_grid.is_contiguous()
+            and min(density_grid.shape[2:]) >= 2 and density_grid.numel() < 2 ** 31)
+
+
+def box_k0_supported(k0_grid):
+    """k0 grids the box march's pass B reads: single slab, channels-last, 3 or 12 channels (16-byte aligned records for 12),
+    >= 2 voxels per axis, 32-bit voxel offsets."""
+    return (k0_grid.is_cuda and k0_grid.dim() == 5 and k0_grid.shape[0] == 1 and k0_grid.shape[1] in (3, 12)
+            and k0_grid.stride(1) == 1 and k0_grid.stride(4) == k0_grid.shape[1] and min(k0_grid.shape[2:]) >= 2
+            and k0_grid[0, 0].numel() < 2 ** 31 and (k0_grid.shape[1] != 12 or k0_grid.data_ptr() % 16 == 0))
+
+
+def tensorf_supported(factors):
+    """TensoRF grids the box march reads: CUDA factors with R + R + Rxy <= 96 (one grad_f_vec row per thread of the backward)."""
+    return all(t.is_cuda for t in factors) and 2 * factors[1].shape[1] + factors[0].shape[1] <= 96
+
+
+class _BoxTensorf(_Box):
+    """The box march for TensoRF models: pass A reads the density -- the six TensoRF factors (its backward adds into their
+    gradients through vec_copies replicated vector copies) or a dense grid -- and pass B writes the survivor points, which the
+    model's own k0 reads."""
+
+    def __init__(self, tensorf_density, vec_copies):
+        self.tensorf_density, self.vec_copies = tensorf_density, vec_copies
+
+    def saved_density(self, density):
+        return tuple(density) if self.tensorf_density else ()      # the adjoint multiplies plane values by line values
+
+    def density_fwd(self, lib, rays, density, ddesc, mask_world, cfg, N, records, tail, st):
+        if not self.tensorf_density:
+            return super().density_fwd(lib, rays, density, ddesc, mask_world, cfg, N, records, tail, st)
+        with _cabi.timed('march_box_tensorf_density_fwd'):
+            check(lib.ubn_march_box_tensorf_density_fwd(*rays, _factor_array(density), ddesc, ptr(mask_world), cfg, c_i64(N),
+                                                        *map(ptr, records), *map(ptr, tail), st))
+
+    def density_bwd(self, lib, ctx, rays, N, args, grads, gd, st):
+        if not self.tensorf_density:
+            return super().density_bwd(lib, ctx, rays, N, args, grads, gd, st)
+        d, K = ctx.ddesc, self.vec_copies
+        vec = torch.empty(K * (d.X * d.R + d.Y * d.R + d.Z * d.Rxy), dtype=torch.float32, device=gd.device)
+        with _cabi.timed('march_box_tensorf_density_bwd'):
+            check(lib.ubn_march_box_tensorf_density_bwd(*rays, _factor_array(ctx.saved_tensors[9:]), d, ctx.cfg, c_i64(N),
+                                                        *map(ptr, args), _factor_array(grads), c_int(K), ptr(gd), ptr(vec), st))
+
+    def pass_b(self, lib, head, k0_grid, dens, alpha, weight, out, st):
+        rays_o, rays_d, _, _, cfg, N, flags, offsets = head
+        with _cabi.timed('march_box_points_fwd'):
+            check(lib.ubn_march_box_points_fwd(rays_o, rays_d, cfg, N, flags, offsets, ptr(alpha), ptr(weight), *map(ptr, out), st))
+        return (), ()
+
+
+class BoxTensorfMarch(torch.autograd.Function):
+    """DirectVoxGO's march for TensoRF models: the inputs it differentiates are the density tensors -- the six TensoRF factors
+    (tensorf_density) or the dense density grid.  Returns (weights[M], alphainv_last[N], raw_alpha[M], points[M, 3], ray_id[M]
+    i64, step_id[M] i64): pass B writes each survivor's point (no gradient) where BoxMarch returns its k0 features, for the
+    model's k0 -- TensoRFGrid or DenseGrid -- to read with its own forward.  A ray needing more than cfg.s_max steps raises."""
+
+    @staticmethod
+    def forward(ctx, rays_o, rays_d, mask_world, cfg, ddesc, tensorf_density, vec_copies, *density):
+        return _forward(ctx, _BoxTensorf(tensorf_density, vec_copies), density, None, rays_o, rays_d, mask_world, cfg, ddesc, None,
+                        d_at=tuple(range(7, 7 + len(density))), k_at=None)
 
     backward = staticmethod(_backward)

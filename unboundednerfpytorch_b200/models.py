@@ -607,7 +607,10 @@ class DirectVoxGO(_CoarseGeo, _GridModel):
     rgbnet_direct=False the march is fused and the torch epilogue sigmoid(rgbnet(cat[k0[:, 3:], emb]) + k0[:, :3]) stays.
     ``forward_ops`` composes the drop-in ops in the reference's order (the cross-check and the path for other grids).  With a
     TensoRFGrid density or k0 (``density_type`` / ``k0_type``, built through ``grid.create_grid`` as dvgo.py does) ``forward`` runs
-    that composition on the TensoRF kernels and shades with ``_shade``, since the fused march reads dense grids only.
+    the same fused box march (march.BoxTensorfMarch) in all three pairings: pass A reads a TensoRF density's factors (or the
+    dense grid), pass B writes the survivor points, and the k0 reads them with its own forward.  Its outputs are bit-identical
+    to that composition on the TensoRF kernels shaded with ``_shade``, which stays the route where the march does not apply
+    (R + R + Rxy > 96, S_max beyond the march's bound, host tensors).
 
     The coarse-to-fine schedule of run_train.py works: maskout_near_cam_vox, voxel_count_views (per-voxel lr), scale_volume_grid,
     update_occupancy_cache, and ``mask_cache_path``.  The latter builds the fine mask as the reference does (dvgo.py:138-152):
@@ -748,7 +751,11 @@ class DirectVoxGO(_CoarseGeo, _GridModel):
         return isinstance(self.density, G.TensoRFGrid) or isinstance(self.k0, G.TensoRFGrid)
 
     def _fused_ok(self, stepsize):
-        if self._tensorf() or not march.box_supported(self.density.grid, self.k0.grid):
+        tf_d, tf_k = isinstance(self.density, G.TensoRFGrid), isinstance(self.k0, G.TensoRFGrid)
+        d_ok = march.tensorf_supported(self.density.factors()) if tf_d else march.box_density_supported(self.density.grid)
+        # a TensoRF model's k0 reads the survivor points with its own forward: any DenseGrid k0 will do next to a TensoRF density
+        k_ok = march.tensorf_supported(self.k0.factors()) if tf_k else (tf_d or march.box_k0_supported(self.k0.grid))
+        if not (d_ok and k_ok):
             return False
         lo, hi = self._host()
         return march.box_s_max(lo, hi, self._stepdist(stepsize)) <= march.BOX_S_MAX_LIMIT
@@ -761,10 +768,9 @@ class DirectVoxGO(_CoarseGeo, _GridModel):
         """dvgo.py:330-397 on the fused box march (see the class docstring); same keys as the reference's ret_dict."""
         assert len(rays_o.shape) == 2 and rays_o.shape[-1] == 3, 'Only suuport point queries in [N, 3] format'
         stepsize = render_kwargs['stepsize']
-        if self._tensorf():
-            # the fused march reads dense grids only: the op-by-op composition with the TensoRF kernels, shaded as the march is
-            return self._compose(rays_o, rays_d, viewdirs, self._shade_k0, render_kwargs)
         if not (rays_o.is_cuda and self._fused_ok(stepsize)):
+            if self._tensorf():     # the op-by-op composition on the TensoRF kernels, shaded as the march is
+                return self._compose(rays_o, rays_d, viewdirs, self._shade_k0, render_kwargs)
             return self.forward_ops(rays_o, rays_d, viewdirs, global_step=global_step, **render_kwargs)
         if self._pending_mask is not None:
             self._resolve_mask_cache()
@@ -773,12 +779,29 @@ class DirectVoxGO(_CoarseGeo, _GridModel):
         cfg = march.make_box_cfg(lo, hi, render_kwargs['near'], self._stepdist(stepsize), host_scalar(self.act_shift),
                                  stepsize * host_scalar(self.voxel_size_ratio), self.fast_color_thres, self.mask_cache.mask, mscale,
                                  mshift)
-        ddesc = G.grid_desc(self.density.grid, *self.density._bounds(), 0)
-        kdesc = G.grid_desc(self.k0.grid, *self.k0._bounds(), 0)
-        weights, alphainv_last, alpha, k0, ray_id, step_id = march.BoxMarch.apply(
-            self.density.grid, self.k0.grid, rays_o, rays_d, self.mask_cache.mask, cfg, ddesc, kdesc)
+        if self._tensorf():
+            weights, alphainv_last, alpha, k0, ray_id, step_id = self._march_tensorf(rays_o, rays_d, cfg)
+        else:
+            ddesc = G.grid_desc(self.density.grid, *self.density._bounds(), 0)
+            kdesc = G.grid_desc(self.k0.grid, *self.k0._bounds(), 0)
+            weights, alphainv_last, alpha, k0, ray_id, step_id = march.BoxMarch.apply(
+                self.density.grid, self.k0.grid, rays_o, rays_d, self.mask_cache.mask, cfg, ddesc, kdesc)
         rgb = self._shade_k0(k0, viewdirs, ray_id)
         return self._finish(N, weights, alphainv_last, alpha, rgb, ray_id, step_id, render_kwargs)
+
+    def _march_tensorf(self, rays_o, rays_d, cfg):
+        """march.BoxTensorfMarch: a TensoRF density is read in pass A; the k0 (TensoRFGrid or DenseGrid) reads the survivor
+        points pass B writes with its own forward and autograd -- the very read _compose runs on the same points."""
+        if isinstance(self.density, G.TensoRFGrid):
+            density = self.density.factors()
+            ddesc = G.tensorf_desc(density, 1, *self.density._bounds())
+        else:
+            density = [self.density.grid]
+            ddesc = G.grid_desc(self.density.grid, *self.density._bounds(), 0)
+        weights, alphainv_last, alpha, points, ray_id, step_id = march.BoxTensorfMarch.apply(
+            rays_o, rays_d, self.mask_cache.mask, cfg, ddesc, isinstance(self.density, G.TensoRFGrid), G.TENSORF_VEC_COPIES,
+            *density)
+        return weights, alphainv_last, alpha, self.k0(points), ray_id, step_id
 
     def _shade_k0(self, k0, viewdirs, ray_id):
         """rgb of the samples as forward computes it: _shade (the tensor-core rgbnet where shade.supported); with
