@@ -300,6 +300,14 @@ typedef struct UbnMarchCfg {
 #define UBN_FLAG_KEEP      8   /* survives every mask: feature query + compacted output */
 #define UBN_FLAG_INNER    16   /* |p| <= 1 before contraction (inner_mask) */
 
+/* update_occupancy_cache_lt_nviews inner loop (dcvgo.py:195-213: per view, `ones = grid.DenseGrid(1, world_size, xyz_min,
+ * xyz_max)`, then `ones(sample_ray(rays_o, rays_d)[0]).sum().backward()` per 8192 rays): grad [X,Y,Z] += the trilinear weights
+ * (align_corners=True) of every contracted sample t_table[s], s < cfg->n_samples, of every ray -- the points pass A generates,
+ * with no inner-mask, cumdist or mask-cache filter.  Only the scene normalisation, contraction and n_samples fields of `cfg`
+ * are read; `desc` is the single-slab ones grid (P = C = 1, unit voxel stride).  Follow with ubn_count_gt(grad, 1). */
+int ubn_view_scatter_ones_contracted(const float* rays_o, const float* rays_d, int64_t n_rays, const float* t_table,
+                                     const UbnMarchCfg* cfg, const UbnGridDesc* desc, float* grad, void* stream);
+
 /* Pass A: per nominal sample (r,s): contracted point, masks, density, alpha, exact sequential
  * transmittance scan (identical arithmetic to alpha2weight, early stop at T < 1e-3 included), weights,
  * both thresholds.  Dense per-sample outputs [n_rays*S]: density, alpha, weight, T, flags.

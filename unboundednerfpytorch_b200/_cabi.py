@@ -99,6 +99,8 @@ _SIGNATURES = {
     'ubn_maxpool3_gt_and': [c_p, c_i64, c_i64, c_i64, c_f, c_p, c_p],
     'ubn_resample_grid': [c_p, ctypes.POINTER(UbnGridDesc), c_p, ctypes.POINTER(UbnGridDesc), c_p],
     'ubn_view_scatter_ones': [c_p, c_p, c_i64, c_i64, c_f, c_f, c_f, ctypes.POINTER(UbnGridDesc), c_p, c_p],
+    'ubn_view_scatter_ones_contracted': [c_p, c_p, c_i64, c_p, ctypes.POINTER(UbnMarchCfg), ctypes.POINTER(UbnGridDesc), c_p,
+                                         c_p],
     'ubn_count_gt': [c_p, c_f, c_i64, c_p, c_p],
     'ubn_maskout_near_cam': [c_p, c_i64, c_i64, c_i64, c_i64, c_p, c_i64, c_f, c_f, c_p],
     'ubn_maskout_near_cam_lattice': [c_p, c_i64, c_i64, c_i64, c_i64, c_p, c_p, c_p, c_i64, c_f, c_f, c_p],

@@ -2,6 +2,7 @@
 //   update_occupancy_cache   FourierGrid_model.py:441-456, dcvgo.py:214-226   -> ubn_lattice_alpha + ubn_maxpool3_gt_and
 //   scale_volume_grid        grid.py:63-68, FourierGrid_grid.py:80-85         -> ubn_resample_grid (F.interpolate trilinear, align_corners)
 //   voxel_count_views        FourierGrid_model.py:390-420, dvgo.py:238-277    -> ubn_view_scatter_ones + ubn_count_gt
+//   update_occupancy_cache_lt_nviews  dcvgo.py:195-213                         -> ubn_view_scatter_ones_contracted + ubn_count_gt
 //   maskout_near_cam_vox     FourierGrid_model.py:375-388, dvgo.py:185-196    -> ubn_maskout_near_cam
 // The reference runs them as whole-grid torch compositions: a [X,Y,Z,3] meshgrid (100-400 MB at 256^3-320^3), a grid_sample over it,
 // an activation, a max_pool3d and a boolean AND for the occupancy update; a [N,S,3] point tensor plus a full autograd backward
@@ -110,6 +111,27 @@ __global__ void __launch_bounds__(256) k_view_scatter_ones(const float* __restri
   trilerp1_scatter(grad, 1, g.X, g.Y, g.Z, cx, cy, cz, 1.f);
 }
 
+// update_occupancy_cache_lt_nviews inner loop (dcvgo.py:195-213): the same adjoint of a ones grid over the contracted samples.
+// Sample s of a ray is the point the fused march and _ContractedBase._sample_dense generate (load_ray + sample_point at
+// t_table[s]), bit for bit, so every addend equals the one grid_sample's backward adds for sample_ray's point tensor.  All
+// n_rays * S samples count: the reference scatters the full tensor, with no inner-mask, cumdist or mask-cache filter.
+__global__ void __launch_bounds__(256) k_view_scatter_ones_contracted(const float* __restrict__ rays_o,
+                                                                      const float* __restrict__ rays_d, int64_t n_rays,
+                                                                      const float* __restrict__ t_table, MarchParams p, GridView g,
+                                                                      float* __restrict__ grad) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n_rays * p.S) return;
+  const int64_t ray = idx / p.S;
+  const int s = (int)(idx - ray * p.S);
+  const Ray r = load_ray(rays_o + 3 * ray, rays_d + 3 * ray, p);
+  float x, y, z;
+  sample_point(r, __ldg(t_table + s), p, x, y, z);
+  const float cx = src_index(norm_coord(x, g.mn[0], g.len[0]), g.X);
+  const float cy = src_index(norm_coord(y, g.mn[1], g.len[1]), g.Y);
+  const float cz = src_index(norm_coord(z, g.mn[2], g.len[2]), g.Z);
+  trilerp1_scatter_pairs(grad, g.X, g.Y, g.Z, cx, cy, cz, 1.f);
+}
+
 __global__ void __launch_bounds__(256) k_count_gt(const float* __restrict__ grad, float thres, int64_t n, float* __restrict__ count) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n && grad[i] > thres) count[i] += 1.f;
@@ -182,6 +204,18 @@ int ubn_view_scatter_ones(const float* rays_o, const float* rays_d, int64_t n_ra
   const GridView g = make_view(nullptr, desc);
   k_view_scatter_ones<<<blocks_for(n_rays * n_samples, 256), 256, 0, as_stream(stream)>>>(
       rays_o, rays_d, n_rays, (int)n_samples, near, far, step, g, desc->xyz_max[0], desc->xyz_max[1], desc->xyz_max[2], grad);
+  UBN_LAUNCH_CHECK();
+  return 0;
+}
+
+int ubn_view_scatter_ones_contracted(const float* rays_o, const float* rays_d, int64_t n_rays, const float* t_table,
+                                     const UbnMarchCfg* cfg, const UbnGridDesc* desc, float* grad, void* stream) {
+  if (n_rays <= 0 || cfg->n_samples <= 0) return 0;
+  if (desc->P != 1 || desc->C != 1 || desc->stride_v != 1) return finish(cudaErrorInvalidValue);
+  const MarchParams p = make_params(cfg);
+  const GridView g = make_view(nullptr, desc);
+  k_view_scatter_ones_contracted<<<blocks_for(n_rays * cfg->n_samples, 256), 256, 0, as_stream(stream)>>>(rays_o, rays_d, n_rays,
+                                                                                                          t_table, p, g, grad);
   UBN_LAUNCH_CHECK();
   return 0;
 }

@@ -111,10 +111,11 @@ class MaskedAdam(torch.optim.Optimizer):
                 self._apply(group, param, self._begin(param))
 
 
-def create_optimizer_or_freeze_model(model, cfg_train, global_step):
+def create_optimizer_or_freeze_model(model, cfg_train, global_step, verbose=False):
     """Optimizer factory with the reference's config keys (FourierGrid/utils.py:26-56): every ``lrate_<name>``
     key names a sub-module / parameter of ``model``; lr decays by 0.1 every ``lrate_decay``*1000 steps;
-    ``skip_zero_grad_fields`` selects the masked update."""
+    ``skip_zero_grad_fields`` selects the masked update.  ``verbose`` is accepted for the reference's signature
+    (run_train.py:54 passes it) and logs nothing."""
     get = (lambda k, d=None: cfg_train.get(k, d)) if hasattr(cfg_train, 'get') else (lambda k, d=None: getattr(cfg_train, k, d))
     keys = cfg_train.keys() if hasattr(cfg_train, 'keys') else vars(cfg_train).keys()
     decay_steps = get('lrate_decay') * 1000

@@ -250,6 +250,30 @@ class _ContractedBase(_GridModel):
         w = weight * float(max(grid.grid.shape[2:])) / 128         # each grid's own largest dimension
         return (w, w, w, dense_mode)
 
+    @torch.no_grad()
+    def update_occupancy_cache_lt_nviews(self, rays_o_tr, rays_d_tr, imsz, render_kwargs, maskout_lt_nviews):
+        """dcvgo.py:195-213: mask_cache.mask &= (number of training views whose contracted samples put a trilinear weight > 1 on a
+        voxel of a ones grid over [xyz_min, xyz_max] at world_size) >= maskout_lt_nviews.  Every one of a view's n_rays * S samples
+        counts, as the reference scatters sample_ray's whole point tensor.  The reference materialises [8192, S, 3] points and runs
+        grid_sample's backward per chunk; here one kernel per view (ops.view_scatter_ones_contracted) generates each sample in
+        registers and scatters its eight weights into a per-view buffer, and ops.count_gt_ adds (buffer > 1) to the count."""
+        from . import ops
+        dev = self.density.grid.device
+        ws = [int(v) for v in self.world_size]
+        t_table = march.t_schedule(self._world_len(), render_kwargs['stepsize'], self.bg_len, self.T_BOUNDARY, dev)
+        center, radius = self._host()
+        lo, hi = self.xyz_min.tolist(), self.xyz_max.tolist()
+        count = torch.zeros(ws, device=dev)
+        buf = torch.empty(ws, device=dev)
+        for rays_o, rays_d in zip(rays_o_tr.split(imsz), rays_d_tr.split(imsz)):
+            rays_o = rays_o.to(dev, torch.float32).reshape(-1, 3).contiguous()
+            rays_d = rays_d.to(dev, torch.float32).reshape(-1, 3).contiguous()
+            buf.zero_()
+            ops.view_scatter_ones_contracted(rays_o, rays_d, t_table, center, radius, self.bg_len, self.contracted_norm, lo, hi, ws,
+                                             buf)
+            ops.count_gt_(count, buf, 1.0)
+        self.mask_cache.mask &= (count >= maskout_lt_nviews)
+
 
 @torch.no_grad()
 def _scale_dense_model(model, num_voxels):
@@ -403,6 +427,60 @@ class FourierGridModel(_CoarseGeo, _ContractedBase):
         """FourierGrid_model.py:390-420 (see _count_views)."""
         return _count_views(self.density, self.world_size_density, self.voxel_size_density, rays_o_tr, rays_d_tr, imsz, near,
                             stepsize, downrate, irregular_shape)
+
+    def update_occupancy_cache_lt_nviews(self, rays_o_tr, rays_d_tr, imsz, render_kwargs, maskout_lt_nviews):
+        """FourierGrid_model.py:458-480 (see _ContractedBase.update_occupancy_cache_lt_nviews).  The reference builds its ones grid
+        as `FourierGrid_grid.FourierGrid(1, world_size_density, xyz_min, xyz_max)` (:466), which lacks three required arguments
+        and raises a TypeError; the evident intent -- a single-slab ones grid over the density lattice -- is what runs here:
+        DirectContractedVoxGO's semantics with this model's t schedule (T_BOUNDARY = 1.5)."""
+        return super().update_occupancy_cache_lt_nviews(rays_o_tr, rays_d_tr, imsz, render_kwargs, maskout_lt_nviews)
+
+    @torch.no_grad()
+    def FourierGrid_get_training_rays(self, rgb_tr_ori, train_poses, HW, Ks, ndc, inverse_y, flip_x, flip_y):
+        """FourierGrid_model.py:263-295 -> (rgb_tr, rays_o_tr, rays_d_tr, viewdirs_tr, indexs_tr, imsz): the flattened rays of
+        rays.get_training_rays_flatten plus indexs_tr, a float [N, 3] tensor holding each ray's view ordinal in all three
+        columns.  pos_emb is always None on this model (:209), so the poses are used as given."""
+        from . import rays
+        rgb_tr, rays_o_tr, rays_d_tr, viewdirs_tr, imsz = rays.get_training_rays_flatten(
+            rgb_tr_ori, train_poses, HW, Ks, ndc, inverse_y, flip_x, flip_y)
+        dev = rgb_tr.device
+        view = torch.arange(len(imsz), dtype=torch.float32, device=dev).repeat_interleave(torch.tensor(imsz, device=dev))
+        indexs_tr = view[:, None].expand(-1, 3).contiguous()
+        return rgb_tr, rays_o_tr, rays_d_tr, viewdirs_tr, indexs_tr, imsz
+
+    def gather_training_rays(self, data_dict, images, cfg, i_train, cfg_train, poses, HW, Ks, render_kwargs):
+        """FourierGrid_model.py:297-333 -> (rgb_tr, rays_o_tr, rays_d_tr, viewdirs_tr, indexs_train, imsz, batch_index_sampler):
+        the training rays of run_train.py's FourierGrid datasets, images kept on the host under load2gpu_on_the_fly."""
+        from . import rays
+        device = torch.device('cuda' if torch.cuda.is_available() else 'cpu')
+        where = 'cpu' if cfg.data.load2gpu_on_the_fly else device
+        if data_dict['irregular_shape']:
+            rgb_tr_ori = [images[i].to(where) for i in i_train]
+        else:
+            rgb_tr_ori = images[i_train].to(where)
+        views = dict(train_poses=poses[i_train], HW=HW[i_train], Ks=Ks[i_train], ndc=cfg.data.ndc, inverse_y=cfg.data.inverse_y,
+                     flip_x=cfg.data.flip_x, flip_y=cfg.data.flip_y)
+        indexs_train = None
+        if cfg.data.dataset_type in ('waymo', 'mega', 'nerfpp') or cfg.model == 'FourierGrid':
+            rgb_tr, rays_o_tr, rays_d_tr, viewdirs_tr, indexs_train, imsz = self.FourierGrid_get_training_rays(
+                rgb_tr_ori=rgb_tr_ori, **views)
+        elif cfg_train.ray_sampler == 'in_maskcache':
+            rgb_tr, rays_o_tr, rays_d_tr, viewdirs_tr, imsz = rays.get_training_rays_in_maskcache_sampling(
+                rgb_tr_ori=rgb_tr_ori, model=self, render_kwargs=render_kwargs, **views)
+        elif cfg_train.ray_sampler == 'flatten':
+            rgb_tr, rays_o_tr, rays_d_tr, viewdirs_tr, imsz = rays.get_training_rays_flatten(rgb_tr_ori=rgb_tr_ori, **views)
+        else:
+            rgb_tr, rays_o_tr, rays_d_tr, viewdirs_tr, imsz = rays.get_training_rays(rgb_tr=rgb_tr_ori, **views)
+        index_generator = rays.batch_indices_generator(len(rgb_tr), cfg_train.N_rand)
+        return rgb_tr, rays_o_tr, rays_d_tr, viewdirs_tr, indexs_train, imsz, lambda: next(index_generator)
+
+    @torch.no_grad()
+    def export_geometry_for_visualize(self, save_path):
+        """FourierGrid_model.py:674-681: npz of alpha = activate_density(density grid) and rgb = sigmoid(k0 grid), slab and channel
+        axes as the reference squeezes and permutes them."""
+        alpha = self.activate_density(self.density.get_dense_grid()).squeeze().cpu().numpy()
+        rgb = torch.sigmoid(self.k0.get_dense_grid()).squeeze().permute(1, 2, 3, 0).cpu().numpy()
+        np.savez_compressed(save_path, alpha=alpha, rgb=rgb)
 
     def sample_ray(self, ori_rays_o, ori_rays_d, stepsize, is_train=False, **render_kwargs):
         """FourierGrid_model.py:509-552 return tuple (ray_pts, indexs, inner_mask, t, rays_d_extend)."""

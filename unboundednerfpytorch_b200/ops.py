@@ -403,6 +403,30 @@ def view_scatter_ones(rays_o, rays_d, xyz_min, xyz_max, world_size, n_samples, n
                                         c_f(float(step)), d, ptr(grad), stream_of(rays_o)))
 
 
+def view_scatter_ones_contracted(rays_o, rays_d, t_table, scene_center, scene_radius, bg_len, contracted_norm, xyz_min, xyz_max,
+                                 world_size, grad):
+    """grad [X,Y,Z] += adjoint of DenseGrid(1, world_size, xyz_min, xyz_max)(pts).sum() over the contracted sample points of the
+    rays: pts[r, s] = the point sample_ray (dcvgo.py:228-262, FourierGrid_model.py:509-552) puts at t_table[s], all of them
+    (dcvgo.py:203-207).  ``scene_center`` / ``scene_radius`` / ``xyz_min`` / ``xyz_max`` are host 3-sequences."""
+    from . import march
+    from ._cabi import UbnGridDesc
+    _chk(rays_o, 'rays_o'); _chk(rays_d, 'rays_d'); _chk(t_table, 't_table'); _chk(grad, 'grad')
+    d = UbnGridDesc()
+    d.P, d.C, d.num_freqs = 1, 1, 0
+    d.X, d.Y, d.Z = [int(v) for v in world_size]
+    if grad.numel() != d.X * d.Y * d.Z:
+        raise RuntimeError('grad must have world_size elements')
+    d.stride_p, d.stride_c, d.stride_v = d.X * d.Y * d.Z, 1, 1
+    for a in range(3):
+        d.xyz_min[a], d.xyz_max[a] = float(xyz_min[a]), float(xyz_max[a])
+    cfg = march.make_cfg(scene_center, scene_radius, bg_len, contracted_norm, t_table.numel(), 0., 0., 0.)
+    n = rays_o.shape[0]
+    with _Guard(rays_o) as lib:
+        check(lib.ubn_view_scatter_ones_contracted(ptr(rays_o), ptr(rays_d), c_i64(n), ptr(t_table), cfg, d, ptr(grad),
+                                                   stream_of(rays_o)))
+    return grad
+
+
 def count_gt_(count, grad, thres=1.0):
     """count += (grad > thres), in place (FourierGrid_model.py:418-419)."""
     _chk(count, 'count', contiguous=False); _chk(grad, 'grad', contiguous=False)
