@@ -29,6 +29,8 @@ __global__ void __launch_bounds__(256) k_lattice_alpha(GridView g, float lox, fl
 }
 
 // mask &= max_pool3d(alpha, 3, stride 1, padding 1) > thres     (F.max_pool3d pads with -inf)
+// The window maximum is ATen's: `v > m || isnan(v)` takes v, so a NaN in the window pools to NaN, NaN > thres is false and the
+// cell is cleared (fmaxf would drop the NaN and keep the cell).
 __global__ void __launch_bounds__(256) k_maxpool3_gt_and(const float* __restrict__ alpha, int X, int Y, int Z, float thres,
                                                          uint8_t* __restrict__ mask) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -39,7 +41,10 @@ __global__ void __launch_bounds__(256) k_maxpool3_gt_and(const float* __restrict
   float m = -INFINITY;
   for (int a = max(i - 1, 0); a <= min(i + 1, X - 1); ++a)
     for (int b = max(j - 1, 0); b <= min(j + 1, Y - 1); ++b)
-      for (int c = max(k - 1, 0); c <= min(k + 1, Z - 1); ++c) m = fmaxf(m, alpha[((int64_t)a * Y + b) * Z + c]);
+      for (int c = max(k - 1, 0); c <= min(k + 1, Z - 1); ++c) {
+        const float v = alpha[((int64_t)a * Y + b) * Z + c];
+        if (v > m || isnan(v)) m = v;
+      }
   mask[idx] = (m > thres) ? 1 : 0;
 }
 
@@ -105,9 +110,9 @@ __global__ void __launch_bounds__(256) k_view_scatter_ones(const float* __restri
   const float nrm = norm3_torch(dx, dy, dz);
   const float t = __fadd_rn(t_min, __fdiv_rn(__fmul_rn(step, (float)s), nrm));
   const float x = __fadd_rn(ox, __fmul_rn(dx, t)), y = __fadd_rn(oy, __fmul_rn(dy, t)), z = __fadd_rn(oz, __fmul_rn(dz, t));
-  const float cx = src_index(norm_coord(x, g.mn[0], g.len[0]), g.X);
-  const float cy = src_index(norm_coord(y, g.mn[1], g.len[1]), g.Y);
-  const float cz = src_index(norm_coord(z, g.mn[2], g.len[2]), g.Z);
+  const float cx = src_index_guarded(norm_coord(x, g.mn[0], g.len[0]), g.X);
+  const float cy = src_index_guarded(norm_coord(y, g.mn[1], g.len[1]), g.Y);
+  const float cz = src_index_guarded(norm_coord(z, g.mn[2], g.len[2]), g.Z);
   trilerp1_scatter(grad, 1, g.X, g.Y, g.Z, cx, cy, cz, 1.f);
 }
 

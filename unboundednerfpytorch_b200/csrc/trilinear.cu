@@ -22,9 +22,9 @@ __global__ void __launch_bounds__(256) k_grid_fwd_c1(GridView g, const float* __
   const float nz = norm_coord(xyz[3 * p + 2], g.mn[2], g.len[2]);
   SlabMean acc;
   for (int s = 0; s < g.P; ++s) {
-    const float cx = src_index(fourier_gamma(s, nx), g.X);
-    const float cy = src_index(fourier_gamma(s, ny), g.Y);
-    const float cz = src_index(fourier_gamma(s, nz), g.Z);
+    const float cx = src_index_guarded(fourier_gamma(s, nx), g.X);
+    const float cy = src_index_guarded(fourier_gamma(s, ny), g.Y);
+    const float cz = src_index_guarded(fourier_gamma(s, nz), g.Z);
     acc.add(s, trilerp1(g.data + s * g.sp, g.sv, g.X, g.Y, g.Z, cx, cy, cz));
   }
   out[p] = acc.mean(g.P);
@@ -41,9 +41,9 @@ __global__ void __launch_bounds__(256) k_grid_bwd_c1(GridView g, const float* __
   const float ny = norm_coord(xyz[3 * p + 1], g.mn[1], g.len[1]);
   const float nz = norm_coord(xyz[3 * p + 2], g.mn[2], g.len[2]);
   for (int s = 0; s < g.P; ++s) {
-    const float cx = src_index(fourier_gamma(s, nx), g.X);
-    const float cy = src_index(fourier_gamma(s, ny), g.Y);
-    const float cz = src_index(fourier_gamma(s, nz), g.Z);
+    const float cx = src_index_guarded(fourier_gamma(s, nx), g.X);
+    const float cy = src_index_guarded(fourier_gamma(s, ny), g.Y);
+    const float cz = src_index_guarded(fourier_gamma(s, nz), g.Z);
     trilerp1_scatter(grad_grid + s * g.sp, g.sv, g.X, g.Y, g.Z, cx, cy, cz, go);
   }
 }
@@ -61,9 +61,9 @@ __global__ void __launch_bounds__(256) k_grid_fwd_generic(GridView g, const floa
   for (int c = 0; c < g.C; ++c) {
     SlabMean acc;
     for (int s = 0; s < g.P; ++s) {
-      const float cx = src_index(fourier_gamma(s, nx), g.X);
-      const float cy = src_index(fourier_gamma(s, ny), g.Y);
-      const float cz = src_index(fourier_gamma(s, nz), g.Z);
+      const float cx = src_index_guarded(fourier_gamma(s, nx), g.X);
+      const float cy = src_index_guarded(fourier_gamma(s, ny), g.Y);
+      const float cz = src_index_guarded(fourier_gamma(s, nz), g.Z);
       acc.add(s, trilerp1(g.data + s * g.sp + c * g.sc, g.sv, g.X, g.Y, g.Z, cx, cy, cz));
     }
     out[p * g.C + c] = acc.mean(g.P);
@@ -79,9 +79,9 @@ __global__ void __launch_bounds__(256) k_grid_bwd_generic(GridView g, const floa
   const float ny = norm_coord(xyz[3 * p + 1], g.mn[1], g.len[1]);
   const float nz = norm_coord(xyz[3 * p + 2], g.mn[2], g.len[2]);
   for (int s = 0; s < g.P; ++s) {
-    const float cx = src_index(fourier_gamma(s, nx), g.X);
-    const float cy = src_index(fourier_gamma(s, ny), g.Y);
-    const float cz = src_index(fourier_gamma(s, nz), g.Z);
+    const float cx = src_index_guarded(fourier_gamma(s, nx), g.X);
+    const float cy = src_index_guarded(fourier_gamma(s, ny), g.Y);
+    const float cz = src_index_guarded(fourier_gamma(s, nz), g.Z);
     for (int c = 0; c < g.C; ++c) {
       float go = grad_out[p * g.C + c];
       go = slab_mean_scale(go, g.P);
@@ -120,8 +120,8 @@ __global__ void __launch_bounds__(32 * kCoopWarps) k_grid_coop(GridView g, const
       const float ny = norm_coord(xyz[3 * p + 1], g.mn[1], g.len[1]);
       const float nz = norm_coord(xyz[3 * p + 2], g.mn[2], g.len[2]);
       for (int s = 0; s < g.P; ++s)
-        my_idx[lane * g.P + s] = make_float4(src_index(fourier_gamma(s, nx), g.X), src_index(fourier_gamma(s, ny), g.Y),
-                                             src_index(fourier_gamma(s, nz), g.Z), 0.f);
+        my_idx[lane * g.P + s] = make_float4(src_index_guarded(fourier_gamma(s, nx), g.X), src_index_guarded(fourier_gamma(s, ny), g.Y),
+                                             src_index_guarded(fourier_gamma(s, nz), g.Z), 0.f);
     }
     __syncwarp();
     const int n_here = (int)min((int64_t)32, n_pts - grp * 32);

@@ -52,6 +52,15 @@ __device__ __forceinline__ float src_index(float coord, int size) {
   return __fmul_rn(__fmul_rn(__fadd_rn(coord, 1.f), 0.5f), (float)(size - 1));
 }
 
+// src_index followed by ATen's guard (GridSampler.cuh: safe_downgrade_to_int_range): an index that is NaN, infinite or outside the
+// int range becomes -100, so every corner of it lies outside the grid.  A point with a NaN or inf coordinate -- or the sin / cos
+// of one -- then reads 0 and scatters nothing, as F.grid_sample does, instead of carrying NaN weights into in-range corners.
+// The stand-alone grid ops and the view count use it; the fused march's points are finite by construction.
+__device__ __forceinline__ float src_index_guarded(float coord, int size) {
+  const float c = src_index(coord, size);
+  return (c > (float)(INT_MAX - 1) || c < (float)INT_MIN || !isfinite(c)) ? -100.f : c;
+}
+
 // Mean over the P slabs exactly as torch-CUDA evaluates `out.mean(0)` on the grid_sample output (FourierGrid_grid.py:72), as
 // probed with scripts/probe_mean_order.py (the sequential and the pairwise-tree orders do not match): ATen's reduction keeps four interleaved accumulators a[i & 3] += x_i, combines them ((a0 + a1) + a2) + a3
 // and multiplies by the fp32 reciprocal of P.  Matching it makes raw_density -- and with it alpha, the weights and every
