@@ -63,7 +63,8 @@ __global__ void __launch_bounds__(kLossThreads) k_render_loss(
     }
     if (alphainv_last) {
       const float a = alphainv_last[r];
-      const float p = fminf(fmaxf(a, 1e-6f), 1.f - 1e-6f);
+      // torch's clamp propagates NaN (fmaxf / fminf would turn it into a bound): a NaN alphainv_last makes the term NaN
+      const float p = isnan(a) ? a : fminf(fmaxf(a, 1e-6f), 1.f - 1e-6f);
       const float lp = logf(p), lq = logf(1.f - p);
       s_ent += (double)(-(p * lp + (1.f - p) * lq));
       // d/dp = -(log p - log(1-p)); clamp passes the gradient on [min, max] inclusive
