@@ -339,8 +339,8 @@ int ubn_get_density_scatter(void);
 
 /* Pass B: for every survivor (flags bit1), in (ray, step) order at offsets[ray]+rank: recompute the
  * contracted point, query the feature grid (k0), and emit the compacted per-survivor records.
- * k0: channels-last with C in {4, 8, 12, 16} (16-byte aligned), or C in {3, 15} with an odd slab count P <= 11 and >= 2 voxels
- * per axis (4-byte aligned records; features bit-identical to F.grid_sample(...).mean(0)). */
+ * k0: channels-last with C in {4, 8, 12, 16} (16-byte aligned), or C in {3, 9, 15} with an odd slab count P <= 11 and >= 2
+ * voxels per axis (4-byte aligned records; features bit-identical to F.grid_sample(...).mean(0)). */
 int ubn_march_feature_fwd(const float* rays_o, const float* rays_d, const float* t_table,
                           const float* k0_grid, const UbnGridDesc* k0_desc, const UbnMarchCfg* cfg,
                           int64_t n_rays, const uint8_t* flags, const int64_t* offsets,
@@ -457,7 +457,8 @@ int ubn_march_box_density_fwd(const float* rays_o, const float* rays_d, const fl
                               void* stream);
 /* Pass B: for every survivor, in (ray, step) order at offsets[ray] + rank, the k0 read (F.grid_sample arithmetic, bit-identical)
  * and the compacted records alpha, weight, ray_id, step_id (step_id = the ray's own step index).  k0: single-slab channels-last
- * grid with C = 12 (16-byte aligned) or C = 3; k0_feat 16-byte aligned; out_alpha / out_weight may be NULL. */
+ * grid with C = 12 (16-byte aligned), C = 9 or C = 3 (4-byte aligned); k0_feat 16-byte aligned; out_alpha / out_weight may be
+ * NULL. */
 int ubn_march_box_feature_fwd(const float* rays_o, const float* rays_d, const float* k0_grid, const UbnGridDesc* k0_desc,
                               const UbnBoxMarchCfg* cfg, int64_t n_rays, const uint8_t* flags, const int64_t* offsets,
                               const float* alpha, const float* weight, float* k0_feat, float* out_alpha, float* out_weight,

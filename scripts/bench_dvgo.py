@@ -1,8 +1,8 @@
 """Time DirectVoxGO (bounded scenes, dvgo.py) on the GPU and print one JSON line.
 
-    python scripts/bench_dvgo.py [--steps 20] [--warmup 5]
+    python scripts/bench_dvgo.py [--steps 20] [--warmup 5] [--shape default|lab] [--rounds 3]
 
-Legs, each from the same parameters:
+Legs of the default shape, each from the same parameters:
 * fine-stage training step (run_train.py:251-288 with configs/default.py's fine weights: entropy_last 1e-3, rgbper 1e-2, no TV,
   MaskedAdam skipping zero gradients on density and k0) at 160^3 voxels, 12-channel k0, 8192 rays: the fused march
   (``forward``), the op-by-op composition (``forward_ops``) and the reference's GPU path (its unmodified dvgo.py and
@@ -12,7 +12,11 @@ Legs, each from the same parameters:
 * one 800x800 frame in 8192-ray chunks.
 Per launch: the march kernels' CUDA-event times and their algorithmic HBM share against 3.35 TB/s, and the rgbnet's share of the
 fused step.  Output check: fused against forward_ops (and against the reference's GPU path) at the timed size.  The GPU name and
-power limit are read in the same run."""
+power limit are read in the same run.
+
+--shape lab: configs/free_dataset/lab.py's fine stage -- a 250^3 voxel budget, 9-channel k0, rgbnet width 64, fast_color_thres
+1e-3, 4096 rays -- with the same training step for the fused, forward_ops and reference_gpu legs alternated for --rounds rounds,
+the per-launch times and the rgbnet's share of the fused step, and the output check at the timed size."""
 import argparse
 import json
 import os
@@ -40,14 +44,16 @@ def _gpu():
         return torch.cuda.get_device_name(0), f'unknown ({type(e).__name__})'
 
 
-def _scene(nv, C, n, seed, cls=None):
+def _scene(nv, C, n, seed, cls=None, width=128, thres=None):
     """C = 12: the fine stage of configs/default.py (alpha_init 1e-2, fast_color_thres 1e-4); C = 3: its coarse stage
-    (rgbnet_dim 0, alpha_init 1e-6, fast_color_thres 1e-7)."""
+    (rgbnet_dim 0, alpha_init 1e-6, fast_color_thres 1e-7); C = 9: lab.py's fine stage (rgbnet width 64, fast_color_thres 1e-3)."""
     from unboundednerfpytorch_b200 import models
     cls = cls or models.DirectVoxGO
     g = torch.Generator().manual_seed(seed)
-    m = cls(xyz_min=LO, xyz_max=HI, num_voxels=nv, num_voxels_base=nv, alpha_init=1e-2 if C == 12 else 1e-6,
-            fast_color_thres=1e-4 if C == 12 else 1e-7, rgbnet_dim=0 if C == 3 else C, rgbnet_direct=True)
+    if thres is None:
+        thres = 1e-7 if C == 3 else 1e-4
+    m = cls(xyz_min=LO, xyz_max=HI, num_voxels=nv, num_voxels_base=nv, alpha_init=1e-6 if C == 3 else 1e-2,
+            fast_color_thres=thres, rgbnet_dim=0 if C == 3 else C, rgbnet_direct=True, rgbnet_width=width)
     with torch.no_grad():
         X, Y, Z = [int(v) for v in m.world_size]
         ax = [torch.linspace(-1, 1, k) for k in (X, Y, Z)]
@@ -130,13 +136,65 @@ def _reference_leg(state, ours, ro, rd, vd, target, args):
     return {'ms': round(ms, 3), 'check_vs_fused': check}
 
 
+def _check(a, b):
+    same = torch.equal(a['ray_id'], b['ray_id'])
+    return {'ray_id_equal': same, 'samples': int(len(a['ray_id'])),
+            'weights_bit_identical': same and torch.equal(a['weights'], b['weights']),
+            'raw_alpha_bit_identical': same and torch.equal(a['raw_alpha'], b['raw_alpha']),
+            'alphainv_last_bit_identical': torch.equal(a['alphainv_last'], b['alphainv_last']),
+            'rgb_marched_max_abs_diff': float((a['rgb_marched'] - b['rgb_marched']).abs().max())}
+
+
+def lab(args):
+    """lab.py's fine stage: the three legs alternated round by round, per-launch times of the fused step."""
+    from unboundednerfpytorch_b200 import _cabi
+    name, power = _gpu()
+    out = {'bench': 'dvgo lab', 'gpu': name, 'power_limit': power, 'steps': args.steps, 'warmup': args.warmup,
+           'shape': dict(num_voxels=250 ** 3, k0_channels=9, rgbnet_width=64, fast_color_thres=1e-3, rays=4096)}
+    base, ro, rd, vd = _scene(250 ** 3, 9, 4096, 0, width=64, thres=1e-3)
+    state = {k: v.clone() for k, v in base.state_dict().items()}
+    with torch.no_grad():
+        target = torch.rand(len(ro), 3, device='cuda', generator=torch.Generator('cuda').manual_seed(1))
+        out['check'] = _check(base(ro, rd, vd, **RK), base.forward_ops(ro, rd, vd, **RK))
+    legs = {'fused': [], 'forward_ops': [], 'reference_gpu': []}
+    for _ in range(args.rounds):
+        for leg in ('fused', 'forward_ops'):
+            base.load_state_dict(state)
+            opt = _opt(base)
+            fn = base.forward if leg == 'fused' else base.forward_ops
+            legs[leg].append(round(_time(lambda i: _step(base, fn, opt, ro, rd, vd, target, i + 1), args.steps, args.warmup), 3))
+        ref = _reference_leg(state, base, ro, rd, vd, target, args)
+        if 'ms' not in ref:
+            legs['reference_gpu'] = ref
+            break
+        legs['reference_gpu'].append(ref['ms'])
+        out['check_vs_reference_gpu'] = ref['check_vs_fused']
+    out['step_ms_rounds'] = legs
+    base.load_state_dict(state)
+    opt = _opt(base)
+    _cabi.TIMER = _cabi.KernelTimer()
+    try:
+        ms = _time(lambda i: _step(base, base.forward, opt, ro, rd, vd, target, i + 1), args.steps, 1)
+        summ = _cabi.TIMER.summary()
+    finally:
+        _cabi.TIMER = None
+    out['launches'] = {k: {'ms': round(v, 4), 'calls': c} for k, (v, c) in summ.items()}
+    out['instrumented_step_ms'] = round(ms, 3)
+    out['rgbnet_share_of_fused_step'] = round(sum(v for k, (v, _) in summ.items() if 'rgbnet' in k) / ms, 3)
+    print(json.dumps(out))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--steps', type=int, default=20)
     ap.add_argument('--warmup', type=int, default=5)
+    ap.add_argument('--shape', choices=('default', 'lab'), default='default')
+    ap.add_argument('--rounds', type=int, default=3)
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit('bench_dvgo needs a CUDA device')
+    if args.shape == 'lab':
+        return lab(args)
     import unboundednerfpytorch_b200 as U
     from unboundednerfpytorch_b200 import _cabi, render
     name, power = _gpu()

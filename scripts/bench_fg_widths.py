@@ -1,24 +1,27 @@
-"""Benchmark of FourierGridModel at the k0 widths of the reference's Waymo and Tanks&Temples configs, on one GPU.  Prints one JSON
-line per shape:
+"""Benchmark of FourierGridModel at the k0 widths of the reference's Waymo, Tanks&Temples and free-dataset configs, on one GPU.
+Prints one JSON line per shape:
 
 * waymo -- configs/waymo/waymo_no_block.py: 300^3 density and k0, fourier_freq_num 3 (P = 7), rgbnet_dim 3, viewbase_pe 2,
            contracted_norm l2, 2048 rays; loss weights main 3, entropy_last 1e-3, rgbper 1e-2, TV density 1e-6 / k0 1e-7;
 * train -- configs/tankstemple_unbounded/train_single.py: 250^3, P = 7, rgbnet_dim 15, viewbase_pe 4, contracted_norm inf,
-           4096 rays; loss weights main 1, entropy_last 1e-3, rgbper 1e-2, TV density 1e-6 / k0 1e-7.
+           4096 rays; loss weights main 1, entropy_last 1e-3, rgbper 1e-2, TV density 1e-6 / k0 1e-7;
+* grass -- configs/free_dataset/grass.py: 250^3, P = 7, rgbnet_dim 9 at rgbnet_width 64, viewbase_pe 4, contracted_norm inf,
+           fast_color_thres 1e-3, 4096 rays; the same loss weights as train.
 
-Both use alpha_init 1e-4, stepsize 0.5 and fast_color_thres 5e-6 (the configs' schedule at step 0).  The Fourier-space MSE term
-(weight_freq, Waymo only) and the distortion loss are not part of the timed step.  Per shape:
+All use alpha_init 1e-4 and stepsize 0.5; waymo and train use fast_color_thres 5e-6 (the configs' schedule at step 0).  The
+Fourier-space MSE term (weight_freq, Waymo only) and the distortion loss are not part of the timed step.  Per shape:
 
 * train_step_ms -- one run_train.py step (forward, loss, backward, dense TV, MaskedAdam) for three legs from the same parameters:
                    ``fused`` (forward), ``forward_ops`` and ``reference_gpu`` (the reference's unmodified FourierGrid_model.py and
                    masked_adam.py, staged under oracle/_ref/py, over its own CUDA extension in oracle/_ref; an ``unavailable``
-                   record when that was not built);
+                   record when that was not built), alternated for --rounds rounds in one process; ``train_step_ms_rounds``
+                   holds every round's time, ``train_step_ms`` each leg's fastest round;
 * kernels_ms    -- per-launch times of the fused step (CUDA events around the C-ABI calls, ``_cabi.timed``) and the rgbnet's
                    share of the step;
 * outputs       -- fused vs forward_ops before the first step: survivor sets equal, max error over scale;
 * gpu / power_limit_w -- where it ran, read in the same run.
 
-    python scripts/bench_fg_widths.py [--steps 10] [--warmup 3] [--only waymo|train]
+    python scripts/bench_fg_widths.py [--steps 10] [--warmup 3] [--rounds 3] [--only waymo|train|grass]
 """
 import argparse
 import contextlib
@@ -38,8 +41,9 @@ sys.path.insert(0, ROOT)
 from scripts.bench_mpi import _gpu_info, _time  # noqa: E402
 
 SHAPES = {
-    'waymo': dict(world=300, rgbnet_dim=3, viewbase_pe=2, norm='l2', rays=2048, w_main=3.0),
-    'train': dict(world=250, rgbnet_dim=15, viewbase_pe=4, norm='inf', rays=4096, w_main=1.0),
+    'waymo': dict(world=300, rgbnet_dim=3, width=128, viewbase_pe=2, norm='l2', rays=2048, w_main=3.0, thres=5e-6),
+    'train': dict(world=250, rgbnet_dim=15, width=128, viewbase_pe=4, norm='inf', rays=4096, w_main=1.0, thres=5e-6),
+    'grass': dict(world=250, rgbnet_dim=9, width=64, viewbase_pe=4, norm='inf', rays=4096, w_main=1.0, thres=1e-3),
 }
 RK = dict(near=0., far=1e9, bg=1, rand_bkgd=False, stepsize=0.5, inverse_y=False, flip_x=False, flip_y=False)
 
@@ -47,8 +51,9 @@ RK = dict(near=0., far=1e9, bg=1, rand_bkgd=False, stepsize=0.5, inverse_y=False
 def _kwargs(s):
     w = s['world'] ** 3
     return dict(xyz_min=[-1.] * 3, xyz_max=[1.] * 3, num_voxels_density=w, num_voxels_base_density=w, num_voxels_rgb=w,
-                num_voxels_base_rgb=w, num_voxels_viewdir=-1, alpha_init=1e-4, fast_color_thres=5e-6, rgbnet_dim=s['rgbnet_dim'],
-                fourier_freq_num=3, viewbase_pe=s['viewbase_pe'], contracted_norm=s['norm'], bg_len=0.2)
+                num_voxels_base_rgb=w, num_voxels_viewdir=-1, alpha_init=1e-4, fast_color_thres=s['thres'],
+                rgbnet_dim=s['rgbnet_dim'], rgbnet_width=s['width'], fourier_freq_num=3, viewbase_pe=s['viewbase_pe'],
+                contracted_norm=s['norm'], bg_len=0.2)
 
 
 def _train_step(m, opt, fwd, ro, rd, vd, target, it, w_main):
@@ -89,6 +94,26 @@ def _reference():
     return FourierGrid_model, masked_adam
 
 
+def _reference_leg(ref, s, state0, ro, rd, vd, target, args):
+    """One timed round of the step on the reference's GPU path, from state0."""
+    import numpy as np
+    from oracle import ref_gpu_py
+    fgm, madam = ref
+    kw = dict(_kwargs(s), xyz_min=np.array([-1.] * 3, dtype=np.float32), xyz_max=np.array([1.] * 3, dtype=np.float32))
+    ref_gpu_py.default_cuda(True)           # run_FourierGrid.py:87: the reference allocates with the default tensor type
+    try:
+        with contextlib.redirect_stdout(io.StringIO()):
+            rm = fgm.FourierGridModel(**kw)
+        rm.load_state_dict(state0, strict=False)
+        rm = rm.cuda()
+        ropt = madam.MaskedAdam([{'params': [rm.density.grid], 'lr': 0.1, 'skip_zero_grad': True},
+                                 {'params': [rm.k0.grid], 'lr': 0.1, 'skip_zero_grad': True},
+                                 {'params': list(rm.rgbnet.parameters()), 'lr': 1e-3, 'skip_zero_grad': False}])
+        return _time(lambda i: _train_step(rm, ropt, rm.forward, ro, rd, vd, target, i + 1, s['w_main']), args.steps, args.warmup)
+    finally:
+        ref_gpu_py.default_cuda(False)
+
+
 def bench(name, s, args):
     import numpy as np
     from unboundednerfpytorch_b200 import _cabi, models
@@ -118,16 +143,6 @@ def bench(name, s, args):
                              for k in ('rgb_marched', 'alphainv_last') + (('weights', 'raw_rgb') if same else ())})
     del a, b
 
-    res['train_step_ms'] = {}
-    for leg in ('fused', 'forward_ops'):
-        m.load_state_dict(state0)
-        opt = create_optimizer_or_freeze_model(m, cfg, global_step=0)
-        fwd = m.forward if leg == 'fused' else m.forward_ops
-        res['train_step_ms'][leg] = _time(lambda i: _train_step(m, opt, fwd, ro, rd, vd, target, i + 1, s['w_main']),
-                                          args.steps, args.warmup)
-        del opt
-        torch.cuda.empty_cache()
-
     # per-launch times of the fused step and the rgbnet's share
     m.load_state_dict(state0)
     opt = create_optimizer_or_freeze_model(m, cfg, global_step=0)
@@ -141,29 +156,30 @@ def bench(name, s, args):
     res['instrumented_step_ms'] = step_ms
     res['rgbnet_share_of_step'] = (k.get('rgbnet_fwd', 0.0) + k.get('rgbnet_bwd', 0.0)) / step_ms
     del opt
-    m.cpu()
     torch.cuda.empty_cache()
 
+    # the legs alternated round by round; this package's model leaves the GPU while the reference's runs
     ref = _reference()
+    times = {leg: [] for leg in ('fused', 'forward_ops', 'reference_gpu')}
+    for _ in range(args.rounds):
+        m.cuda()
+        for leg in ('fused', 'forward_ops'):
+            m.load_state_dict(state0)
+            opt = create_optimizer_or_freeze_model(m, cfg, global_step=0)
+            fwd = m.forward if leg == 'fused' else m.forward_ops
+            times[leg].append(_time(lambda i: _train_step(m, opt, fwd, ro, rd, vd, target, i + 1, s['w_main']), args.steps,
+                                    args.warmup))
+            del opt
+        m.cpu()
+        torch.cuda.empty_cache()
+        if ref is not None:
+            times['reference_gpu'].append(_reference_leg(ref, s, state0, ro, rd, vd, target, args))
+            torch.cuda.empty_cache()
+    res['train_step_ms_rounds'] = times
+    res['train_step_ms'] = {leg: min(v) for leg, v in times.items() if v}
     if ref is None:
         res['train_step_ms']['reference_gpu'] = {'unavailable': 'oracle/_ref not built (needs the reference checkout at build time)'}
     else:
-        fgm, madam = ref
-        from oracle import ref_gpu_py
-        kw = dict(_kwargs(s), xyz_min=np.array([-1.] * 3, dtype=np.float32), xyz_max=np.array([1.] * 3, dtype=np.float32))
-        ref_gpu_py.default_cuda(True)           # run_FourierGrid.py:87: the reference allocates with the default tensor type
-        try:
-            with contextlib.redirect_stdout(io.StringIO()):
-                rm = fgm.FourierGridModel(**kw)
-            rm.load_state_dict(state0, strict=False)
-            rm = rm.cuda()
-            ropt = madam.MaskedAdam([{'params': [rm.density.grid], 'lr': 0.1, 'skip_zero_grad': True},
-                                     {'params': [rm.k0.grid], 'lr': 0.1, 'skip_zero_grad': True},
-                                     {'params': list(rm.rgbnet.parameters()), 'lr': 1e-3, 'skip_zero_grad': False}])
-            res['train_step_ms']['reference_gpu'] = _time(
-                lambda i: _train_step(rm, ropt, rm.forward, ro, rd, vd, target, i + 1, s['w_main']), args.steps, args.warmup)
-        finally:
-            ref_gpu_py.default_cuda(False)
         res['speedup_vs_reference_gpu'] = res['train_step_ms']['reference_gpu'] / res['train_step_ms']['fused']
     res['speedup_vs_forward_ops'] = res['train_step_ms']['forward_ops'] / res['train_step_ms']['fused']
     return res
@@ -173,6 +189,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--steps', type=int, default=10)
     ap.add_argument('--warmup', type=int, default=3)
+    ap.add_argument('--rounds', type=int, default=3)
     ap.add_argument('--only', choices=list(SHAPES), default=None)
     args = ap.parse_args()
     assert torch.cuda.is_available(), 'bench_fg_widths.py needs a GPU'

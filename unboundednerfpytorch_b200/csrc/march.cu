@@ -493,7 +493,7 @@ static int g_density_scatter = 1;      // 1 = run-merging two-launch scatter (de
 static int get_density_scatter() { return g_density_scatter; }
 
 static bool feature_grid_ok(const GridView& g) {
-  if (g.C == 3 || g.C == 15)      // march_feature.cu's scalar-channel kernels: 4-byte aligned records, odd P <= 11, >= 2 voxels per axis
+  if (g.C == 3 || g.C == 9 || g.C == 15)   // march_feature.cu's scalar-channel kernels: 4-byte aligned records, odd P <= 11, >= 2 voxels per axis
     return g.sc == 1 && g.sv == g.C && g.P >= 1 && g.P <= 11 && (g.P & 1) && g.X >= 2 && g.Y >= 2 && g.Z >= 2 &&
            ((uintptr_t)g.data & 3) == 0;
   return g.sc == 1 && g.sv == g.C && (g.C == 4 || g.C == 8 || g.C == 12 || g.C == 16) && g.P <= 16 &&
@@ -646,7 +646,7 @@ int ubn_march_feature_fwd(const float* rays_o, const float* rays_d, const float*
                                    as_stream(stream));
     if (e >= 0) return e;
   }
-  if (g.C % 4) return finish(cudaErrorInvalidValue);     // C = 3 / 15 beyond 32-bit slab offsets: no kernel
+  if (g.C % 4) return finish(cudaErrorInvalidValue);     // C = 3 / 9 / 15 beyond 32-bit slab offsets: no kernel
   const size_t smem = sizeof(float4) * kMarchWarps * 32 * g.P;
   k_march_feature<false><<<blocks_for(n_rays, kMarchWarps), 32 * kMarchWarps, smem, as_stream(stream)>>>(
       rays_o, rays_d, t_table, g, p, n_rays, flags, offsets, density, alpha, weight, k0_feat, nullptr, out_density,
@@ -668,7 +668,7 @@ int ubn_march_feature_bwd(const float* rays_o, const float* rays_d, const float*
                                    nullptr, nullptr, as_stream(stream));
     if (e >= 0) return e;
   }
-  if (g.C % 4) return finish(cudaErrorInvalidValue);     // C = 3 / 15 beyond 32-bit slab offsets: no kernel
+  if (g.C % 4) return finish(cudaErrorInvalidValue);     // C = 3 / 9 / 15 beyond 32-bit slab offsets: no kernel
   const size_t smem = sizeof(float4) * kMarchWarps * 32 * g.P;
   k_march_feature<true><<<blocks_for(n_rays, kMarchWarps), 32 * kMarchWarps, smem, as_stream(stream)>>>(
       rays_o, rays_d, t_table, g, p, n_rays, flags, offsets, nullptr, nullptr, nullptr, const_cast<float*>(grad_feat),

@@ -279,6 +279,18 @@ __device__ __forceinline__ void red_add_from(float* q, const float* v) {
   }
 }
 
+// q[0 .. kC) += v for a record that starts at any of the four 4-byte phases of a 16-byte line: one unrolled reduction sequence
+// per phase, so every channel index is a compile-time constant and v stays in registers
+template <int kC>
+__device__ __forceinline__ void red_add_record_phased(float* q, const float* v) {
+  switch ((reinterpret_cast<uintptr_t>(q) >> 2) & 3) {
+    case 0: red_add_from<kC, 0, 0>(q, v); break;
+    case 1: red_add_from<kC, 0, 1>(q, v); break;
+    case 2: red_add_from<kC, 0, 2>(q, v); break;
+    default: red_add_from<kC, 0, 3>(q, v); break;
+  }
+}
+
 // q[0 .. kC) += v with the widest reductions each address allows (red.v4 at 16-byte, red.v2 at 8-byte alignment, scalar
 // otherwise): the k0 scatters of the NDC / box march (C = 3, 9, 12) and of the contracted march at C = 3 and 15
 template <int kC>
@@ -299,12 +311,7 @@ __device__ __forceinline__ void red_add_record(float* q, const float* v) {
     return;
   }
   if constexpr (kC == 15) {                   // a 60-byte record starts at any of the four phases of a 16-byte line
-    switch ((reinterpret_cast<uintptr_t>(q) >> 2) & 3) {
-      case 0: red_add_from<kC, 0, 0>(q, v); break;
-      case 1: red_add_from<kC, 0, 1>(q, v); break;
-      case 2: red_add_from<kC, 0, 2>(q, v); break;
-      default: red_add_from<kC, 0, 3>(q, v); break;
-    }
+    red_add_record_phased<kC>(q, v);
     return;
   }
   int ch = 0;

@@ -581,9 +581,9 @@ static int launch_bwd_slab(const float* rays_o, const float* rays_d, const float
 }
 
 // =====================================================================================================================
-// C = 3 and C = 15 (FourierGridModel with rgbnet_dim = 3 -- the Waymo / Mega-NeRF configs -- or 15, and every colour-grid stage
-// with rgbnet_dim <= 0).  A 12- or 60-byte record is only 4-byte aligned, so neither the float4 quads of the kernels above nor
-// their lane roles apply.
+// C = 3, 9 and 15 (FourierGridModel with rgbnet_dim = 3 -- the Waymo / Mega-NeRF configs --, 9 -- the free-dataset grass config --
+// or 15, DirectContractedVoxGO at the same widths, and every colour-grid stage with rgbnet_dim <= 0).  A 12-, 36- or 60-byte record
+// is only 4-byte aligned, so neither the float4 quads of the kernels above nor their lane roles apply.
 //   Gather: lane = sample, as k_march_feature_v3: scalar loads, every channel accumulated in ATen's corner order (fma chain
 //   tnw .. bse) and the slabs combined in torch-CUDA's mean order, so the features are bit-identical to
 //   F.grid_sample(...).mean(0).
@@ -677,6 +677,14 @@ __global__ void __launch_bounds__(32 * kMarchWarps, 4) k_march_feature_narrow(
   }
 }
 
+// a record of the run scatter: red_add_record, except at C = 9, where its generic loop (which DirectMPIGO's scatter keeps) would
+// index the sum with a run-time channel and keep it in local memory
+template <int kC>
+__device__ __forceinline__ void red_add_narrow(float* q, const float* v) {
+  if constexpr (kC == 9) red_add_record_phased<kC>(q, v);
+  else red_add_record<kC>(q, v);
+}
+
 template <int kC, int kP>
 __global__ void __launch_bounds__(32 * kMarchWarps, 8) k_march_feature_bwd_narrow(
     const float* __restrict__ rays_o, const float* __restrict__ rays_d, const float* __restrict__ t_table,
@@ -744,7 +752,7 @@ __global__ void __launch_bounds__(32 * kMarchWarps, 8) k_march_feature_bwd_narro
       const float wgt = slab_mean_scale(((bz ? fz : 1.f - fz) * (by ? fy : 1.f - fy)) * (bx ? fx : 1.f - fx), kP);
       const float* gi = gfeat + (out_base + rj) * kC;
       if (v != open) {
-        if (open >= 0) red_add_record<kC>(slab + (int64_t)open * kC, acc);
+        if (open >= 0) red_add_narrow<kC>(slab + (int64_t)open * kC, acc);
         open = v;
 #pragma unroll
         for (int c = 0; c < kC; ++c) acc[c] = wgt * __ldg(gi + c);
@@ -753,7 +761,7 @@ __global__ void __launch_bounds__(32 * kMarchWarps, 8) k_march_feature_bwd_narro
         for (int c = 0; c < kC; ++c) acc[c] += wgt * __ldg(gi + c);
       }
     }
-    if (open >= 0) red_add_record<kC>(slab + (int64_t)open * kC, acc);
+    if (open >= 0) red_add_narrow<kC>(slab + (int64_t)open * kC, acc);
     out_base += __popc(km);
   }
 }
@@ -822,10 +830,13 @@ int march_feature_v2(bool backward, const float* rays_o, const float* rays_d, co
                      uint8_t* o_inner, cudaStream_t st) {
   if (g.X < 2 || g.Y < 2 || g.Z < 2) return -1;
   if ((int64_t)g.X * g.Y * g.Z * g.C >= (1ll << 31)) return -1;   // 32-bit voxel offsets inside a slab
-  if (g.C == 3 || g.C == 15) {                            // every variant: the lane-per-sample gather, the slab-major run scatter
+  if (g.C == 3 || g.C == 9 || g.C == 15) {               // every variant: the lane-per-sample gather, the slab-major run scatter
     const int n_split = g_feature_kernel == 4 ? 2 : g_feature_kernel == 5 ? 4 : 1;
     if (g.C == 3)
       return march_feature_narrow<3>(backward, rays_o, rays_d, t_table, g, p, n_rays, flags, offsets, density, alpha, weight, feat,
+                                     grad_grid, o_density, o_alpha, o_weight, o_ray_id, o_step_id, o_t, o_inner, n_split, st);
+    if (g.C == 9)
+      return march_feature_narrow<9>(backward, rays_o, rays_d, t_table, g, p, n_rays, flags, offsets, density, alpha, weight, feat,
                                      grad_grid, o_density, o_alpha, o_weight, o_ray_id, o_step_id, o_t, o_inner, n_split, st);
     return march_feature_narrow<15>(backward, rays_o, rays_d, t_table, g, p, n_rays, flags, offsets, density, alpha, weight, feat,
                                     grad_grid, o_density, o_alpha, o_weight, o_ray_id, o_step_id, o_t, o_inner, n_split, st);

@@ -2,9 +2,10 @@
 // (DirectVoxGO.forward, dvgo.py:365-366), and their adjoints.
 //
 // Pass A and its backward are the contracted march's kernels (march.cu) instantiated with NdcSampler / BoxSampler.  The feature
-// read is separate because these models' k0 grids are single-slab with C = 9 (LLFF), 12 (DVGO fine stage) or 3 (rgbnet_dim = 0)
-// channels: a 36- or 12-byte channels-last record is only 4-byte aligned, so the float4 quads of the contracted kernels do not
-// apply there; a 48-byte record (C = 12) is 16-byte aligned and is read with float4 loads.  The sampling policy is a template
+// read is separate because these models' k0 grids are single-slab with C = 9 (LLFF, and DVGO on the free-dataset lab config),
+// 12 (DVGO fine stage) or 3 (rgbnet_dim = 0) channels: a 36- or 12-byte channels-last record is only 4-byte aligned, so the
+// float4 quads of the contracted kernels do not apply there; a 48-byte record (C = 12) is 16-byte aligned and is read with
+// float4 loads.  The sampling policy is a template
 // parameter: the box march's rays stop at their own n_steps.
 //
 // Lane = sample: each lane that holds a survivor of the current 32-sample chunk reads its 8 corner records with scalar loads and
@@ -157,9 +158,9 @@ static bool ndc_feature_grid_ok(const GridView& g) {
          (int64_t)g.X * g.Y * g.Z < (1ll << 31) && ((uintptr_t)g.data & 3) == 0;
 }
 
-// the box march's k0: single slab, channels-last, C in {3, 12}, 16-byte aligned for C = 12 (float4 records)
+// the box march's k0: single slab, channels-last, C in {3, 9, 12}, 16-byte aligned for C = 12 (float4 records), 4-byte otherwise
 static bool box_feature_grid_ok(const GridView& g) {
-  return g.P == 1 && g.sc == 1 && g.sv == g.C && (g.C == 3 || g.C == 12) && g.X >= 2 && g.Y >= 2 && g.Z >= 2 &&
+  return g.P == 1 && g.sc == 1 && g.sv == g.C && (g.C == 3 || g.C == 9 || g.C == 12) && g.X >= 2 && g.Y >= 2 && g.Z >= 2 &&
          (int64_t)g.X * g.Y * g.Z < (1ll << 31) && ((uintptr_t)g.data & (g.C == 12 ? 15 : 3)) == 0;
 }
 
@@ -173,6 +174,7 @@ static int launch_ndc_feature(const float* rays_o, const float* rays_d, const Gr
       rays_o, rays_d, g, p, n_rays, flags, offsets, alpha, weight, feat, grad_grid, o_alpha, o_weight, o_ray_id, o_step_id)
   if constexpr (std::is_same<Smp, BoxSampler>::value) {
     if (g.C == 12) UBN_NDC_FEAT(12);
+    else if (g.C == 9) UBN_NDC_FEAT(9);
     else UBN_NDC_FEAT(3);
   } else {
     if (g.C == 9) UBN_NDC_FEAT(9);

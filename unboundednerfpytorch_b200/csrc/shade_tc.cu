@@ -1303,8 +1303,8 @@ int rgbnet_bwd_tc_fused_w(const float* feat, const int64_t* ray_id, const float*
                           const float* rgb, const float* h1_save, const float* h2_save, const float* grad_rgb, int64_t n_pts,
                           float* grad_feat, float* grad_view_bias, float* grad_W1k, float* grad_W2, float* grad_b2, float* grad_W3,
                           float* grad_b3, uint32_t* h2_mask_scratch, const uint32_t* h1_mask, int single_pass, void* stream) {
+  if (n_pts <= 0) return 0;              // a batch without survivors: its zero-sized mask buffers have no address
   if ((single_pass & 4) == 0 || h1_mask == nullptr || h2_mask_scratch == nullptr) return finish(cudaErrorInvalidValue);
-  if (n_pts <= 0) return 0;
   const bool one = (single_pass & 1) != 0;
   cudaStream_t st = as_stream(stream);
   constexpr int W = tc::w64::kBwdWarps, C = tc::w64::kBwdCtas, C2 = tc::w64::kDw2Ctas;

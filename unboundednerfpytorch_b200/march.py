@@ -373,9 +373,9 @@ def box_density_supported(density_grid):
 
 
 def box_k0_supported(k0_grid):
-    """k0 grids the box march's pass B reads: single slab, channels-last, 3 or 12 channels (16-byte aligned records for 12),
+    """k0 grids the box march's pass B reads: single slab, channels-last, 3, 9 or 12 channels (16-byte aligned records for 12),
     >= 2 voxels per axis, 32-bit voxel offsets."""
-    return (k0_grid.is_cuda and k0_grid.dim() == 5 and k0_grid.shape[0] == 1 and k0_grid.shape[1] in (3, 12)
+    return (k0_grid.is_cuda and k0_grid.dim() == 5 and k0_grid.shape[0] == 1 and k0_grid.shape[1] in (3, 9, 12)
             and k0_grid.stride(1) == 1 and k0_grid.stride(4) == k0_grid.shape[1] and min(k0_grid.shape[2:]) >= 2
             and k0_grid[0, 0].numel() < 2 ** 31 and (k0_grid.shape[1] != 12 or k0_grid.data_ptr() % 16 == 0))
 

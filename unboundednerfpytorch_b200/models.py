@@ -219,7 +219,7 @@ class _ContractedBase(_GridModel):
     # ---- the fused forward --------------------------------------------------------------------------
     def _fused_ok(self):
         kg = self.k0.grid
-        if kg.shape[1] in (3, 15):         # march_feature.cu's scalar-channel kernels: odd slab counts up to 11
+        if kg.shape[1] in (3, 9, 15):      # march_feature.cu's scalar-channel kernels: odd slab counts up to 11
             return (kg.is_cuda and kg.shape[0] in (1, 3, 5, 7, 9, 11) and kg.stride(1) == 1 and min(kg.shape[2:]) >= 2
                     and kg[0].numel() < 2 ** 31)       # 32-bit offsets inside a slab
         return kg.is_cuda and kg.shape[1] in (4, 8, 12, 16) and kg.shape[0] <= 16

@@ -6,8 +6,8 @@ The view-direction half of the first Linear is constant along a ray, so the host
 ``vb = emb(viewdirs) @ W1[:, K:].T + b1`` ([N,W], one tiny GEMM that torch differentiates for dW1[:,K:], db1) and the
 kernel runs the per-sample part: K -> W -> W -> 3 with the activations resident on chip, fp32 arithmetic.  W = 128 with K = 12
 (every 12-channel config) has every engine below; K = 3 (rgbnet_dim = 3: the Waymo / Mega-NeRF FourierGrid configs), K = 15
-(Tanks&Temples Train) and W = 64 with K = 9 (DirectMPIGO of llff_default) run the tensor-core forward and the fused backward with
-ReLU masks, at the precision UBN_RGBNET_MODE picks.
+(Tanks&Temples Train) and W = 64 with K = 9 (DirectMPIGO of llff_default; FourierGridModel and DirectVoxGO of the free-dataset
+grass and lab configs) run the tensor-core forward and the fused backward with ReLU masks, at the precision UBN_RGBNET_MODE picks.
 """
 import torch
 
@@ -122,7 +122,7 @@ class _ShadeFn(torch.autograd.Function):
         return g_feat, g_vb, None, gW1k, gW2, gb2, gW3, gb3, None
 
 
-# (features, hidden width) pairs with kernels: rgbnet_dim 3 / 12 / 15 at width 128, and DirectMPIGO's llff_default (9, 64)
+# (features, hidden width) pairs with kernels: rgbnet_dim 3 / 12 / 15 at width 128, and (9, 64): llff_default, free-dataset grass / lab
 KERNEL_SHAPES = {(3, 128), (12, 128), (15, 128), (9, 64)}
 
 
