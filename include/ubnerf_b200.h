@@ -655,6 +655,18 @@ int ubn_lattice_bounds(const float* grid, const UbnGridDesc* desc, const float* 
 int ubn_lattice_bounds_alpha(const float* alpha, const float* lattice_min, const float* lattice_max, int64_t X, int64_t Y,
                              int64_t Z, float thres, float* bounds, int64_t* count, void* stream);
 
+/* ---- image metrics (FourierGrid/utils.py) ------------------------------------------------------------------------------------ */
+#define UBN_SSIM_MAX_TAPS 32
+#define UBN_SSIM_MAX_CTAS 1056
+/* utils.rgb_ssim (utils.py:79-125) of one frame pair: img0, img1 contiguous fp32 [H, W, 3] (device); the separable 1-D Gaussian
+ * taps[filter_size] (HOST fp64, 1 <= filter_size <= UBN_SSIM_MAX_TAPS, H and W >= filter_size) applied to each channel in 'valid'
+ * mode; c1 = (k1 * max_val)^2, c2 = (k2 * max_val)^2.  The products img0^2, img1^2, img0 * img1 are rounded to fp32, the five
+ * filtered moments and everything after them are fp64, the epilogue in numpy's order with no contraction, and NaN propagates as
+ * in numpy.  Writes the map [H - f + 1, W - f + 1, 3] (fp64, when map != NULL) and *mean (device fp64).  scratch: device fp64,
+ * at least UBN_SSIM_MAX_CTAS (per-block partial sums, added in a fixed order: the mean is deterministic). */
+int ubn_rgb_ssim(const float* img0, const float* img1, int64_t H, int64_t W, int filter_size, const double* taps, double c1,
+                 double c2, double* map, double* scratch, double* mean, void* stream);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

@@ -4,7 +4,7 @@ to this package instead of the reference's ``python setup.py install`` build (RE
 
 ``install_models(*modules)`` goes one step further: it points the reference modules' own names for the model classes and the
 optimizer factory at this package's, so run_train.py / run_render.py / FourierGrid_ckpt_manager.py run unedited on the fused
-models (INTEGRATION.md §3)."""
+models (INTEGRATION.md §3).  ``install_metrics(*modules)`` does the same for the evaluation score utils.rgb_ssim."""
 import importlib
 import sys
 
@@ -36,7 +36,7 @@ def model_names():
 
 
 class ModelPatch:
-    """What install_models changed: ``restore()`` (or leaving the ``with`` block) puts every original name back."""
+    """What install_models / install_metrics changed: ``restore()`` (or leaving the ``with`` block) puts every original name back."""
 
     def __init__(self, saved):
         self.saved = saved          # [(module, name, original object)]
@@ -59,7 +59,18 @@ def install_models(*reference_modules):
     masked_adam ...), rebind every name of model_names() the module defines to this package's class or function.  Callers
     that look the names up at call time -- create_new_model, load_existing_model, the isinstance checks of run_train.py:191-196
     -- then build, load and rescale the fused models with no edit.  Returns a ModelPatch that restores the originals."""
-    table = model_names()
+    return _rebind(reference_modules, model_names())
+
+
+def install_metrics(*reference_modules):
+    """In each given reference module that defines ``rgb_ssim`` (utils.py:79-125), rebind it to metrics.rgb_ssim: same arguments,
+    same result types, computed on the GPU.  run_render.render_viewpoints looks it up as ``utils.rgb_ssim`` at call time, so with
+    install_metrics(utils) its ``eval_ssim`` scores on the GPU with no edit.  Returns a ModelPatch that restores the originals."""
+    from .. import metrics
+    return _rebind(reference_modules, {'rgb_ssim': metrics.rgb_ssim})
+
+
+def _rebind(reference_modules, table):
     saved = []
     for module in reference_modules:
         for name, ours in table.items():

@@ -10,13 +10,14 @@ SURVEY.md 8e:
 * ``render_blocks_idw``         -- Block-NeRF style (eval_block_nerf.py:95-133, :215-216): one spatial block per rank, every rank
                                    renders the same frame, blocks that do not see the view are gated out, the frame is the
                                    inverse-distance-weighted mean of the visible blocks' images (one all-reduce).
-Out of scope (raise): SSIM / LPIPS evaluation (third-party metric networks)."""
+``eval_ssim`` scores each frame on the device (metrics.rgb_ssim); LPIPS raises (it needs pretrained network weights)."""
 import os
 
 import numpy as np
 import torch
 
 from . import dist as D
+from . import metrics as M
 from . import rays as R
 
 KEYS = ('rgb_marched', 'depth', 'alphainv_last')
@@ -89,9 +90,17 @@ def render_viewpoints(cfg, model, render_poses, HW, Ks, ndc, render_kwargs, gt_i
                       render_factor=0, render_video_flipy=False, render_video_rot90=0, eval_ssim=False, eval_lpips_alex=False,
                       eval_lpips_vgg=False, verbose=True, chunk=8192):
     """run_render.py:15-114.  ``cfg`` only supplies cfg.data.flip_x / flip_y (None -> False).  Returns (rgbs, depths, bgmaps) as
-    numpy arrays [n_views, H, W, K] like the reference; prints the average PSNR when ``gt_imgs`` is given."""
-    if eval_ssim or eval_lpips_alex or eval_lpips_vgg:
-        raise NotImplementedError('SSIM / LPIPS evaluation is outside the hot-path scope (third-party metric networks)')
+    numpy arrays [n_views, H, W, K] like the reference; prints the average PSNR when ``gt_imgs`` is given.
+
+    ``eval_ssim`` scores each frame against its ``gt_imgs`` entry with metrics.rgb_ssim(max_val=1) while the frame is still on
+    the device, and prints ``Ssim <mean> (avg)`` after the Psnr line.  The reference scores only where it computes PSNR -- with
+    ``gt_imgs`` and ``render_factor == 0`` -- and silently skips SSIM elsewhere; here ``eval_ssim`` outside that case raises
+    NotImplementedError, so a requested score is never dropped without notice.  LPIPS raises: it needs pretrained networks."""
+    if eval_lpips_alex or eval_lpips_vgg:
+        raise NotImplementedError('LPIPS evaluation needs pretrained network weights, which this package does not ship')
+    if eval_ssim and (gt_imgs is None or render_factor != 0):
+        raise NotImplementedError('eval_ssim scores rendered frames against gt_imgs at render_factor 0 only (as run_render.py '
+                                  'does); here there is nothing to score')
     assert len(render_poses) == len(HW) and len(HW) == len(Ks)
     HW, Ks = np.asarray(HW), np.asarray(Ks, dtype=np.float64)
     if render_factor != 0:
@@ -101,14 +110,17 @@ def render_viewpoints(cfg, model, render_poses, HW, Ks, ndc, render_kwargs, gt_i
     data = getattr(cfg, 'data', None)
     flip_x, flip_y = bool(getattr(data, 'flip_x', False)), bool(getattr(data, 'flip_y', False))
     dev = next(model.parameters()).device
-    rgbs, depths, bgmaps, psnrs = [], [], [], []
+    rgbs, depths, bgmaps, psnrs, ssims = [], [], [], [], []
     rk = {k: v for k, v in render_kwargs.items() if k != 'indexs'}
     for i, c2w in enumerate(render_poses):
         H, W = int(HW[i][0]), int(HW[i][1])
         c2w = torch.as_tensor(np.asarray(c2w), dtype=torch.float32)
         ro, rd, vd = R._rays_of_a_view(H, W, Ks[i], c2w, ndc, rk.get('inverse_y', False), flip_x, flip_y, 'center', device=dev)
         res = render_frame_sharded(model, ro.view(-1, 3), rd.view(-1, 3), vd.view(-1, 3), rk, chunk)
-        rgb = res['rgb_marched'].reshape(H, W, -1).cpu().numpy()
+        frame = res['rgb_marched'].reshape(H, W, -1)
+        if eval_ssim:
+            ssims.append(M.rgb_ssim(frame, torch.as_tensor(gt_imgs[i], device=dev), max_val=1))
+        rgb = frame.cpu().numpy()
         rgbs.append(rgb)
         depths.append(res['depth'].reshape(H, W, -1).cpu().numpy())
         bgmaps.append(res['alphainv_last'].reshape(H, W, -1).cpu().numpy())
@@ -116,6 +128,8 @@ def render_viewpoints(cfg, model, render_poses, HW, Ks, ndc, render_kwargs, gt_i
             psnrs.append(-10. * np.log10(np.mean(np.square(rgb - gt_imgs[i]))))
     if len(psnrs) and verbose:
         print('Psnr', np.mean(psnrs), '(avg)')
+        if eval_ssim:
+            print('Ssim', np.mean(torch.stack(ssims).cpu().numpy()), '(avg)')
     if render_video_flipy:
         rgbs, depths, bgmaps = ([np.flip(x, axis=0) for x in xs] for xs in (rgbs, depths, bgmaps))
     if render_video_rot90 != 0:
