@@ -64,44 +64,3 @@ def test_block_idw_composite_world1_and_visibility_gate():
     rgb2, info2 = RD.render_blocks_idw(m, ro, rd, vd, rk, centroid=[0.5, 0., 0.], cam_origin=[0., 0., 0.])
     assert not bool(info2['visible']) and float(info2['den']) == 0.0
 
-
-def test_tma_staged_feature_read_matches_the_gather_kernel():
-    """csrc/render_tma.cu: bricks staged by TMA for 32 adjacent rays x 4 steps.  Same survivors, same per-sample records, features
-    equal to the warp-cooperative gather kernel to fp32 rounding; coherent (image-ordered) rays are served by TMA, random rays by
-    the in-kernel fallback -- with identical results either way."""
-    from tests.util import seeded_rays
-    from unboundednerfpytorch_b200 import march, rays as R
-    m = _model(7)
-    H, W = 48, 64
-    K = np.array([[float(W), 0., W / 2], [0., float(W), H / 2], [0., 0., 1.]])
-    c2w = torch.tensor([[1., 0., 0., 0.1], [0., 1., 0., -0.2], [0., 0., 1., 0.3]])
-    ro, rd, vd = (t.view(-1, 3) for t in R.get_rays_of_a_view(H, W, K, c2w, False, False, False, False))
-    rk = dict(near=0., far=1e9, bg=1, rand_bkgd=False, stepsize=0.5, render_depth=True)
-    stats = torch.zeros(2, dtype=torch.int64, device=DEV)
-    march.TMA_STATS = stats
-    try:
-        with torch.no_grad():
-            a = m(ro, rd, vd, coherent_rays=True, **rk)
-            n_tma, n_fb = [int(v) for v in stats.tolist()]
-            b = m(ro, rd, vd, **rk)
-            stats.zero_()
-            ro2, rd2, vd2 = seeded_rays(3001, 5, DEV)                     # random rays, ragged last warp
-            c = m(ro2, rd2, vd2, coherent_rays=True, **rk)
-            n_tma2, n_fb2 = [int(v) for v in stats.tolist()]
-            d = m(ro2, rd2, vd2, **rk)
-    finally:
-        march.TMA_STATS = None
-    print(f'[tma] coherent 64x48 frame: {n_tma} blocks by TMA, {n_fb} by the fallback; random rays: {n_tma2} / {n_fb2}')
-    assert n_tma > 4 * max(n_fb, 1), (n_tma, n_fb)        # image-ordered rays (coarse 64-px-wide view): bricks, not gathers
-    assert n_fb2 > n_tma2, (n_tma2, n_fb2)                                # random rays: mostly the fallback
-    for x, y, nm in ((a, b, 'coherent'), (c, d, 'random')):
-        assert torch.equal(x['ray_id'], y['ray_id']) and torch.equal(x['step_id'], y['step_id']), nm
-        for k in ('weights', 'raw_alpha', 'raw_density', 't', 'alphainv_last'):
-            assert torch.equal(x[k], y[k]), f'{nm} {k}'                   # pass A is shared, the records are copied
-        for k in ('raw_rgb', 'rgb_marched', 'depth'):
-            assert_close(x[k], y[k], rtol=1e-5, atol=2e-6, what=f'{nm} {k}')
-    # and against the op-by-op composition (stand-alone grid op in ATen's corner order)
-    with torch.no_grad():
-        e = m.forward_ops(ro, rd, vd, global_step=None, **rk)
-    assert torch.equal(a['ray_id'], e['ray_id'])
-    assert_close(a['rgb_marched'], e['rgb_marched'], rtol=1e-5, atol=2e-6, what='tma vs ops')

@@ -17,7 +17,11 @@
 // (16-byte loads, 4 bytes of flags per step block).  First version (one warp per ray group, all 128 blocks): 3x slower than the
 // gather kernel on the garden frame, because 64 CTAs per chunk left more than half of the SMs idle.
 // The trilinear sum runs in ATen's corner order (tnw .. bse, FMA chain), so the features are bit-identical to the stand-alone
-// grid op (trilinear.cu) and to torch F.grid_sample, which the reference calls.  Outputs = those of ubn_march_feature_fwd.
+// grid op (trilinear.cu) and to torch F.grid_sample, which the reference calls, at every sample whose unnormalised coordinates
+// ((c + 1) / 2) * (size - 1) lie in [0, size - 1] -- every sample of the contracted models, whose points stay inside the k0
+// grid's bounds.  A coordinate beyond a face (a k0 grid with narrower bounds than the points) keeps its clamped cell (cell_of,
+// as march_feature.cu::make_cell) and extrapolates linearly, where F.grid_sample zero-pads the corners past the face.
+// Outputs = those of ubn_march_feature_fwd.
 #include <cuda.h>
 
 #include <algorithm>
