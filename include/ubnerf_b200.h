@@ -667,6 +667,20 @@ int ubn_lattice_bounds_alpha(const float* alpha, const float* lattice_min, const
 int ubn_rgb_ssim(const float* img0, const float* img1, int64_t H, int64_t W, int filter_size, const double* taps, double c1,
                  double c2, double* map, double* scratch, double* mean, void* stream);
 
+/* ---- colour transfer of the ARF stylizer (FourierGrid/arf.py) ----------------------------------------------------------------- */
+#define UBN_COLOR_MAX_CTAS 1056
+/* The moments of arf.py:65-69 (mu_c / mu_s = mean(0), cov_c / cov_s = (X - mu)^T (X - mu) / n) of n_px >= 1 packed RGB fp32 pixels
+ * px[n_px * 3] (device, 4-byte aligned; any offset).  Sums of d = x - k and of the six products d_i d_j, with k the first pixel,
+ * are accumulated in fp64 and reduced in a fixed order (per-block partials in scratch, added in block order by a closing
+ * launch): two calls give the same bits.  Writes out[9] (device fp64) = mean (k + sum(d) / n, 3 values) and the population
+ * covariance's upper triangle c00, c01, c02, c11, c12, c22.  scratch: device fp64, at least 9 * UBN_COLOR_MAX_CTAS. */
+int ubn_color_moments(const float* px, int64_t n_px, double* scratch, double* out, void* stream);
+/* The transform of arf.py:83-84 (image_set @ tmp_mat.T + tmp_vec, clamp_(0, 1)) on packed RGB fp32 pixels in[n_px * 3] ->
+ * out[n_px * 3] (device, 4-byte aligned; in == out is allowed).  T[9] (row-major 3 x 3) and b[3] are HOST fp32, passed to the
+ * kernel by value.  Channel c is fma(T[3c+2], x2, fma(T[3c+1], x1, fma(T[3c], x0, b[c]))), clamped as torch.clamp_ (NaN stays
+ * NaN). */
+int ubn_color_affine(const float* in, float* out, int64_t n_px, const float* T, const float* b, void* stream);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

@@ -34,6 +34,7 @@ class UbnTensorfDesc(ctypes.Structure):
 TENSORF_BWD_MAX_CTAS = 528   # UBN_TENSORF_BWD_MAX_CTAS of include/ubnerf_b200.h
 SSIM_MAX_TAPS = 32           # UBN_SSIM_MAX_TAPS
 SSIM_MAX_CTAS = 1056         # UBN_SSIM_MAX_CTAS
+COLOR_MAX_CTAS = 1056        # UBN_COLOR_MAX_CTAS
 
 
 class UbnMarchCfg(ctypes.Structure):
@@ -161,6 +162,8 @@ _SIGNATURES = {
     'ubn_lattice_bounds_alpha': [c_p, c_p, c_p, c_i64, c_i64, c_i64, c_f, c_p, c_p, c_p],
     'ubn_rgb_ssim': [c_p, c_p, c_i64, c_i64, c_int, ctypes.POINTER(ctypes.c_double), ctypes.c_double, ctypes.c_double,
                      c_p, c_p, c_p, c_p],
+    'ubn_color_moments': [c_p, c_i64, c_p, c_p, c_p],
+    'ubn_color_affine': [c_p, c_p, c_i64, ctypes.POINTER(c_f), ctypes.POINTER(c_f), c_p],
 }
 _RESTYPE = {'ubn_last_error_string': ctypes.c_char_p, 'ubn_launch_count': c_i64, 'ubn_reset_launch_count': None}
 

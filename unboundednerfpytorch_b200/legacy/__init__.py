@@ -4,7 +4,8 @@ to this package instead of the reference's ``python setup.py install`` build (RE
 
 ``install_models(*modules)`` goes one step further: it points the reference modules' own names for the model classes and the
 optimizer factory at this package's, so run_train.py / run_render.py / FourierGrid_ckpt_manager.py run unedited on the fused
-models (INTEGRATION.md §3).  ``install_metrics(*modules)`` does the same for the evaluation score utils.rgb_ssim."""
+models (INTEGRATION.md §3).  ``install_metrics(*modules)`` does the same for the evaluation score utils.rgb_ssim, and
+``install_arf(*modules)`` for the stylizer class ARF of arf.py."""
 import importlib
 import sys
 
@@ -36,7 +37,8 @@ def model_names():
 
 
 class ModelPatch:
-    """What install_models / install_metrics changed: ``restore()`` (or leaving the ``with`` block) puts every original name back."""
+    """What install_models / install_metrics / install_arf changed: ``restore()`` (or leaving the ``with`` block) puts every
+    original name back."""
 
     def __init__(self, saved):
         self.saved = saved          # [(module, name, original object)]
@@ -68,6 +70,15 @@ def install_metrics(*reference_modules):
     install_metrics(utils) its ``eval_ssim`` scores on the GPU with no edit.  Returns a ModelPatch that restores the originals."""
     from .. import metrics
     return _rebind(reference_modules, {'rgb_ssim': metrics.rgb_ssim})
+
+
+def install_arf(*reference_modules):
+    """In each given reference module that defines ``ARF`` (arf.py:9-89; run_render.py imports it by name), rebind it to
+    arf.ARF: same constructor and attributes, match_colors_for_image_set with the same result types, computed on the GPU.
+    run_render.run_render builds ``ARF(cfg, data_dict, device)`` at call time, so with install_arf(run_render) its block render
+    stylizes on the colour kernels with no edit.  Returns a ModelPatch that restores the originals."""
+    from .. import arf
+    return _rebind(reference_modules, {'ARF': arf.ARF})
 
 
 def _rebind(reference_modules, table):
