@@ -361,6 +361,23 @@ int ubn_march_feature_fwd_tma(const float* rays_o, const float* rays_d, const fl
                               float* o_density, float* o_alpha, float* o_weight, int64_t* o_ray_id, int64_t* o_step_id, float* o_t,
                               uint8_t* o_inner, unsigned long long* stats2, void* stream);
 
+/* Render a batch of rays of a contracted model (FourierGridModel / DirectContractedVoxGO) in one fused pass with no per-sample
+ * global memory: pass A's march (same arithmetic, the ray left at T < 1e-3), the k0 read of every kept sample (pass B's
+ * lane-per-sample read), the 3-layer rgbnet on the tensor cores (3xTF32; W1 NULL: sigmoid(k0), C = 3) and the composite.
+ * density_desc: C = 1 with the k0's slab count (one k0 slab without an rgbnet); k0_desc: channels-last, odd P <= 11.
+ * rgbnet (C, viewbase_pe) = (12, 4) or (3, 8), width 128: W1 [128][C + 3 + 6 viewbase_pe], b1 [128], W2 [128][128], b2, W3 [3][128],
+ * b3 (nn.Linear weights); viewdirs [n,3] feed the view embedding.  Kept samples: listed, scanned before the stop and, with
+ * fast_color_thres > 0, weight > fast_color_thres.  Outputs: rgb_marched [n,3] = sum w rgb in step order (+ alphainv_last * bg
+ * when use_bg), depth [n] = sum w (1 - 1 / (1 + t)), alphainv_last [n] (bit-identical to pass A's); optional (NULL = none):
+ * n_shaded [n], the kept samples per ray, and n_marched [n], the samples of the 32-sample chunks marched before the ray stopped.
+ * Every output is written once: deterministic and independent of how rays are batched. */
+int ubn_render_contracted(const float* rays_o, const float* rays_d, const float* viewdirs, const float* t_table,
+                          const float* density_grid, const UbnGridDesc* density_desc, const float* k0_grid,
+                          const UbnGridDesc* k0_desc, const uint8_t* mask_world, const UbnMarchCfg* cfg, int64_t n_rays,
+                          const float* W1, const float* b1, const float* W2, const float* b2, const float* W3, const float* b3,
+                          int width, int viewbase_pe, int use_bg, float bg, float* rgb_marched, float* depth,
+                          float* alphainv_last, int32_t* n_shaded, int32_t* n_marched, void* stream);
+
 /* Backward of pass B: scatter grad_feat[M,C] into grad_k0 (adjoint of the trilinear read). */
 int ubn_march_feature_bwd(const float* rays_o, const float* rays_d, const float* t_table,
                           const UbnGridDesc* k0_desc, const UbnMarchCfg* cfg, int64_t n_rays,

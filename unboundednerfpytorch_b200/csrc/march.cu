@@ -57,46 +57,9 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_fwd(
 
   for (int base = 0; base < n; base += 32) {
     const int s = base + lane;
-    const bool valid = s < n;
-    float x = 0, y = 0, z = 0;
-    bool inner = false, in_domain = false;
-    if (valid) in_domain = Smp::point(r, t_table, s, p, x, y, z, inner);
-
-    bool queried = valid && in_domain;
-    if (p.use_cumdist) {
-      // dist[s] = || pts[s+1] - pts[s] || (torch .norm), s <= S-2; mask[s+1] |= cumdist(dist)[s]
-      float dist = 0.f;
-      if (s + 1 < S) {
-        float x1, y1, z1;
-        bool inner1;
-        Smp::point(r, t_table, s + 1, p, x1, y1, z1, inner1);
-        const float ex = __fsub_rn(x1, x), ey = __fsub_rn(y1, y), ez = __fsub_rn(z1, z);
-        dist = norm3_torch(ex, ey, ez);
-      }
-      bool over_here = false;   // result for dist index s (applies to sample s+1)
-      const int n_d = min(32, S - 1 - base);
-      for (int j = 0; j < n_d; ++j) {
-        const float dj = __shfl_sync(0xffffffffu, dist, j);
-        cum += dj;
-        const bool over = (cum > p.cumdist_thres);
-        cum *= float(!over);
-        if (lane == j) over_here = over;
-      }
-      // shift by one sample: sample s gets the flag of dist index s-1
-      const int prev = __shfl_up_sync(0xffffffffu, (int)over_here, 1);
-      const bool flag_for_me = (lane == 0) ? carry_over : (prev != 0);
-      carry_over = __shfl_sync(0xffffffffu, (int)over_here, 31) != 0;
-      queried = valid && (inner || (s > 0 && flag_for_me));
-    }
-    if (p.use_mask && queried) {
-      const int i = roundf(x * p.mscale[0] + p.mshift[0]);
-      const int j = roundf(y * p.mscale[1] + p.mshift[1]);
-      const int k = roundf(z * p.mscale[2] + p.mshift[2]);
-      bool hit = false;
-      if (0 <= i && i < p.msz[0] && 0 <= j && j < p.msz[1] && 0 <= k && k < p.msz[2])
-        hit = mask_world[((int64_t)i * p.msz[1] + j) * p.msz[2] + k] != 0;
-      queried = hit;
-    }
+    const MarchSample ms = march_chunk_point<Smp>(r, t_table, mask_world, p, base, lane, cum, carry_over);
+    const bool valid = ms.valid, inner = ms.inner, queried = ms.queried;
+    const float x = ms.x, y = ms.y, z = ms.z;
 
     float dens = 0.f, alpha = 0.f;
     if (queried) {
@@ -107,25 +70,13 @@ __global__ void __launch_bounds__(32 * kMarchWarps) k_march_density_fwd(
         dens = kP > 0 ? grid_density_fast<(kP > 0 ? kP : 1)>(g, x, y, z) : grid_density(g, x, y, z);
       }
       dens = Smp::density(p, dens, x, y, z);
-      const float e = expf(dens + p.shift);
-      alpha = 1 - powf(1 + e, -p.interval);
+      alpha = march_alpha(dens, p);
     }
-    const bool listed = queried && (p.thres > 0.f ? (alpha > p.thres) : true);
+    const bool listed = march_listed(queried, alpha, p);
 
-    // exact sequential transmittance scan over the listed samples of this chunk (alpha2weight order)
-    float myT = 1.f, myW = 0.f;
-    bool scanned = false;
-    unsigned m = __ballot_sync(0xffffffffu, listed);
-    if (!done) {
-      while (m) {
-        const int j = __ffs(m) - 1;
-        m &= m - 1;
-        const float a = __shfl_sync(0xffffffffu, alpha, j);
-        if (lane == j) { myT = T_cum; myW = T_cum * alpha; scanned = true; }
-        T_cum *= (1. - a);            // double intermediate (render_utils_kernel.cu:596)
-        if (T_cum < 1e-3) { done = true; break; }
-      }
-    }
+    float myT, myW;
+    bool scanned;
+    transmittance_scan(listed, alpha, lane, T_cum, done, myT, myW, scanned);
     const bool keep = listed && (p.thres > 0.f ? (myW > p.thres) : true);
     n_keep += __popc(__ballot_sync(0xffffffffu, keep));
 

@@ -334,4 +334,142 @@ __device__ __forceinline__ void red_add_record(float* q, const float* v) {
 
 constexpr int kMarchWarps = 4;
 
+// ------------------------------------------------------------------------------------------------
+// One 32-sample chunk of the forward march (lane = sample base + lane), shared by pass A (march.cu) and the fused render
+// (render.cu).  march_chunk_point: sample point, cumdist filter and mask cache -> whether the density is queried; the caller
+// reads the density, then march_alpha (Raw2Alpha) and march_listed (the `alpha > thres` listing).  cum / carry_over are the
+// warp-uniform cumdist state carried from chunk to chunk.
+// ------------------------------------------------------------------------------------------------
+struct MarchSample {
+  float x, y, z;
+  bool valid, inner, queried;
+};
+
+template <class Smp>
+__device__ __forceinline__ MarchSample march_chunk_point(const Ray& r, const float* __restrict__ t_table,
+                                                         const uint8_t* __restrict__ mask_world, const MarchParams& p, int base,
+                                                         int lane, float& cum, bool& carry_over) {
+  const int S = p.S;
+  const int s = base + lane;
+  MarchSample m;
+  m.valid = s < r.n;
+  m.x = 0; m.y = 0; m.z = 0;
+  m.inner = false;
+  bool in_domain = false;
+  if (m.valid) in_domain = Smp::point(r, t_table, s, p, m.x, m.y, m.z, m.inner);
+
+  bool queried = m.valid && in_domain;
+  if (p.use_cumdist) {
+    // dist[s] = || pts[s+1] - pts[s] || (torch .norm), s <= S-2; mask[s+1] |= cumdist(dist)[s]
+    float dist = 0.f;
+    if (s + 1 < S) {
+      float x1, y1, z1;
+      bool inner1;
+      Smp::point(r, t_table, s + 1, p, x1, y1, z1, inner1);
+      const float ex = __fsub_rn(x1, m.x), ey = __fsub_rn(y1, m.y), ez = __fsub_rn(z1, m.z);
+      dist = norm3_torch(ex, ey, ez);
+    }
+    bool over_here = false;   // result for dist index s (applies to sample s+1)
+    const int n_d = min(32, S - 1 - base);
+    for (int j = 0; j < n_d; ++j) {
+      const float dj = __shfl_sync(0xffffffffu, dist, j);
+      cum += dj;
+      const bool over = (cum > p.cumdist_thres);
+      cum *= float(!over);
+      if (lane == j) over_here = over;
+    }
+    // shift by one sample: sample s gets the flag of dist index s-1
+    const int prev = __shfl_up_sync(0xffffffffu, (int)over_here, 1);
+    const bool flag_for_me = (lane == 0) ? carry_over : (prev != 0);
+    carry_over = __shfl_sync(0xffffffffu, (int)over_here, 31) != 0;
+    queried = m.valid && (m.inner || (s > 0 && flag_for_me));
+  }
+  if (p.use_mask && queried) {
+    const int i = roundf(m.x * p.mscale[0] + p.mshift[0]);
+    const int j = roundf(m.y * p.mscale[1] + p.mshift[1]);
+    const int k = roundf(m.z * p.mscale[2] + p.mshift[2]);
+    bool hit = false;
+    if (0 <= i && i < p.msz[0] && 0 <= j && j < p.msz[1] && 0 <= k && k < p.msz[2])
+      hit = mask_world[((int64_t)i * p.msz[1] + j) * p.msz[2] + k] != 0;
+    queried = hit;
+  }
+
+  m.queried = queried;
+  return m;
+}
+
+// Raw2Alpha (render_utils_kernel.cu:431-443) of a queried sample's raw density
+__device__ __forceinline__ float march_alpha(float dens, const MarchParams& p) {
+  const float e = expf(dens + p.shift);
+  return 1 - powf(1 + e, -p.interval);
+}
+
+__device__ __forceinline__ bool march_listed(bool queried, float alpha, const MarchParams& p) {
+  return queried && (p.thres > 0.f ? (alpha > p.thres) : true);
+}
+
+// exact sequential transmittance scan over the listed samples of this chunk (alpha2weight order): myT / myW of the lanes it reaches,
+// T_cum and `done` (T < 1e-3, render_utils_kernel.cu:591-603) carried warp-uniform from chunk to chunk
+__device__ __forceinline__ void transmittance_scan(bool listed, float alpha, int lane, float& T_cum, bool& done, float& myT, float& myW,
+                                                   bool& scanned) {
+  myT = 1.f;
+  myW = 0.f;
+  scanned = false;
+  unsigned m = __ballot_sync(0xffffffffu, listed);
+  if (!done) {
+    while (m) {
+      const int j = __ffs(m) - 1;
+      m &= m - 1;
+      const float a = __shfl_sync(0xffffffffu, alpha, j);
+      if (lane == j) { myT = T_cum; myW = T_cum * alpha; scanned = true; }
+      T_cum *= (1. - a);            // double intermediate (render_utils_kernel.cu:596)
+      if (T_cum < 1e-3) { done = true; break; }
+    }
+  }
+}
+
+// The k0 features of one sample at normalised coordinates (nx, ny, nz), lane = sample: every channel accumulated in ATen's corner
+// order (fma chain tnw .. bse) and the slabs combined in torch-CUDA's mean order (accumulator a = slab & 3, ((a0 + a1) + a2) + a3),
+// so the features are bit-identical to F.grid_sample(...).mean(0).  Records of C % 4 == 0 channels are read as float4.
+template <int kC, int kP>
+__device__ __forceinline__ void lane_features(const GridView& g, float nx, float ny, float nz, float (&out)[kC]) {
+  const int dY = g.Z * kC, dX = g.Y * g.Z * kC;
+  float tot[kC], grp[kC];
+#pragma unroll
+  for (int a = 0; a < 4 && a < kP; ++a) {
+#pragma unroll
+    for (int sl = a; sl < kP; sl += 4) {
+      const CellR cell = make_cell(src_index(fourier_gamma(sl, nx), g.X), src_index(fourier_gamma(sl, ny), g.Y),
+                                   src_index(fourier_gamma(sl, nz), g.Z), g.X, g.Y, g.Z);
+      const float* rec = g.data + sl * g.sp + (int64_t)cell.v * kC;
+      float val[kC];
+#pragma unroll
+      for (int c = 0; c < kC; ++c) val[c] = 0.f;
+#pragma unroll
+      for (int corner = 0; corner < 8; ++corner) {        // tnw, tne, tsw, tse, bnw, bne, bsw, bse (z fastest)
+        const int bx = corner >> 2, by = (corner >> 1) & 1, bz = corner & 1;
+        const float wgt = ((bz ? cell.fz : 1.f - cell.fz) * (by ? cell.fy : 1.f - cell.fy)) * (bx ? cell.fx : 1.f - cell.fx);
+        const float* q = rec + bx * dX + by * dY + bz * kC;
+        if constexpr (kC % 4 == 0) {
+#pragma unroll
+          for (int c4 = 0; c4 < kC; c4 += 4) {
+            const float4 v = __ldg(reinterpret_cast<const float4*>(q + c4));
+            val[c4] = fmaf(v.x, wgt, val[c4]); val[c4 + 1] = fmaf(v.y, wgt, val[c4 + 1]);
+            val[c4 + 2] = fmaf(v.z, wgt, val[c4 + 2]); val[c4 + 3] = fmaf(v.w, wgt, val[c4 + 3]);
+          }
+        } else {
+#pragma unroll
+          for (int c = 0; c < kC; ++c) val[c] = fmaf(__ldg(q + c), wgt, val[c]);
+        }
+      }
+#pragma unroll
+      for (int c = 0; c < kC; ++c) grp[c] = (sl == a) ? __fadd_rn(0.f, val[c]) : __fadd_rn(grp[c], val[c]);
+    }
+#pragma unroll
+    for (int c = 0; c < kC; ++c) tot[c] = (a == 0) ? grp[c] : __fadd_rn(tot[c], grp[c]);
+  }
+#pragma unroll
+  for (int c = 0; c < kC; ++c) out[c] = slab_mean_scale(tot[c], kP);
+}
+
 }  // namespace ubn

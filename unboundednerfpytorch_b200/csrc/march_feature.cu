@@ -608,7 +608,6 @@ __global__ void __launch_bounds__(32 * kMarchWarps, 4) k_march_feature_narrow(
   if (out_base == out_end) return;
   const Ray r = load_ray(rays_o + 3 * ray, rays_d + 3 * ray, p);
   const int S = p.S;
-  const int dY = g.Z * kC, dX = g.Y * g.Z * kC;
 
   for (int base = 0; base < S && out_base < out_end; base += 32) {
     const int s = base + lane;
@@ -643,35 +642,11 @@ __global__ void __launch_bounds__(32 * kMarchWarps, 4) k_march_feature_narrow(
       nz = __shfl_sync(0xffffffffu, nz, src);
     }
     if (lane < n_here) {
-      // slabs visited in torch's mean order: accumulator a = slab & 3; `tot` = ((a0 + a1) + a2) + a3
-      float tot[kC], grp[kC];
-#pragma unroll
-      for (int a = 0; a < 4 && a < kP; ++a) {
-#pragma unroll
-        for (int sl = a; sl < kP; sl += 4) {
-          CellR cell;
-          slab_cell<kP>(g, sl, nx, ny, nz, cell);
-          const float* rec = g.data + sl * g.sp + (int64_t)cell.v * kC;
-          float val[kC];
-#pragma unroll
-          for (int c = 0; c < kC; ++c) val[c] = 0.f;
-#pragma unroll
-          for (int corner = 0; corner < 8; ++corner) {        // tnw, tne, tsw, tse, bnw, bne, bsw, bse (z fastest)
-            const int bx = corner >> 2, by = (corner >> 1) & 1, bz = corner & 1;
-            const float wgt = ((bz ? cell.fz : 1.f - cell.fz) * (by ? cell.fy : 1.f - cell.fy)) * (bx ? cell.fx : 1.f - cell.fx);
-            const float* q = rec + bx * dX + by * dY + bz * kC;
-#pragma unroll
-            for (int c = 0; c < kC; ++c) val[c] = fmaf(__ldg(q + c), wgt, val[c]);
-          }
-#pragma unroll
-          for (int c = 0; c < kC; ++c) grp[c] = (sl == a) ? __fadd_rn(0.f, val[c]) : __fadd_rn(grp[c], val[c]);
-        }
-#pragma unroll
-        for (int c = 0; c < kC; ++c) tot[c] = (a == 0) ? grp[c] : __fadd_rn(tot[c], grp[c]);
-      }
+      float v[kC];
+      lane_features<kC, kP>(g, nx, ny, nz, v);
       float* o = feat + (out_base + lane) * kC;
 #pragma unroll
-      for (int c = 0; c < kC; ++c) o[c] = slab_mean_scale(tot[c], kP);
+      for (int c = 0; c < kC; ++c) o[c] = v[c];
     }
     out_base += n_here;
   }

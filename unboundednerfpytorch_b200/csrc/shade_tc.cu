@@ -20,83 +20,10 @@
 // compare-and-swap loops).
 #include <algorithm>
 
-#include "common.cuh"
+#include "rgbnet_tc.cuh"
 
 namespace ubn {
 namespace tc {
-
-// Hidden width kW is a template parameter of every kernel: 128 (every 12-channel config, the FourierGrid K = 3 / 15 configs)
-// or 64 (DirectMPIGO's llff_default, K = 9).  Everything below that sizes a layer derives from it.
-constexpr int kHidden = 128;            // the width of the kernels that keep their own names (k_shade_fwd_tc, k_shade_bwd_tc, ...)
-constexpr int kFeat = 12;               // feature columns of every shipped 12-channel config; kernels take kF in {3, 9, 12, 15}
-constexpr int kUnit = 16;               // samples per warp unit (the M of one mma)
-constexpr int kPanelRows = 128;         // row block of the panel save layout
-__host__ __device__ constexpr int n_tiles(int w) { return w / 8; }      // 8-column tiles of a w-wide layer
-__host__ __device__ constexpr int stride(int w) { return w + 8; }       // floats per row of a shared-memory operand tile
-                                                                        // (conflict-free both ways)
-
-// B-fragment tables (uint4 per lane): [n-tile][k-step][32 lanes]
-__host__ __device__ constexpr uint32_t frag_w2(int w) { return n_tiles(w) * n_tiles(w) * 32 * 16; }  // 128 KB at w = 128
-__host__ __device__ constexpr uint32_t frag_w1(int w) { return n_tiles(w) * 2 * 32 * 16; }  // layer 1: K <= 16 (2 k-steps)
-
-__device__ __forceinline__ uint32_t tf32_hi_bits(float x) { return __float_as_uint(x) & 0xFFFFE000u; }
-
-__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-__device__ __forceinline__ void split4(const float (&v)[4], uint32_t (&hi)[4], uint32_t (&lo)[4]) {
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    hi[i] = tf32_hi_bits(v[i]);
-    lo[i] = __float_as_uint(v[i] - __uint_as_float(hi[i]));
-  }
-}
-
-// d += a . b with (a, b) given as hi / lo halves; kThree adds the two cross terms
-template <bool kThree>
-__device__ __forceinline__ void mma3(float (&d)[4], const uint32_t (&ah)[4], const uint32_t (&al)[4], uint4 b) {
-  if (kThree) {
-    mma_tf32(d, al, b.x, b.y);
-    mma_tf32(d, ah, b.z, b.w);
-  }
-  mma_tf32(d, ah, b.x, b.y);
-}
-
-// Stage B[k][n] (k < K, n < N; zero outside) as B fragments for k-steps reading units 8 s + 2 t / 8 s + 2 t + 1:
-// lane (g, t) of (n-tile j, k-step s) gets {hi(B[8s+2t][8j+g]), hi(B[8s+2t+1][8j+g]), lo(..), lo(..)}.
-// B[k][n] = trans ? W[n * ld + k] : W[k * ld + n].
-__device__ void stage_frags(const float* __restrict__ W, int ld, bool trans, int K, int N, int n_ksteps, int n_ntiles,
-                            uint4* dst, int tid, int nthreads) {
-  for (int i = tid; i < n_ntiles * n_ksteps * 32; i += nthreads) {
-    const int lane = i & 31, s = (i >> 5) % n_ksteps, j = (i >> 5) / n_ksteps;
-    const int n = 8 * j + (lane >> 2), k0 = 8 * s + 2 * (lane & 3);
-    float w[2];
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      const int k = k0 + e;
-      w[e] = (k < K && n < N) ? (trans ? W[n * ld + k] : W[k * ld + n]) : 0.f;
-    }
-    const uint32_t h0 = tf32_hi_bits(w[0]), h1 = tf32_hi_bits(w[1]);
-    dst[i] = make_uint4(h0, h1, __float_as_uint(w[0] - __uint_as_float(h0)), __float_as_uint(w[1] - __uint_as_float(h1)));
-  }
-}
-
-// acc[NT] += X . B, X given in accumulator layout (x[s] = column tile s of the previous layer), B from stage_frags
-template <int KS, int NT, bool kThree>
-__device__ __forceinline__ void warp_gemm(float (&acc)[NT][4], const float (&x)[KS][4], const uint4* __restrict__ frag, int lane) {
-#pragma unroll
-  for (int s = 0; s < KS; ++s) {
-    const float av[4] = {x[s][0], x[s][2], x[s][1], x[s][3]};
-    uint32_t ah[4], al[4];
-    split4(av, ah, al);
-#pragma unroll
-    for (int j = 0; j < NT; ++j) mma3<kThree>(acc[j], ah, al, frag[(j * KS + s) * 32 + lane]);
-  }
-}
 
 // element offset of (row, col) in a save buffer: row-major [n][kW], or the panel layout [n/128][kW/4 quads][128 rows][4]
 template <bool kPanel, int kW>
@@ -187,16 +114,11 @@ __device__ __forceinline__ void shade_fwd_tc(UBN_SHADE_FWD_PARAMS) {
     for (int j = 0; j < kNT; ++j) h[j][0] = h[j][1] = h[j][2] = h[j][3] = 0.f;
     warp_gemm<kKS, kNT, kThree>(h, x, fW1, lane);
     // epilogue 1: + vb[ray], ReLU
-#pragma unroll
-    for (int j = 0; j < kNT; ++j)
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const float2 bias = __ldg(reinterpret_cast<const float2*>(vb + ray[r] * kW + 8 * j + 2 * t));
-        h[j][2 * r] = fmaxf(h[j][2 * r] + bias.x, 0.f);
-        h[j][2 * r + 1] = fmaxf(h[j][2 * r + 1] + bias.y, 0.f);
-        if (kSave && live[r])
-          *reinterpret_cast<float2*>(h1_out + save_idx<kPanel, kW>(row[r], 8 * j + 2 * t)) = make_float2(h[j][2 * r], h[j][2 * r + 1]);
-      }
+    epi_bias_relu<kNT>(
+        h, t, [&](int r, int c) { return __ldg(reinterpret_cast<const float2*>(vb + ray[r] * kW + c)); },
+        [&](int r, int c, float v0, float v1) {
+          if (kSave && live[r]) *reinterpret_cast<float2*>(h1_out + save_idx<kPanel, kW>(row[r], c)) = make_float2(v0, v1);
+        });
     if (kSave && kPanel && h1_mask) {
 #pragma unroll
       for (int c = 0; c < kW / 32; ++c)
@@ -213,34 +135,16 @@ __device__ __forceinline__ void shade_fwd_tc(UBN_SHADE_FWD_PARAMS) {
     warp_gemm<kNT, kNT, kThree>(z, h, fW2, lane);
     // epilogue 2: + b2, ReLU, layer 3 (N = 3: CUDA cores), sigmoid
     float p[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+    epi_hidden_layer3<kW, kNT>(z, 0, t, sB2, sW3, p, [&](int r, int c, float a0, float a1) {
+      if (kSave && live[r]) *reinterpret_cast<float2*>(h2_out + save_idx<kPanel, kW>(row[r], c)) = make_float2(a0, a1);
+    });
+    epi_rgb(p, b3v, t, [&](int r, const float (&v)[3]) {
+      if (live[r]) {
+        float* o = rgb + row[r] * 3;
 #pragma unroll
-    for (int j = 0; j < kNT; ++j) {
-      const int c = 8 * j + 2 * t;
-      const float2 bb = *reinterpret_cast<const float2*>(sB2 + c);
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const float a0 = fmaxf(z[j][2 * r] + bb.x, 0.f), a1 = fmaxf(z[j][2 * r + 1] + bb.y, 0.f);
-        if (kSave && live[r]) *reinterpret_cast<float2*>(h2_out + save_idx<kPanel, kW>(row[r], c)) = make_float2(a0, a1);
-#pragma unroll
-        for (int i = 0; i < 3; ++i) p[r][i] = fmaf(a1, sW3[i * kW + c + 1], fmaf(a0, sW3[i * kW + c], p[r][i]));
+        for (int i = 0; i < 3; ++i) o[i] = v[i];
       }
-    }
-#pragma unroll
-    for (int r = 0; r < 2; ++r)
-#pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        p[r][i] += __shfl_xor_sync(0xffffffffu, p[r][i], 1);
-        p[r][i] += __shfl_xor_sync(0xffffffffu, p[r][i], 2);
-      }
-    if (t == 0) {
-#pragma unroll
-      for (int r = 0; r < 2; ++r)
-        if (live[r]) {
-          float* o = rgb + row[r] * 3;
-#pragma unroll
-          for (int i = 0; i < 3; ++i) o[i] = 1.f / (1.f + expf(-(p[r][i] + b3v[i])));
-        }
-    }
+    });
   }
 }
 
@@ -281,41 +185,6 @@ __host__ __device__ constexpr int sum_rows(int f) { return f + 3 + 3; }
 __host__ __device__ constexpr uint32_t warp_bytes(int f, int w) { return tile_bytes(w) + (sum_rows(f) + 1) * stride(w) * 4; }
 __host__ __device__ constexpr uint32_t smem_bytes(int warps, int f, int w) { return oWarp(w) + warps * warp_bytes(f, w); }
 }  // namespace bk
-
-// lane (g, t) of (n-tile j, k-step s) gets the fp32 pair {B[8s+2t][8j+g], B[8s+2t+1][8j+g]}, B[k][n] = W[k * ld + n]
-__device__ void stage_frags_f32(const float* __restrict__ W, int ld, int K, int N, int n_ksteps, int n_ntiles, uint2* dst, int tid,
-                                int nthreads) {
-  for (int i = tid; i < n_ntiles * n_ksteps * 32; i += nthreads) {
-    const int lane = i & 31, s = (i >> 5) % n_ksteps, j = (i >> 5) / n_ksteps;
-    const int n = 8 * j + (lane >> 2), k = 8 * s + 2 * (lane & 3);
-    const float w0 = (k < K && n < N) ? W[k * ld + n] : 0.f, w1 = (k + 1 < K && n < N) ? W[(k + 1) * ld + n] : 0.f;
-    dst[i] = make_uint2(__float_as_uint(w0), __float_as_uint(w1));
-  }
-}
-
-// mma3 with the B fragment given as fp32: the same hi / lo split (and the same three products in the same order) as stage_frags
-template <bool kThree>
-__device__ __forceinline__ void mma3f(float (&d)[4], const uint32_t (&ah)[4], const uint32_t (&al)[4], uint2 b) {
-  const uint32_t h0 = b.x & 0xFFFFE000u, h1 = b.y & 0xFFFFE000u;
-  if (kThree) {
-    mma_tf32(d, al, h0, h1);
-    mma_tf32(d, ah, __float_as_uint(__uint_as_float(b.x) - __uint_as_float(h0)),
-             __float_as_uint(__uint_as_float(b.y) - __uint_as_float(h1)));
-  }
-  mma_tf32(d, ah, h0, h1);
-}
-
-template <int KS, int NT, bool kThree>
-__device__ __forceinline__ void warp_gemm_f(float (&acc)[NT][4], const float (&x)[KS][4], const uint2* __restrict__ frag, int lane) {
-#pragma unroll
-  for (int s = 0; s < KS; ++s) {
-    const float av[4] = {x[s][0], x[s][2], x[s][1], x[s][3]};
-    uint32_t ah[4], al[4];
-    split4(av, ah, al);
-#pragma unroll
-    for (int j = 0; j < NT; ++j) mma3f<kThree>(acc[j], ah, al, frag[(j * KS + s) * 32 + lane]);
-  }
-}
 
 // B fragment of the warp tile S[16][kStride] (sample = k): k-step s, column tile j -> S[8 s + t][8 j + g], S[8 s + t + 4][..]
 template <int kStride>

@@ -224,8 +224,8 @@ class _ContractedBase(_GridModel):
                     and kg[0].numel() < 2 ** 31)       # 32-bit offsets inside a slab
         return kg.is_cuda and kg.shape[1] in (4, 8, 12, 16) and kg.shape[0] <= 16
 
-    def _march(self, rays_o, rays_d, stepsize, coherent=False):
-        dev = rays_o.device
+    def _march_inputs(self, stepsize, dev):
+        """(t table, march cfg, mask cache or None, density desc, k0 desc) of the fused march and the fused render."""
         t_table = march.t_schedule(self._world_len(), stepsize, self.bg_len, self.T_BOUNDARY, dev)
         interval = stepsize * float(self._voxel_size_ratio())
         center, radius = self._host()
@@ -241,10 +241,81 @@ class _ContractedBase(_GridModel):
         kmn, kmx = self.k0._bounds()
         ddesc = G.grid_desc(self.density.grid, dmn, dmx, self.density.num_freqs)
         kdesc = G.grid_desc(self.k0.grid, kmn, kmx, self.k0.num_freqs)
+        return t_table, cfg, mask, ddesc, kdesc
+
+    def _march(self, rays_o, rays_d, stepsize, coherent=False):
+        t_table, cfg, mask, ddesc, kdesc = self._march_inputs(stepsize, rays_o.device)
         dense_known = (self.fast_color_thres <= 0) and not self.USE_CUMDIST and not self.USE_MASKCACHE
         out = march.March.apply(self.density.grid, self.k0.grid, rays_o, rays_d, t_table, mask, cfg, ddesc, kdesc,
                                 dense_known, coherent)
         return out, t_table
+
+    # ---- the fused render ---------------------------------------------------------------------------
+    RENDER_USES_BG = False      # DirectContractedVoxGO adds alphainv_last * bg outside training
+
+    def render_fused_ok(self, rays_o, render_kwargs):
+        """Whether render_fused covers this model and call (render.render_rays takes it exactly then): one-slab density and k0
+        grids (DirectContractedVoxGO; FourierGridModel at fourier_freq_num 0 -- with Fourier slabs the fused pass was slower than
+        the chunk loop on dense scenes, DESIGN.md §7), a channels-last k0 of 12 or 3 channels, the reference's unbounded rgbnets
+        ((rgbnet_dim, viewbase_pe) = (12, 4) or (3, 8), width 128, depth 3) or none (sigmoid(k0), 3 channels), no gradient, CUDA
+        rays, and a background the fused composite reproduces: none for FourierGridModel (rand_bkgd draws a random one), a number
+        for DirectContractedVoxGO."""
+        kg, dg = self.k0.grid, self.density.grid
+        if torch.is_grad_enabled() or not (rays_o.is_cuda and kg.is_cuda and dg.is_cuda and self._fused_ok()):
+            return False
+        C = kg.shape[1]
+        if not (kg.shape[0] == 1 and C in (3, 12) and kg.stride(1) == 1 and kg.dtype == torch.float32
+                and tuple(dg.shape[:2]) == (1, 1) and dg.is_contiguous() and dg.dtype == torch.float32):
+            return False
+        if self.RENDER_USES_BG:
+            if not isinstance(render_kwargs.get('bg', 0), (int, float)):
+                return False
+        elif render_kwargs.get('rand_bkgd', False):
+            return False
+        net = self.rgbnet
+        if net is None:
+            return C == 3
+        try:
+            l1, l2, l3 = net[0], net[2][0], net[3]
+        except Exception:
+            return False
+        pe = self.viewfreq.numel()
+        return (len(net) == 4 and (C, pe) in ((12, 4), (3, 8)) and tuple(l1.weight.shape) == (128, C + 3 + 6 * pe)
+                and tuple(l2.weight.shape) == (128, 128) and tuple(l3.weight.shape) == (3, 128)
+                and all(t.is_cuda and t.dtype == torch.float32 for t in (l1.weight, l2.weight, l3.weight)))
+
+    @torch.no_grad()
+    def render_fused(self, rays_o, rays_d, viewdirs, n_shaded=None, n_marched=None, **render_kwargs):
+        """{'rgb_marched' [N,3], 'depth' [N], 'alphainv_last' [N]} of N rays in one launch (csrc/render.cu): the march, the k0
+        read of the kept samples, the rgbnet and the composite with no per-sample buffers, so a whole frame is one call.  Same
+        kept samples and alphainv_last (bit for bit) as forward; rgb_marched and depth as forward's composite, summed in step order.
+        n_shaded / n_marched: optional int32 [N] that receive each ray's kept samples / the samples of the 32-sample chunks
+        marched before the ray stopped.  Only where render_fused_ok holds."""
+        from . import _cabi
+        from ._cabi import c_f, c_i64, c_int, check, ptr, stream_of
+        N = rays_o.shape[0]
+        dev = rays_o.device
+        rays_o = rays_o.contiguous().float()
+        rays_d = rays_d.contiguous().float()
+        viewdirs = viewdirs.contiguous().float()
+        rgb = torch.empty(N, 3, dtype=torch.float32, device=dev)
+        depth = torch.empty(N, dtype=torch.float32, device=dev)
+        last = torch.empty(N, dtype=torch.float32, device=dev)
+        t_table, cfg, mask, ddesc, kdesc = self._march_inputs(render_kwargs['stepsize'], dev)
+        if self.rgbnet is not None:
+            l1, l2, l3 = self.rgbnet[0], self.rgbnet[2][0], self.rgbnet[3]
+            net = tuple(t.detach().contiguous() for t in (l1.weight, l1.bias, l2.weight, l2.bias, l3.weight, l3.bias))
+            pe = self.viewfreq.numel()
+        else:
+            net, pe = (None,) * 6, 0
+        use_bg = 1 if self.RENDER_USES_BG else 0
+        bg = float(render_kwargs.get('bg', 0)) if use_bg else 0.0
+        with _cabi.timed('render_contracted'):
+            check(_cabi.load().ubn_render_contracted(
+                ptr(rays_o), ptr(rays_d), ptr(viewdirs), ptr(t_table), ptr(self.density.grid), ddesc, ptr(self.k0.grid), kdesc,
+                ptr(mask), cfg, c_i64(N), *map(ptr, net), c_int(128), c_int(pe), c_int(use_bg), c_f(bg), ptr(rgb), ptr(depth),
+                ptr(last), ptr(n_shaded), ptr(n_marched), stream_of(rgb)))
+        return {'rgb_marched': rgb, 'depth': depth, 'alphainv_last': last}
 
     def _tv_weights(self, grid, weight, dense_mode):
         w = weight * float(max(grid.grid.shape[2:])) / 128         # each grid's own largest dimension
@@ -551,6 +622,7 @@ class DirectContractedVoxGO(_ContractedBase):
     T_BOUNDARY = 2.0
     USE_CUMDIST = True
     USE_MASKCACHE = True
+    RENDER_USES_BG = True
 
     def __init__(self, xyz_min, xyz_max, num_voxels=0, num_voxels_base=0, alpha_init=None, mask_cache_world_size=None,
                  fast_color_thres=0, bg_len=0.2, contracted_norm='inf', density_type='DenseGrid', k0_type='DenseGrid',

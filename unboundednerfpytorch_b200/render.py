@@ -5,7 +5,8 @@ SURVEY.md 8e:
                                    device (one launch), 8192-ray chunks through ``model(...)`` (run_render.py:56-63), numpy
                                    (rgbs, depths, bgmaps).  With torch.distributed initialised every rank renders a contiguous
                                    shard of each frame's rays and the frame is assembled with one all-gather (BASELINE config 4).
-* ``render_rays``               -- the chunk loop on flat ray arrays.
+* ``render_rays``               -- flat ray arrays: one fused launch for the contracted models models.render_fused
+                                   covers, otherwise the chunk loop.
 * ``render_frame_sharded``      -- one frame: contiguous ray shard per rank + ``dist.gather_frame``.
 * ``render_blocks_idw``         -- Block-NeRF style (eval_block_nerf.py:95-133, :215-216): one spatial block per rank, every rank
                                    renders the same frame, blocks that do not see the view are gated out, the frame is the
@@ -32,6 +33,11 @@ def render_rays(model, rays_o, rays_d, viewdirs, render_kwargs, chunk=8192, keys
     # kernel (csrc/render_tma.cu).  Opt-in: the lane-per-sample gather stays the default (the TMA kernel was slower on a full
     # garden frame when it was last compared; not re-measured on the H100).
     rk.setdefault('coherent_rays', False)
+    # contracted models the fused render covers (models._ContractedBase.render_fused_ok) take the whole ray array in one launch
+    # (memory O(n), no per-sample buffers); every other model or configuration keeps the chunk loop
+    if hasattr(model, 'render_fused_ok') and model.render_fused_ok(rays_o, rk):
+        ret = model.render_fused(rays_o, rays_d, viewdirs, **rk)
+        return {k: ret[k].reshape(rays_o.shape[0], -1) for k in keys}
     outs = {k: [] for k in keys}
     for ro, rd, vd in zip(rays_o.split(chunk, 0), rays_d.split(chunk, 0), viewdirs.split(chunk, 0)):
         ret = model(ro, rd, vd, **rk)
