@@ -582,6 +582,13 @@ int ubn_rgbnet_bwd_tc_fused_kw(int n_feat, int n_hidden, const float* feat, cons
  * same per-chunk fp32 running sums, so the same results up to the tensor cores' accumulation order.  Process-wide like
  * ubn_set_feature_kernel.  Returns cudaErrorInvalidValue for other values. */
 int ubn_set_dw2_engine(int engine);
+/* Which kernel runs the width-128, 12-feature rgbnet forward (ubn_rgbnet_fwd_tc / _k / _kw without bit 1 of single_pass, with or
+ * without saves): 1 (the default) = warpgroup MMA (wgmma) on 64-sample tiles with a producer warpgroup staging the feature rows;
+ * 0 = the mma.sync kernel.  Same saves, mask words and products, so the same results up to the tensor cores' accumulation order.
+ * Process-wide like ubn_set_dw2_engine.  Returns cudaErrorInvalidValue for other values. */
+int ubn_set_fwd_engine(int engine);
+/* The forward engine ubn_set_fwd_engine last set (1 unless changed). */
+int ubn_get_fwd_engine(void);
 
 /* ---- TensoRFGrid: the vector-matrix (VM) factorised grid (FourierGrid/grid.py:90-201) ------------------------------------------
  * Six factors, in this order everywhere: 0 xy_plane [1,Rxy,X,Y], 1 xz_plane [1,R,X,Z], 2 yz_plane [1,R,Y,Z], 3 x_vec [1,R,X,1],

@@ -20,10 +20,11 @@ Prints one JSON line:
                     dropped for this check, as in tests/test_gpu_models.py);
 * dw2            -- with --dw2 mma,wgmma (width 128): the dW2 engines timed alternately in this one run, --rounds times each
                     (a torch.profiler pass per round), with the rates of the fastest round and max_err for each engine;
+* fwd            -- with --fwd mma,wgmma (width 128): the same for the forward engines (k_shade_fwd_tc, k_shade_fwd_wgmma);
 * gpu / power_limit_w -- where it ran, read in the same run.
 
     python scripts/bench_rgbnet.py [--shape truck|llff] [--iters 20] [--warmup 3] [--profile DIR] [--no-check]
-                                   [--dw2 mma,wgmma] [--rounds 3]
+                                   [--dw2 mma,wgmma] [--fwd mma,wgmma] [--rounds 3]
 """
 import argparse
 import json
@@ -45,6 +46,7 @@ HMMA_PER_SAMPLE = {'k_shade_fwd_tc': 864 / 16,      # layer 1 (2 k-steps) + laye
                    'k_shade_bwd_tc': 1120 / 16,     # dH1 768 + dX 96 + dW1k/view bias 96 + dW3 96 + E 64, per 16-sample unit
                    'k_shade_dw2_tc': 1536 / 32,     # 8 warps x 4 k-steps x 16 column tiles x 3 passes per 32-sample chunk
                    'k_shade_dw2_wgmma': 1536 / 32,  # the same products as 2 warpgroups x 4 k-steps x 3 wgmma.m64n128k8
+                   'k_shade_fwd_wgmma': 864 / 16,   # the same products as 18 k-steps x 3 wgmma.m64n128k8 per 64-sample tile
                    # width 64, 9 features
                    'k_shade_fwd_tc_w': 240 / 16,    # layer 1 (2 k-steps) + layer 2 (8 k-steps), 8 column tiles, 3 passes
                    'k_shade_bwd_tc_w': 368 / 16,    # dH1 192 + dX 48 + dW1k/view bias 48 + dW3 48 + E 32, per 16-sample unit
@@ -54,12 +56,15 @@ BYTES_PER_SAMPLE = {'k_shade_fwd_tc': 48 + 8 + 12 + 512 + 512 + 16,          # f
                     'k_shade_bwd_tc': 512 + 48 + 12 + 12 + 8 + 16 + 48 + 16,  # H2, feat, rgb, grad_rgb, ray_id, H1 masks; grad_feat, H2 masks
                     'k_shade_dw2_tc': 512 + 16 + 12 + 12,                     # H1, H2 masks, rgb, grad_rgb
                     'k_shade_dw2_wgmma': 512 + 16 + 12 + 12,
+                    'k_shade_fwd_wgmma': 48 + 8 + 12 + 512 + 512 + 16,
                     'k_shade_fwd_tc_w': 36 + 8 + 12 + 256 + 256 + 8,          # the same at width 64 with 9 features
                     'k_shade_bwd_tc_w': 256 + 36 + 12 + 12 + 8 + 8 + 36 + 8,
                     'k_shade_dw2_tc_w': 256 + 8 + 12 + 12}
 # shape -> feature columns, hidden width, view-embedding columns, kernel-name suffix, default samples and rays
 # --dw2 engine name -> ubn_set_dw2_engine value and the kernel it runs at width 128
 DW2_ENGINES = {'mma': (0, 'k_shade_dw2_tc'), 'wgmma': (1, 'k_shade_dw2_wgmma')}
+# --fwd engine name -> ubn_set_fwd_engine value and the forward kernel it runs at width 128
+FWD_ENGINES = {'mma': (0, 'k_shade_fwd_tc'), 'wgmma': (1, 'k_shade_fwd_wgmma')}
 SHAPES = {'truck': dict(K=12, W=128, E=27, sfx='', samples=4_194_304, rays=8192),
           'llff': dict(K=9, W=64, E=3, sfx='_w', samples=LLFF_SURVIVORS, rays=None)}
 
@@ -162,7 +167,8 @@ def main():
     ap.add_argument('--profile', default=None, help='also run a torch.profiler pass and write its trace under this directory')
     ap.add_argument('--no-check', action='store_true')
     ap.add_argument('--dw2', default=None, help='comma list of dW2 engines (mma, wgmma) to time alternately, width 128 only')
-    ap.add_argument('--rounds', type=int, default=3, help='rounds of the --dw2 alternation')
+    ap.add_argument('--fwd', default=None, help='comma list of forward engines (mma, wgmma) to time alternately, width 128 only')
+    ap.add_argument('--rounds', type=int, default=3, help='rounds of the --dw2 / --fwd alternation')
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit('bench_rgbnet.py needs a GPU')
@@ -174,10 +180,15 @@ def main():
     net, k0, emb, ray_id, gr = _inputs(M, args.rays or sh['rays'], sh['K'], sh['W'], sh['E'])
     assert shade.supported(net, sh['K'])
     k0.requires_grad_(True)
+    from unboundednerfpytorch_b200 import ops
     fwd_k, bwd_k = (f'k_shade_{n}_tc{sh["sfx"]}' for n in ('fwd', 'bwd'))
+    if sh['W'] == 128 and shade.MODE in ('tc3', 'tc1') and ops.get_fwd_engine() == FWD_ENGINES['wgmma'][0]:
+        fwd_k = FWD_ENGINES['wgmma'][1]     # the 8-warp forward's engine; tc3w4 runs the 4-warp k_shade_fwd_tc
     dw2_k = DW2_ENGINES['wgmma'][1] if sh['W'] == 128 else 'k_shade_dw2_tc_w'
     engines = args.dw2.split(',') if args.dw2 else []
     assert all(e in DW2_ENGINES for e in engines) and (not engines or sh['W'] == 128), '--dw2 takes mma / wgmma at width 128'
+    fwd_engines = args.fwd.split(',') if args.fwd else []
+    assert all(e in FWD_ENGINES for e in fwd_engines) and (not fwd_engines or sh['W'] == 128), '--fwd takes mma / wgmma at width 128'
     res = dict(metric=f'rgbnet forward + backward, {args.shape} shape', gpu=name, power_limit_w=power, samples=M,
                rays=emb.shape[0], features=sh['K'], width=sh['W'], mode=shade.MODE, bwd_mode=shade.BWD_MODE)
     for _ in range(args.warmup):
@@ -201,28 +212,30 @@ def main():
         res['kernels_ms'] = {k: round(v, 3) for k, v in kms.items()}
         for k, v in kms.items():
             res['rates'][k] = _rates(k, v, M)
-    if engines:
-        from unboundednerfpytorch_b200 import ops
-        runs = {e: [] for e in engines}
+    for key, names, table, setter in (('dw2', engines, DW2_ENGINES, ops.set_dw2_engine),
+                                      ('fwd', fwd_engines, FWD_ENGINES, ops.set_fwd_engine)):
+        if not names:
+            continue
+        runs = {e: [] for e in names}
         try:
             for _ in range(args.rounds):
-                for e in engines:
-                    value, kname = DW2_ENGINES[e]
-                    ops.set_dw2_engine(value)
+                for e in names:
+                    value, kname = table[e]
+                    setter(value)
                     for _ in range(args.warmup):
                         _step(shade, net, k0, emb, ray_id, gr)
                     torch.cuda.synchronize()
                     runs[e].append(_kernel_ms(shade, (net, k0, emb, ray_id, gr), args.iters, (kname,))[kname])
-            res['dw2'] = {}
-            for e in engines:
-                value, kname = DW2_ENGINES[e]
-                res['dw2'][e] = dict(kernel=kname, ms_rounds=[round(v, 3) for v in runs[e]], **_rates(kname, min(runs[e]), M))
+            res[key] = {}
+            for e in names:
+                value, kname = table[e]
+                res[key][e] = dict(kernel=kname, ms_rounds=[round(v, 3) for v in runs[e]], **_rates(kname, min(runs[e]), M))
                 if not args.no_check:
-                    ops.set_dw2_engine(value)
+                    setter(value)
                     err, _ = _check(shade, net, k0.detach(), emb, ray_id, gr)
-                    res['dw2'][e]['max_err_of_scale'] = {k: float(f'{v:.3g}') for k, v in err.items()}
+                    res[key][e]['max_err_of_scale'] = {k: float(f'{v:.3g}') for k, v in err.items()}
         finally:
-            ops.set_dw2_engine(1)
+            setter(1)
     if not args.no_check:
         err, n = _check(shade, net, k0.detach(), emb, ray_id, gr)
         res['max_err_of_scale'] = {k: float(f'{v:.3g}') for k, v in err.items()}

@@ -159,7 +159,6 @@ __global__ void __launch_bounds__(32 * kWarps, kCtas) k_shade_fwd_tc_w(UBN_SHADE
   shade_fwd_tc<kF, kW, kSave, kThree, kWarps, kPanel>(UBN_SHADE_FWD_ARGS);
 }
 #undef UBN_SHADE_FWD_ARGS
-#undef UBN_SHADE_FWD_PARAMS
 
 // ---- backward, launch 1 --------------------------------------------------------------------------------------------------
 //   dz3 = g_rgb * rgb (1 - rgb);  dZ2 = (dz3 . W3) * [H2 > 0];  dH1 = dZ2 . W2;  dZ1 = dH1 * [H1 > 0]
@@ -992,6 +991,202 @@ __global__ void __launch_bounds__(wg::kThreads, 1) k_shade_dw2_wgmma(const float
 #undef UBN_SHADE_DW2_ARGS
 #undef UBN_SHADE_DW2_PARAMS
 
+// ---- forward on warpgroup MMA (width 128, 12 features) --------------------------------------------------------------------
+// The contract of shade_fwd_tc<12, 128, kSave, kThree, 8, kPanel> on wgmma.m64n128k8 (TF32), 64-sample tiles: W1k and W2 are read
+// by the tensor cores from shared memory by descriptor, so no warp reloads B fragments per tile.  One persistent CTA per SM:
+//   * warpgroup 0 (producer) copies each tile's feature rows and ray ids into a ring of kStages stages with cp.async (zeros past
+//     n_pts); the ring's full barrier completes when the copies land (cp.async.mbarrier.arrive), so no producer thread waits on
+//     them;
+//   * warpgroups 1 and 2 (consumers) take alternate tiles, so one warpgroup's epilogue stores overlap the other's MMAs.  Warp w
+//     of a consumer owns rows 16 w + g and 16 w + g + 8 of the tile and, like an mma.sync warp, columns 8 j + 2 t, + 1: the
+//     wgmma accumulator of layer 1 is the per-warp m16n8k8 A layout of layer 2 under the k-permutation of shade_fwd_tc
+//     (a0..a3 = d[4 s], d[4 s + 2], d[4 s + 1], d[4 s + 3]).  The K-major W2 tile of k-step s therefore holds hidden units
+//     8 s + {0, 2, 4, 6, 1, 3, 5, 7} in k order.
+// Both weight matrices are staged once per CTA, split into hi / lo, in the 128-byte-swizzle layout of sw128_off (four
+// [128][32] tiles per W2 half, one per W1k half with features 12..31 zero).  3xTF32 issues the mma3 products al.Bh, ah.Bl,
+// ah.Bh per k-step; single pass ah.Bh.  The epilogues are shade_fwd_tc's (epi_bias_relu, mask_chunk, epi_hidden_layer3, epi_rgb),
+// so the saves keep their layout and mask words and rgb differs from the mma.sync kernel only by accumulation order.  All three
+// forms (panel saves, row-major saves, no saves) run the same arithmetic, so a no_grad forward gives the training forward's bits.
+namespace fg {
+constexpr int kThreads = 384;
+constexpr int kRows = 64;                                       // samples per tile (the M of one wgmma)
+constexpr int kStages = 4;
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;          // 128 * 40 + 256 * 232 <= 384 * 168 (launch allotment)
+constexpr uint32_t kTile = kHidden * 32 * 4;                    // one [128][32] fp32 tile: 16 KB
+constexpr uint32_t kFeatBytes = kRows * kFeat * 4;              // [64][12] fp32 feature rows
+constexpr uint32_t kStage = kFeatBytes + kRows * 8;             // + [64] ray ids
+constexpr int kChunks = kFeatBytes / 8;                         // 8-byte copies per tile (rows are 8-byte aligned)
+__host__ __device__ constexpr uint32_t oW2(int half) { return half * 4 * kTile; }                 // hi, lo
+__host__ __device__ constexpr uint32_t oW1(bool three, int half) { return (three ? 8 : 4) * kTile + half * kTile; }
+__host__ __device__ constexpr uint32_t oRing(bool three) { return oW1(three, three ? 2 : 1); }
+__host__ __device__ constexpr uint32_t oW3(bool three) { return oRing(three) + kStages * kStage; }
+__host__ __device__ constexpr uint32_t oB2(bool three) { return oW3(three) + 3 * kHidden * 4; }
+__host__ __device__ constexpr uint32_t oBar(bool three) { return oB2(three) + kHidden * 4; }
+// + full and empty barriers, + slack to align the base to 1 KB
+__host__ __device__ constexpr uint32_t smem(bool three) { return oBar(three) + 2 * kStages * 8 + 1024; }
+}  // namespace fg
+
+__device__ __forceinline__ void cp_async8(uint32_t dst, const void* src, bool ok) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;" ::"r"(dst), "l"(src), "r"(ok ? 8 : 0) : "memory");
+}
+
+template <bool kThree, bool kSave, bool kPanel>
+__global__ void __launch_bounds__(fg::kThreads, 1) k_shade_fwd_wgmma(UBN_SHADE_FWD_PARAMS) {
+  constexpr int kW = kHidden, kF = kFeat, kNT = n_tiles(kHidden);
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  const int tid = threadIdx.x;
+  for (int i = tid; i < kW * kW; i += fg::kThreads) {         // W2[n][unit]: k-step s, k p <- unit 8 s + (p < 4 ? 2 p : 2 p - 7)
+    const int n = i >> 7, kk = i & 127, p = kk & 7;
+    const float w = W2[n * kW + (kk & ~7) + (p < 4 ? 2 * p : 2 * p - 7)];
+    const uint32_t hi = tf32_hi_bits(w), off = (kk >> 5) * fg::kTile + sw128_off(n, kk & 31);
+    *reinterpret_cast<uint32_t*>(smem + fg::oW2(0) + off) = hi;
+    if (kThree) *reinterpret_cast<uint32_t*>(smem + fg::oW2(1) + off) = __float_as_uint(w - __uint_as_float(hi));
+  }
+  for (int i = tid; i < kW * 32; i += fg::kThreads) {          // W1k[n][feature], features >= kF zero
+    const int n = i >> 5, k = i & 31;
+    const float w = k < kF ? W1k[n * kF + k] : 0.f;
+    const uint32_t hi = tf32_hi_bits(w), off = sw128_off(n, k);
+    *reinterpret_cast<uint32_t*>(smem + fg::oW1(kThree, 0) + off) = hi;
+    if (kThree) *reinterpret_cast<uint32_t*>(smem + fg::oW1(kThree, 1) + off) = __float_as_uint(w - __uint_as_float(hi));
+  }
+  float* sW3 = reinterpret_cast<float*>(smem + fg::oW3(kThree));
+  float* sB2 = reinterpret_cast<float*>(smem + fg::oB2(kThree));
+  for (int i = tid; i < 3 * kW; i += fg::kThreads) sW3[i] = W3[i];
+  for (int i = tid; i < kW; i += fg::kThreads) sB2[i] = b2[i];
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // the weight tiles, before wgmma reads them
+  const uint32_t full0 = smem_u32(smem + fg::oBar(kThree)), empty0 = full0 + 8 * fg::kStages;
+  if (tid == 0) {
+    for (int s = 0; s < fg::kStages; ++s) {
+      mbar_init(full0 + 8 * s, 128);
+      mbar_init(empty0 + 8 * s, 128);
+    }
+  }
+  __syncthreads();
+  const int64_t n_tiles = (n_pts + fg::kRows - 1) / fg::kRows, step = gridDim.x;
+  uint8_t* ring = smem + fg::oRing(kThree);
+
+  if (tid < 128) {                                          // producer
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(fg::kProducerRegs));
+    int i = 0;
+    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += step, ++i) {
+      const int s = i % fg::kStages;
+      mbar_wait(empty0 + 8 * s, ((i / fg::kStages) & 1) ^ 1);
+      const int64_t r0 = tile * fg::kRows;
+      const uint32_t dst = smem_u32(ring + s * fg::kStage);
+      for (int q = tid; q < fg::kChunks; q += 128) {
+        const bool ok = r0 + q / (kF / 2) < n_pts;
+        cp_async8(dst + 8 * q, ok ? feat + r0 * kF + 2 * q : feat, ok);
+      }
+      if (tid < fg::kRows) cp_async8(dst + fg::kFeatBytes + 8 * tid, r0 + tid < n_pts ? ray_id + r0 + tid : ray_id, r0 + tid < n_pts);
+      asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(full0 + 8 * s) : "memory");
+    }
+    asm volatile("cp.async.wait_all;" ::: "memory");
+    return;
+  }
+
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(fg::kConsumerRegs));
+  const int c = (tid >> 7) - 1, lane = tid & 31, g = lane >> 2, t = lane & 3;
+  const int rl = 16 * ((tid >> 5) & 3) + g;                  // this thread's rows rl and rl + 8 of the tile
+  const float b3v[3] = {b3[0], b3[1], b3[2]};
+  const uint32_t w2 = smem_u32(smem + fg::oW2(0)), w1 = smem_u32(smem + fg::oW1(kThree, 0));
+  int i = c;
+  for (int64_t tile = blockIdx.x + c * step; tile < n_tiles; tile += 2 * step, i += 2) {
+    const int s = i % fg::kStages;
+    mbar_wait(full0 + 8 * s, (i / fg::kStages) & 1);
+    const float* sf = reinterpret_cast<const float*>(ring + s * fg::kStage);
+    const int64_t* sr = reinterpret_cast<const int64_t*>(ring + s * fg::kStage + fg::kFeatBytes);
+    // layer-1 A: k-step 0 = features 0..7, k-step 1 = features 8..11 (k = t) and zeros (k = t + 4)
+    const float x[2][4] = {{sf[rl * kF + t], sf[(rl + 8) * kF + t], sf[rl * kF + t + 4], sf[(rl + 8) * kF + t + 4]},
+                           {sf[rl * kF + 8 + t], sf[(rl + 8) * kF + 8 + t], 0.f, 0.f}};
+    const int64_t ray[2] = {sr[rl], sr[rl + 8]};
+    mbar_arrive(empty0 + 8 * s);
+    const int64_t row[2] = {tile * fg::kRows + rl, tile * fg::kRows + rl + 8};
+    const bool live[2] = {row[0] < n_pts, row[1] < n_pts};
+
+    // layer 1
+    float h[kNT][4];
+    float(&hv)[64] = reinterpret_cast<float(&)[64]>(h);
+    {
+      uint32_t xh[2][4], xl[2][4];
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) split4(x[ks], xh[ks], xl[ks]);
+#pragma unroll
+      for (int e = 0; e < 64; ++e) hv[e] = 0.f;
+      asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) {
+        const uint64_t bh = sw128_desc(w1 + 32 * ks);
+        if (kThree) {
+          wgmma_tf32<1>(hv, xl[ks], bh);
+          wgmma_tf32<1>(hv, xh[ks], sw128_desc(w1 + fg::kTile + 32 * ks));
+        }
+        wgmma_tf32<1>(hv, xh[ks], bh);
+      }
+      asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+      asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+#pragma unroll
+      for (int e = 0; e < 64; ++e) asm volatile("" : "+f"(hv[e])::"memory");
+    }
+    // epilogue 1: + vb[ray], ReLU, H1 save and mask words
+    epi_bias_relu<kNT>(
+        h, t, [&](int r, int cc) { return __ldg(reinterpret_cast<const float2*>(vb + ray[r] * kW + cc)); },
+        [&](int r, int cc, float v0, float v1) {
+          if (kSave && live[r]) *reinterpret_cast<float2*>(h1_out + save_idx<kPanel, kW>(row[r], cc)) = make_float2(v0, v1);
+        });
+    if (kSave && kPanel && h1_mask) {
+#pragma unroll
+      for (int cc = 0; cc < kW / 32; ++cc)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const uint32_t w = mask_chunk(h, cc, 2 * r, t);
+          if (t == 0 && live[r]) h1_mask[mask_idx<kW>(row[r], cc)] = w;
+        }
+    }
+    // layer 2: A = H1 straight from the accumulator
+    float z[kNT][4];
+    float(&zv)[64] = reinterpret_cast<float(&)[64]>(z);
+    {
+      uint32_t ah[kNT][4], al[kNT][4];
+#pragma unroll
+      for (int ks = 0; ks < kNT; ++ks) {
+        const float av[4] = {h[ks][0], h[ks][2], h[ks][1], h[ks][3]};
+        split4(av, ah[ks], al[ks]);
+      }
+#pragma unroll
+      for (int e = 0; e < 64; ++e) zv[e] = 0.f;
+      asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+      for (int ks = 0; ks < kNT; ++ks) {
+        const uint32_t off = (ks >> 2) * fg::kTile + 32 * (ks & 3);
+        const uint64_t bh = sw128_desc(w2 + off);
+        if (kThree) {
+          wgmma_tf32<1>(zv, al[ks], bh);
+          wgmma_tf32<1>(zv, ah[ks], sw128_desc(w2 + fg::oW2(1) + off));
+        }
+        wgmma_tf32<1>(zv, ah[ks], bh);
+      }
+      asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+      asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+#pragma unroll
+      for (int e = 0; e < 64; ++e) asm volatile("" : "+f"(zv[e])::"memory");
+    }
+    // epilogue 2: + b2, ReLU, H2 save, layer 3 (CUDA cores), sigmoid
+    float p[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+    epi_hidden_layer3<kW, kNT>(z, 0, t, sB2, sW3, p, [&](int r, int cc, float a0, float a1) {
+      if (kSave && live[r]) *reinterpret_cast<float2*>(h2_out + save_idx<kPanel, kW>(row[r], cc)) = make_float2(a0, a1);
+    });
+    epi_rgb(p, b3v, t, [&](int r, const float (&v)[3]) {
+      if (live[r]) {
+        float* o = rgb + row[r] * 3;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) o[k] = v[k];
+      }
+    });
+  }
+}
+#undef UBN_SHADE_FWD_PARAMS
+
 // Width 64 (DirectMPIGO, K = 9): warps per CTA and resident CTAs per SM of each launch, from the -Xptxas -v figures of DESIGN §4
 namespace w64 {
 constexpr int kFwdWarps = 8, kFwdCtas = 2;
@@ -1093,6 +1288,22 @@ int launch_dw2_wgmma(const float* W3, const float* rgb, const float* h1, const u
   return 0;
 }
 
+// which kernel runs the width-128, 12-feature forward (8-warp form): 1 = k_shade_fwd_wgmma (default), 0 = k_shade_fwd_tc
+int g_fwd_engine = 1;
+
+template <bool kThree, bool kSave, bool kPanel>
+int launch_fwd_wgmma(const float* feat, const float* vb, const int64_t* ray_id, const float* W1k, const float* W2, const float* b2,
+                     const float* W3, const float* b3, int64_t n, float* rgb, float* h1, float* h2, uint32_t* m1, cudaStream_t st) {
+  auto k = tc::k_shade_fwd_wgmma<kThree, kSave, kPanel>;
+  constexpr uint32_t bytes = tc::fg::smem(kThree);
+  if (int e = set_smem(k, bytes)) return e;
+  const int64_t n_tiles = (n + tc::fg::kRows - 1) / tc::fg::kRows;
+  k<<<(unsigned)std::min<int64_t>(kNumSMs, n_tiles), tc::fg::kThreads, bytes, st>>>(feat, vb, ray_id, W1k, W2, b2, W3, b3, n, rgb,
+                                                                                      h1, h2, m1);
+  UBN_LAUNCH_CHECK();
+  return 0;
+}
+
 template <int kF>
 int rgbnet_fwd_tc(const float* feat, const float* view_bias, const int64_t* ray_id, const float* W1k, const float* W2, const float* b2,
                   const float* W3, const float* b3, int64_t n_pts, float* rgb, float* h1_save, float* h2_save, uint32_t* h1_mask,
@@ -1103,6 +1314,16 @@ int rgbnet_fwd_tc(const float* feat, const float* view_bias, const int64_t* ray_
   cudaStream_t st = as_stream(stream);
 #define UBN_FWD(SAVE, THREE, W) \
   return launch_fwd_p<kF, SAVE, THREE, W>(panel, feat, view_bias, ray_id, W1k, W2, b2, W3, b3, n_pts, rgb, h1_save, h2_save, h1_mask, st)
+  if constexpr (kF == tc::kFeat) {
+    if (!four && g_fwd_engine == 1) {
+#define UBN_FWD_WG(THREE, SAVE, P) \
+  return launch_fwd_wgmma<THREE, SAVE, P>(feat, view_bias, ray_id, W1k, W2, b2, W3, b3, n_pts, rgb, h1_save, h2_save, h1_mask, st)
+      if (save && panel) { if (one) UBN_FWD_WG(false, true, true); else UBN_FWD_WG(true, true, true); }
+      if (save) { if (one) UBN_FWD_WG(false, true, false); else UBN_FWD_WG(true, true, false); }
+      if (one) UBN_FWD_WG(false, false, false); else UBN_FWD_WG(true, false, false);
+#undef UBN_FWD_WG
+    }
+  }
   if (save) {
     if (one) { if (four) UBN_FWD(true, false, 4); else UBN_FWD(true, false, 8); }
     if (four) UBN_FWD(true, true, 4); else UBN_FWD(true, true, 8);
@@ -1194,6 +1415,14 @@ extern "C" int ubn_set_dw2_engine(int engine) {
   g_dw2_engine = engine;
   return 0;
 }
+
+extern "C" int ubn_set_fwd_engine(int engine) {
+  if (engine < 0 || engine > 1) return finish(cudaErrorInvalidValue);
+  g_fwd_engine = engine;
+  return 0;
+}
+
+extern "C" int ubn_get_fwd_engine(void) { return g_fwd_engine; }
 
 extern "C" int ubn_rgbnet_fwd_tc(const float* feat, const float* view_bias, const int64_t* ray_id, const float* W1k,
                                  const float* W2, const float* b2, const float* W3, const float* b3, int64_t n_pts,

@@ -492,6 +492,18 @@ def set_dw2_engine(engine):
     check(load().ubn_set_dw2_engine(c_int(int(engine))))
 
 
+def set_fwd_engine(engine):
+    """The width-128, 12-feature rgbnet forward (8-warp form): 1 = warpgroup MMA (default), 0 = mma.sync
+    (ubn_set_fwd_engine).  Process-wide."""
+    from ._cabi import load
+    check(load().ubn_set_fwd_engine(c_int(int(engine))))
+
+
+def get_fwd_engine():
+    from ._cabi import load
+    return int(load().ubn_get_fwd_engine())
+
+
 def cumdist_thres(dist, thres):
     _chk(dist, 'dist')
     mask = torch.empty(dist.shape, dtype=torch.bool, device=dist.device)
