@@ -436,6 +436,21 @@ int ubn_march_ndc_feature_bwd(const float* rays_o, const float* rays_d, const Ub
                               int64_t n_rays, const uint8_t* flags, const int64_t* offsets, const float* grad_feat,
                               float* grad_k0, void* stream);
 
+/* Render a batch of rays of DirectMPIGO (dmpigo.py:224-331) in one fused pass with no per-sample global memory, as
+ * ubn_render_contracted does for the contracted models: pass A's NDC march (density + the act_shift grid, same arithmetic; the ray
+ * left at T < 1e-3), the k0 read of every kept sample (ubn_march_ndc_feature_fwd's arithmetic), the 3-layer rgbnet on the tensor
+ * cores (3xTF32; W1 NULL: sigmoid(k0), C = 3) and the composite.  density: contiguous single-slab C = 1 grid; act_shift: the
+ * single-slab [1,1,1,1,mpi_depth] grid; k0: single-slab channels-last.  rgbnet (C, viewbase_pe, width) = (9, 0, 64) (llff_default):
+ * W1 [64][C + 3], b1, W2 [64][64], b2, W3 [3][64], b3; viewdirs [n,3] feed the view embedding.  Outputs: rgb_marched [n,3] =
+ * sum w rgb in step order + alphainv_last * bg (dmpigo.py:318-320 without rand_bkgd), depth [n] = sum w (step_id + 0.5) / S
+ * (dmpigo.py:331), alphainv_last [n] (bit-identical to pass A's); optional n_shaded / n_marched as for ubn_render_contracted. */
+int ubn_render_ndc(const float* rays_o, const float* rays_d, const float* viewdirs, const float* density_grid,
+                   const UbnGridDesc* density_desc, const float* act_shift_grid, const UbnGridDesc* act_shift_desc,
+                   const float* k0_grid, const UbnGridDesc* k0_desc, const uint8_t* mask_world, const UbnNdcMarchCfg* cfg,
+                   int64_t n_rays, const float* W1, const float* b1, const float* W2, const float* b2, const float* W3,
+                   const float* b3, int width, int viewbase_pe, float bg, float* rgb_marched, float* depth, float* alphainv_last,
+                   int32_t* n_shaded, int32_t* n_marched, void* stream);
+
 /* Backward of pass A: exact reverse scan (alpha2weight_backward) -> raw2alpha_backward -> scatter into the density-grid gradient.
  * act_shift gets no gradient (requires_grad = False, dmpigo.py:50).  gd_scratch as for ubn_march_density_bwd. */
 int ubn_march_ndc_density_bwd(const float* rays_o, const float* rays_d, const UbnGridDesc* density_desc,
@@ -484,6 +499,21 @@ int ubn_march_box_feature_fwd(const float* rays_o, const float* rays_d, const fl
 int ubn_march_box_feature_bwd(const float* rays_o, const float* rays_d, const UbnGridDesc* k0_desc, const UbnBoxMarchCfg* cfg,
                               int64_t n_rays, const uint8_t* flags, const int64_t* offsets, const float* grad_feat,
                               float* grad_k0, void* stream);
+/* Render a batch of rays of DirectVoxGO (dvgo.py:306-415) in one fused pass with no per-sample global memory, as
+ * ubn_render_contracted does for the contracted models: pass A's box march (same arithmetic; the ray's own n_steps clamped to
+ * cfg->s_max, a longer ray sets *overflow as ubn_march_box_density_fwd does; the ray left at T < 1e-3), the k0 read of every kept
+ * sample (ubn_march_box_feature_fwd's arithmetic), the 3-layer rgbnet on the tensor cores (3xTF32, rgbnet_direct; W1 NULL:
+ * sigmoid(k0), C = 3) and the composite.  density: contiguous single-slab C = 1 grid; k0: single-slab channels-last.  rgbnet
+ * (C, viewbase_pe, width) = (12, 4, 128) or (9, 4, 64): W1 [width][C + 3 + 6 viewbase_pe], b1, W2 [width][width], b2, W3 [3][width],
+ * b3 (nn.Linear weights); viewdirs [n,3] feed the view embedding.  Outputs: rgb_marched [n,3] = sum w rgb in step order +
+ * alphainv_last * bg (dvgo.py:406), depth [n] = sum w step_id (dvgo.py:415), alphainv_last [n] (bit-identical to pass A's);
+ * optional (NULL = none) n_shaded / n_marched as for ubn_render_contracted.  overflow: device int32 the caller zeroes (or NULL). */
+int ubn_render_box(const float* rays_o, const float* rays_d, const float* viewdirs, const float* density_grid,
+                   const UbnGridDesc* density_desc, const float* k0_grid, const UbnGridDesc* k0_desc, const uint8_t* mask_world,
+                   const UbnBoxMarchCfg* cfg, int64_t n_rays, const float* W1, const float* b1, const float* W2, const float* b2,
+                   const float* W3, const float* b3, int width, int viewbase_pe, float bg, float* rgb_marched, float* depth,
+                   float* alphainv_last, int32_t* n_shaded, int32_t* n_marched, int32_t* overflow, void* stream);
+
 /* Backward of pass A: exact reverse scan -> raw2alpha_backward -> scatter into the density-grid gradient.  gd_scratch as for
  * ubn_march_density_bwd, with S = cfg->s_max. */
 int ubn_march_box_density_bwd(const float* rays_o, const float* rays_d, const UbnGridDesc* density_desc,

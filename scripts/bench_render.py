@@ -1,14 +1,21 @@
-"""Time the fused whole-frame render (models._ContractedBase.render_fused, csrc/render.cu) against the chunk loop it replaces
-(``model(...)`` per 8192 rays, what render.render_rays ran before) and print one JSON line per workload.
+"""Time the fused whole-frame render (render_fused of the contracted models, csrc/render.cu, and of DirectVoxGO / DirectMPIGO,
+csrc/render_bounded.cu) against the chunk loop (``model(...)`` per 8192 rays, what render.render_rays runs without it) and print one
+JSON line per workload.
 
-    python scripts/bench_render.py [--rounds 3] [--warmup 1]
+    python scripts/bench_render.py [--rounds 3] [--warmup 1] [--workloads garden-dense,lego-opaque,...]
 
 Workloads, each in a 'dense' scene (random density as in bench.py: rays rarely stop) and an 'opaque' one (the same plus a solid
 sphere of high density, radius half the scene: most rays stop early):
   garden: bench.py --workload garden's model (DirectContractedVoxGO 320^3, l2 norm, 12-channel k0, rgbnet 128, viewbase_pe 4,
           fast_color_thres 0) and its 1600 x 1067 frame;
   truck:  a truck-shaped FourierGridModel (153^3, fourier_freq_num 4 -> 9 slabs, 12 channels, stepsize 0.5) on the same frame.
-          The fused render does not cover Fourier slabs (render_fused_ok), so only the chunk loop is timed there.
+          The fused render does not cover Fourier slabs (render_fused_ok), so only the chunk loop is timed there;
+  lego:   DirectVoxGO at the NeRF-synthetic fine shape as scripts/bench_dvgo.py builds it (160^3, 12-channel k0, rgbnet 128,
+          viewbase_pe 4, stepsize 0.5, fast_color_thres 1e-4, bg 1, its object-in-box scene: 'dense'; 'opaque' adds a solid ball of
+          high density, radius half the box) and its 800 x 800 frame;
+  fern:   DirectMPIGO at llff_default as scripts/bench_mpi.py builds it (256^3 voxel budget, mpi_depth 128, stepsize 0.5, 9-channel
+          k0, rgbnet 64, viewbase_pe 0, fast_color_thres 1e-3, seeded grids: 'dense'; 'opaque' adds four planes of high density
+          half way through) and one 1008 x 756 NDC frame.
 The two paths alternate in one process (fused, loop, fused, loop ...).  Per workload: CUDA-event ms per frame of each (median and
 all rounds), samples nominal (rays x samples per ray), marched (the 32-sample chunks the fused march walked before each ray
 stopped) and shaded (its kept samples), peak device memory of each
@@ -31,20 +38,51 @@ from bench_dvgo import _gpu  # noqa: E402
 SEED = 777
 RK_GARDEN = dict(near=0., far=1e9, bg=1, rand_bkgd=False, stepsize=1.045, render_depth=True, coherent_rays=False)
 RK_TRUCK = dict(RK_GARDEN, stepsize=0.5)
+RK_LEGO = dict(near=2.0, far=6.0, bg=1., rand_bkgd=False, stepsize=0.5, render_depth=True)
+RK_FERN = dict(near=0., far=1., bg=1, rand_bkgd=False, stepsize=0.5, render_depth=True)
 
 
-def _frame(dev, H=1067, W=1600):
+def _frame(dev, name):
     import numpy as np
     from unboundednerfpytorch_b200 import rays as R
-    K = np.array([[float(W), 0, W / 2], [0, float(W), H / 2], [0, 0, 1]], dtype=np.float64)
-    c2w = torch.tensor([[1., 0., 0., 0.15], [0., 1., 0., -0.10], [0., 0., 1., 0.35]])
-    ro, rd, vd = R._rays_of_a_view(H, W, K, c2w, False, False, False, False, 'center', device=dev)
-    return ro.view(-1, 3), rd.view(-1, 3), vd.view(-1, 3)
+    ndc = name == 'fern'
+    if name == 'lego':          # scripts/bench_dvgo.py's frame: 4 units out, looking at the box
+        H, W = 800, 800
+        K = np.array([[1111., 0., 400.], [0., 1111., 400.], [0., 0., 1.]])
+        c2w = torch.tensor([[1., 0., 0., 0.], [0., 1., 0., 0.], [0., 0., 1., 4.0]])
+    elif ndc:
+        H, W = 756, 1008
+        K = np.array([[815., 0., 504.], [0., 815., 378.], [0., 0., 1.]])
+        c2w = torch.tensor([[1., 0., 0., 0.], [0., 1., 0., 0.], [0., 0., 1., 0.]])
+    else:
+        H, W = 1067, 1600
+        K = np.array([[float(W), 0, W / 2], [0, float(W), H / 2], [0, 0, 1]], dtype=np.float64)
+        c2w = torch.tensor([[1., 0., 0., 0.15], [0., 1., 0., -0.10], [0., 0., 1., 0.35]])
+    ro, rd, vd = R._rays_of_a_view(H, W, K, c2w, ndc, False, False, False, 'center', device=dev)
+    return ro.reshape(-1, 3), rd.reshape(-1, 3), vd.reshape(-1, 3)
 
 
 def _model(name, scene, dev):
     from unboundednerfpytorch_b200 import models
     torch.manual_seed(SEED)
+    if name == 'lego':
+        from bench_dvgo import _scene
+        m = _scene(160 ** 3, 12, 1, 0)[0]
+        if scene == 'opaque':
+            X, Y, Z = m.density.grid.shape[2:]
+            ax = [torch.linspace(-1, 1, n, device=dev) for n in (X, Y, Z)]
+            r = (ax[0][:, None, None] ** 2 + ax[1][None, :, None] ** 2 + ax[2][None, None, :] ** 2).sqrt()
+            with torch.no_grad():
+                m.density.grid.add_(torch.where(r < 0.5, 40.0, 0.0))
+        return m
+    if name == 'fern':
+        from bench_mpi import _scene
+        m = _scene(1)[0]
+        if scene == 'opaque':
+            Z = m.density.grid.shape[-1]
+            with torch.no_grad():
+                m.density.grid[..., Z // 2:Z // 2 + 4] += 40.0
+        return m
     if name == 'garden':
         w = 320
         m = models.DirectContractedVoxGO(xyz_min=[-1.] * 3, xyz_max=[1.] * 3, num_voxels=w ** 3, num_voxels_base=w ** 3,
@@ -106,14 +144,19 @@ def main():
     build.build()
     dev = torch.device('cuda', 0)
     gpu, power = _gpu()
-    ro, rd, vd = _frame(dev)
-    n = ro.shape[0]
     for wl in args.workloads.split(','):
         name, scene = wl.split('-')
+        ro, rd, vd = _frame(dev, name)
+        n = ro.shape[0]
         m = _model(name, scene, dev)
-        rk = RK_GARDEN if name == 'garden' else RK_TRUCK
+        rk = {'garden': RK_GARDEN, 'truck': RK_TRUCK, 'lego': RK_LEGO, 'fern': RK_FERN}[name]
         covered = m.render_fused_ok(ro, rk)
-        S = int(m._march_inputs(rk['stepsize'], dev)[0].numel())
+        if name == 'lego':
+            S = int(m._box_cfg(rk).s_max)          # the bound of a ray's steps; its own n_steps may be fewer
+        elif name == 'fern':
+            S = int(m._ndc_cfg(rk)[1])
+        else:
+            S = int(m._march_inputs(rk['stepsize'], dev)[0].numel())
         ns = torch.empty(n, dtype=torch.int32, device=dev)
         nm = torch.empty(n, dtype=torch.int32, device=dev)
         if not covered:                       # the 9-slab truck-shaped model: render_rays keeps the chunk loop

@@ -149,6 +149,11 @@ _SIGNATURES = {
                                   c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
     'ubn_march_box_feature_bwd': [c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnBoxMarchCfg), c_i64,
                                   c_p, c_p, c_p, c_p, c_p],
+    'ubn_render_ndc': [c_p, c_p, c_p, c_p, ctypes.POINTER(UbnGridDesc), c_p, ctypes.POINTER(UbnGridDesc), c_p,
+                       ctypes.POINTER(UbnGridDesc), c_p, ctypes.POINTER(UbnNdcMarchCfg), c_i64] + [c_p] * 6 + [c_int, c_int, c_f]
+                      + [c_p] * 6,
+    'ubn_render_box': [c_p, c_p, c_p, c_p, ctypes.POINTER(UbnGridDesc), c_p, ctypes.POINTER(UbnGridDesc), c_p,
+                       ctypes.POINTER(UbnBoxMarchCfg), c_i64] + [c_p] * 6 + [c_int, c_int, c_f] + [c_p] * 7,
     'ubn_march_box_density_bwd': [c_p, c_p, ctypes.POINTER(UbnGridDesc), ctypes.POINTER(UbnBoxMarchCfg), c_i64,
                                   c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
     'ubn_tensorf_fwd': [c_p, c_p, ctypes.POINTER(UbnTensorfDesc), c_p, c_i64, c_p, c_p],

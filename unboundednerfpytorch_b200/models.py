@@ -120,6 +120,40 @@ class _GridModel(nn.Module):
             return shade_mod.shade(self.rgbnet, k0, emb, ray_id)          # fused on-chip MLP (csrc/shade.cu)
         return torch.sigmoid(self.rgbnet(torch.cat([k0, emb[ray_id]], -1)))   # other widths / depths: torch (cuBLAS)
 
+    # ---- the fused render of the bounded models (DirectVoxGO, DirectMPIGO) ------------------------------------------------
+    FUSED_FRAME_BY_DEFAULT = True      # render.render_rays takes render_fused where it applies even without fused_frame=True
+
+    def _render_net_ok(self, C, covered):
+        """Whether the fused render kernels take this model's rgbnet on a C-channel k0: none with C = 3 (sigmoid(k0)), or a
+        3-layer float32 CUDA rgbnet on cat[k0, view embedding] whose (C, viewbase_pe, width) is in ``covered``."""
+        net = self.rgbnet
+        if net is None:
+            return C == 3
+        try:
+            l1, l2, l3 = net[0], net[2][0], net[3]
+        except Exception:
+            return False
+        pe, W = self.viewfreq.numel(), l1.weight.shape[0]
+        return (len(net) == 4 and (C, pe, W) in covered and tuple(l1.weight.shape) == (W, C + 3 + 6 * pe)
+                and tuple(l2.weight.shape) == (W, W) and tuple(l3.weight.shape) == (3, W)
+                and all(t.is_cuda and t.dtype == torch.float32 for t in (l1.weight, l2.weight, l3.weight)))
+
+    def _render_net_args(self):
+        """((W1, b1, W2, b2, W3, b3), width, viewbase_pe) for a render entry; NULL weights, 0, 0 without an rgbnet."""
+        if self.rgbnet is None:
+            return (None,) * 6, 0, 0
+        l1, l2, l3 = self.rgbnet[0], self.rgbnet[2][0], self.rgbnet[3]
+        net = tuple(t.detach().contiguous() for t in (l1.weight, l1.bias, l2.weight, l2.bias, l3.weight, l3.bias))
+        return net, l1.weight.shape[0], self.viewfreq.numel()
+
+    def _render_grids_ok(self, rays_o, render_kwargs):
+        """What both bounded models' render_fused_ok require besides their own geometry: no gradient, CUDA rays, a contiguous
+        float32 one-slab density, a float32 k0 and a numeric bg."""
+        dg, kg = self.density.grid, self.k0.grid
+        return (not torch.is_grad_enabled() and rays_o.is_cuda and isinstance(render_kwargs.get('bg'), (int, float))
+                and march.box_density_supported(dg) and dg.dtype == torch.float32 and kg.dtype == torch.float32
+                and kg.numel() < 2 ** 31)
+
     def _mask_lattice(self, world_size):
         """[X, Y, Z, 3]: linspace(xyz_min, xyz_max, world_size) per axis, the points a mask cache is built on."""
         ws = [int(v) for v in world_size]
@@ -922,13 +956,8 @@ class DirectVoxGO(_CoarseGeo, _GridModel):
             if self._tensorf():     # the op-by-op composition on the TensoRF kernels, shaded as the march is
                 return self._compose(rays_o, rays_d, viewdirs, self._shade_k0, render_kwargs)
             return self.forward_ops(rays_o, rays_d, viewdirs, global_step=global_step, **render_kwargs)
-        if self._pending_mask is not None:
-            self._resolve_mask_cache()
         N = len(rays_o)
-        mscale, mshift, lo, hi = self._mask_geometry()
-        cfg = march.make_box_cfg(lo, hi, render_kwargs['near'], self._stepdist(stepsize), host_scalar(self.act_shift),
-                                 stepsize * host_scalar(self.voxel_size_ratio), self.fast_color_thres, self.mask_cache.mask, mscale,
-                                 mshift)
+        cfg = self._box_cfg(render_kwargs)
         if self._tensorf():
             weights, alphainv_last, alpha, k0, ray_id, step_id = self._march_tensorf(rays_o, rays_d, cfg)
         else:
@@ -938,6 +967,68 @@ class DirectVoxGO(_CoarseGeo, _GridModel):
                 self.density.grid, self.k0.grid, rays_o, rays_d, self.mask_cache.mask, cfg, ddesc, kdesc)
         rgb = self._shade_k0(k0, viewdirs, ray_id)
         return self._finish(N, weights, alphainv_last, alpha, rgb, ray_id, step_id, render_kwargs)
+
+    def _box_cfg(self, render_kwargs):
+        """The box march cfg of forward and render_fused (a pending coarse mask cache resolved first): the bbox, near, the step
+        length, act_shift, interval = stepsize * voxel_size_ratio, the threshold and the mask cache's geometry."""
+        if self._pending_mask is not None:
+            self._resolve_mask_cache()
+        stepsize = render_kwargs['stepsize']
+        mscale, mshift, lo, hi = self._mask_geometry()
+        return march.make_box_cfg(lo, hi, render_kwargs['near'], self._stepdist(stepsize), host_scalar(self.act_shift),
+                                  stepsize * host_scalar(self.voxel_size_ratio), self.fast_color_thres, self.mask_cache.mask,
+                                  mscale, mshift)
+
+    # ---- the fused render -----------------------------------------------------------------------------------------------------
+    FUSED_FRAME_BY_DEFAULT = False     # render.render_rays takes render_fused only with fused_frame=True (DESIGN.md §7)
+    RENDER_NETS = ((12, 4, 128), (9, 4, 64))      # (k0 channels, viewbase_pe, width) of csrc/render_bounded.cu's box kernels
+
+    def render_fused_ok(self, rays_o, render_kwargs):
+        """Whether render_fused covers this model and call (render.render_rays with fused_frame=True takes it exactly then): no
+        gradient, CUDA rays, DenseGrid density and k0 where forward's fused box march applies (a contiguous one-slab density, a
+        channels-last k0 of 12, 9 or 3 channels; no TensoRFGrid), an rgbnet_direct rgbnet with (rgbnet_dim, viewbase_pe, width) =
+        (12, 4, 128) (the fine stage) or (9, 4, 64), or none with a 3-channel k0 (sigmoid(k0), the coarse stage), and a numeric
+        bg."""
+        if self._tensorf() or not self._render_grids_ok(rays_o, render_kwargs) or 'stepsize' not in render_kwargs:
+            return False
+        if not self._fused_ok(render_kwargs['stepsize']):
+            return False
+        if self.rgbnet is not None and not self.rgbnet_direct:
+            return False
+        return self._render_net_ok(self.k0.grid.shape[1], self.RENDER_NETS)
+
+    @torch.no_grad()
+    def render_fused(self, rays_o, rays_d, viewdirs, n_shaded=None, n_marched=None, **render_kwargs):
+        """{'rgb_marched' [N,3], 'depth' [N], 'alphainv_last' [N]} of N rays in one launch (csrc/render_bounded.cu): the box
+        march, the k0 read of the kept samples, the rgbnet and the composite with no per-sample buffers, so a whole frame is one
+        call.  Same kept samples and alphainv_last (bit for bit) as forward; rgb_marched (+ alphainv_last * bg) and depth (sum of
+        w * step_id) as forward's composite, summed in step order.  A ray needing more than the cfg's S_max steps raises as
+        forward does.  n_shaded / n_marched: optional int32 [N] that receive each ray's kept samples / the samples of the
+        32-sample chunks marched before the ray stopped.  Only where render_fused_ok holds."""
+        from . import _cabi
+        from ._cabi import c_f, c_i64, c_int, check, ptr, stream_of
+        N = rays_o.shape[0]
+        dev = rays_o.device
+        rays_o = rays_o.contiguous().float()
+        rays_d = rays_d.contiguous().float()
+        viewdirs = viewdirs.contiguous().float()
+        rgb = torch.empty(N, 3, dtype=torch.float32, device=dev)
+        depth = torch.empty(N, dtype=torch.float32, device=dev)
+        last = torch.empty(N, dtype=torch.float32, device=dev)
+        over = torch.zeros(1, dtype=torch.int32, device=dev)
+        cfg = self._box_cfg(render_kwargs)
+        ddesc = G.grid_desc(self.density.grid, *self.density._bounds(), 0)
+        kdesc = G.grid_desc(self.k0.grid, *self.k0._bounds(), 0)
+        net, width, pe = self._render_net_args()
+        with _cabi.timed('render_box'):
+            check(_cabi.load().ubn_render_box(
+                ptr(rays_o), ptr(rays_d), ptr(viewdirs), ptr(self.density.grid), ddesc, ptr(self.k0.grid), kdesc,
+                ptr(self.mask_cache.mask), cfg, c_i64(N), *map(ptr, net), c_int(width), c_int(pe), c_f(float(render_kwargs['bg'])),
+                ptr(rgb), ptr(depth), ptr(last), ptr(n_shaded), ptr(n_marched), ptr(over), stream_of(rgb)))
+        if N > 0 and int(over.item()):
+            raise RuntimeError(f'box march: a ray needs more than s_max = {cfg.s_max} steps (bbox / stepsize / ray origin out of '
+                               'range)')
+        return {'rgb_marched': rgb, 'depth': depth, 'alphainv_last': last}
 
     def _march_tensorf(self, rays_o, rays_d, cfg):
         """march.BoxTensorfMarch: a TensoRF density is read in pass A; the k0 (TensoRFGrid or DenseGrid) reads the survivor
@@ -1138,16 +1229,69 @@ class DirectMPIGO(_GridModel):
             return self.forward_ops(rays_o, rays_d, viewdirs, global_step=global_step, **render_kwargs)
         assert render_kwargs['near'] == 0 and render_kwargs['far'] == 1
         N = len(rays_o)
-        N_samples = self._n_samples(render_kwargs['stepsize'])
-        lo, hi = self._host()
-        mscale, mshift = self._mask_geometry()
-        cfg = march.make_ndc_cfg(lo, hi, N_samples, render_kwargs['stepsize'] * self.voxel_size_ratio, self.fast_color_thres,
-                                 self.mask_cache.mask, mscale, mshift)
+        cfg, N_samples = self._ndc_cfg(render_kwargs)
         descs = [G.grid_desc(g.grid, *g._bounds(), 0) for g in (self.density, self.k0, self.act_shift)]
         weights, alphainv_last, alpha, k0, ray_id, step_id = march.NdcMarch.apply(
             self.density.grid, self.k0.grid, self.act_shift.grid, rays_o, rays_d, self.mask_cache.mask, cfg, *descs)
         rgb = self._shade(k0, viewdirs, ray_id)
         return self._finish(N, weights, alphainv_last, alpha, rgb, ray_id, step_id, N_samples, global_step, render_kwargs)
+
+    def _ndc_cfg(self, render_kwargs):
+        """(NDC march cfg, N_samples) of forward and render_fused: the bbox, N_samples = int((mpi_depth - 1) / stepsize) + 1,
+        interval = stepsize * voxel_size_ratio, the threshold and the mask cache's geometry."""
+        stepsize = render_kwargs['stepsize']
+        N_samples = self._n_samples(stepsize)
+        lo, hi = self._host()
+        mscale, mshift = self._mask_geometry()
+        cfg = march.make_ndc_cfg(lo, hi, N_samples, stepsize * self.voxel_size_ratio, self.fast_color_thres, self.mask_cache.mask,
+                                 mscale, mshift)
+        return cfg, N_samples
+
+    # ---- the fused render -----------------------------------------------------------------------------------------------------
+    FUSED_FRAME_BY_DEFAULT = False     # render.render_rays takes render_fused only with fused_frame=True (DESIGN.md §7)
+    RENDER_NETS = ((9, 0, 64),)        # (k0 channels, viewbase_pe, width) of csrc/render_bounded.cu's NDC kernel: llff_default
+
+    def render_fused_ok(self, rays_o, render_kwargs):
+        """Whether render_fused covers this model and call (render.render_rays with fused_frame=True takes it exactly then): no
+        gradient, CUDA rays, grids where forward's fused NDC march applies (a contiguous one-slab density, a channels-last k0 of
+        9 or 3 channels, a one-slab act_shift grid), an rgbnet with (rgbnet_dim, viewbase_pe, width) = (9, 0, 64)
+        (llff_default) or none with a 3-channel k0 (sigmoid(k0)), a numeric bg, and near = 0, far = 1."""
+        sg = self.act_shift.grid
+        if not (self._render_grids_ok(rays_o, render_kwargs) and self._fused_ok() and 'stepsize' in render_kwargs
+                and render_kwargs.get('near') == 0 and render_kwargs.get('far') == 1):
+            return False
+        if not (sg.is_cuda and sg.dtype == torch.float32 and tuple(sg.shape[:2]) == (1, 1) and sg.is_contiguous()
+                and self._n_samples(render_kwargs['stepsize']) >= 2):
+            return False
+        return self._render_net_ok(self.k0.grid.shape[1], self.RENDER_NETS)
+
+    @torch.no_grad()
+    def render_fused(self, rays_o, rays_d, viewdirs, n_shaded=None, n_marched=None, **render_kwargs):
+        """{'rgb_marched' [N,3], 'depth' [N], 'alphainv_last' [N]} of N rays in one launch (csrc/render_bounded.cu): the NDC
+        march, the k0 read of the kept samples, the rgbnet and the composite with no per-sample buffers, so a whole frame is one
+        call.  Same kept samples and alphainv_last (bit for bit) as forward; rgb_marched (+ alphainv_last * bg; a render has no
+        global_step, so never rand_bkgd) and depth (sum of w * (step_id + 0.5) / N_samples) as forward's composite, summed in step
+        order.  n_shaded / n_marched: optional int32 [N] that receive each ray's kept samples / the samples of the 32-sample
+        chunks marched before the ray stopped.  Only where render_fused_ok holds."""
+        from . import _cabi
+        from ._cabi import c_f, c_i64, c_int, check, ptr, stream_of
+        N = rays_o.shape[0]
+        dev = rays_o.device
+        rays_o = rays_o.contiguous().float()
+        rays_d = rays_d.contiguous().float()
+        viewdirs = viewdirs.contiguous().float()
+        rgb = torch.empty(N, 3, dtype=torch.float32, device=dev)
+        depth = torch.empty(N, dtype=torch.float32, device=dev)
+        last = torch.empty(N, dtype=torch.float32, device=dev)
+        cfg, _ = self._ndc_cfg(render_kwargs)
+        ddesc, sdesc, kdesc = (G.grid_desc(g.grid, *g._bounds(), 0) for g in (self.density, self.act_shift, self.k0))
+        net, width, pe = self._render_net_args()
+        with _cabi.timed('render_ndc'):
+            check(_cabi.load().ubn_render_ndc(
+                ptr(rays_o), ptr(rays_d), ptr(viewdirs), ptr(self.density.grid), ddesc, ptr(self.act_shift.grid), sdesc,
+                ptr(self.k0.grid), kdesc, ptr(self.mask_cache.mask), cfg, c_i64(N), *map(ptr, net), c_int(width), c_int(pe),
+                c_f(float(render_kwargs['bg'])), ptr(rgb), ptr(depth), ptr(last), ptr(n_shaded), ptr(n_marched), stream_of(rgb)))
+        return {'rgb_marched': rgb, 'depth': depth, 'alphainv_last': last}
 
     def forward_ops(self, rays_o, rays_d, viewdirs, global_step=None, **render_kwargs):
         """Op-by-op composition in the reference's order (dmpigo.py:251-340)."""
