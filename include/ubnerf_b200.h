@@ -378,6 +378,17 @@ int ubn_render_contracted(const float* rays_o, const float* rays_d, const float*
                           int width, int viewbase_pe, int use_bg, float bg, float* rgb_marched, float* depth,
                           float* alphainv_last, int32_t* n_shaded, int32_t* n_marched, void* stream);
 
+/* ubn_render_contracted for FourierGridModel with Fourier slabs: density and k0 with the same slab count P in {7, 9, 11}
+ * (density: contiguous single-channel; k0: 12 channels, channels-last), the (12, 4) width-128 rgbnet (W1 [128][39]).  Same
+ * arguments, kept samples and outputs as ubn_render_contracted, and its kernel (12 warps per SM, each marching and shading its own
+ * rays), instantiated on the slab count.  Anything else returns cudaErrorInvalidValue. */
+int ubn_render_fourier(const float* rays_o, const float* rays_d, const float* viewdirs, const float* t_table,
+                       const float* density_grid, const UbnGridDesc* density_desc, const float* k0_grid,
+                       const UbnGridDesc* k0_desc, const uint8_t* mask_world, const UbnMarchCfg* cfg, int64_t n_rays,
+                       const float* W1, const float* b1, const float* W2, const float* b2, const float* W3, const float* b3,
+                       int width, int viewbase_pe, int use_bg, float bg, float* rgb_marched, float* depth,
+                       float* alphainv_last, int32_t* n_shaded, int32_t* n_marched, void* stream);
+
 /* Backward of pass B: scatter grad_feat[M,C] into grad_k0 (adjoint of the trilinear read). */
 int ubn_march_feature_bwd(const float* rays_o, const float* rays_d, const float* t_table,
                           const UbnGridDesc* k0_desc, const UbnMarchCfg* cfg, int64_t n_rays,

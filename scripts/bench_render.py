@@ -8,8 +8,11 @@ Workloads, each in a 'dense' scene (random density as in bench.py: rays rarely s
 sphere of high density, radius half the scene: most rays stop early):
   garden: bench.py --workload garden's model (DirectContractedVoxGO 320^3, l2 norm, 12-channel k0, rgbnet 128, viewbase_pe 4,
           fast_color_thres 0) and its 1600 x 1067 frame;
-  truck:  a truck-shaped FourierGridModel (153^3, fourier_freq_num 4 -> 9 slabs, 12 channels, stepsize 0.5) on the same frame.
-          The fused render does not cover Fourier slabs (render_fused_ok), so only the chunk loop is timed there;
+  truck:  a truck-shaped FourierGridModel (153^3, fourier_freq_num 4 -> 9 slabs, 12 channels, stepsize 0.5) on the same frame;
+  fg7:    the shape of the reference's *_single FourierGrid configs: FourierGridModel 200^3, fourier_freq_num 3 -> 7 slabs,
+          12 channels, stepsize 0.5, on the same frame.
+          The Fourier-slab models take the fused render (csrc/render_fourier.cu) only with render_kwargs['fused_slabs'], which
+          this script sets unless --fused-slabs 0 is given; then only their chunk loop is timed;
   lego:   DirectVoxGO at the NeRF-synthetic fine shape as scripts/bench_dvgo.py builds it (160^3, 12-channel k0, rgbnet 128,
           viewbase_pe 4, stepsize 0.5, fast_color_thres 1e-4, bg 1, its object-in-box scene: 'dense'; 'opaque' adds a solid ball of
           high density, radius half the box) and its 800 x 800 frame;
@@ -37,7 +40,7 @@ from bench_dvgo import _gpu  # noqa: E402
 
 SEED = 777
 RK_GARDEN = dict(near=0., far=1e9, bg=1, rand_bkgd=False, stepsize=1.045, render_depth=True, coherent_rays=False)
-RK_TRUCK = dict(RK_GARDEN, stepsize=0.5)
+RK_TRUCK = dict(RK_GARDEN, stepsize=0.5)          # truck and fg7
 RK_LEGO = dict(near=2.0, far=6.0, bg=1., rand_bkgd=False, stepsize=0.5, render_depth=True)
 RK_FERN = dict(near=0., far=1., bg=1, rand_bkgd=False, stepsize=0.5, render_depth=True)
 
@@ -88,10 +91,10 @@ def _model(name, scene, dev):
         m = models.DirectContractedVoxGO(xyz_min=[-1.] * 3, xyz_max=[1.] * 3, num_voxels=w ** 3, num_voxels_base=w ** 3,
                                          alpha_init=1e-4, fast_color_thres=0, rgbnet_dim=12, contracted_norm='l2').to(dev)
     else:
-        w = 153
+        w, F_ = (153, 4) if name == 'truck' else (200, 3)
         m = models.FourierGridModel(xyz_min=[-1.] * 3, xyz_max=[1.] * 3, num_voxels_density=w ** 3, num_voxels_base_density=w ** 3,
                                     num_voxels_rgb=w ** 3, num_voxels_base_rgb=w ** 3, num_voxels_viewdir=-1, alpha_init=1e-4,
-                                    fast_color_thres=0, rgbnet_dim=12, fourier_freq_num=4).to(dev)
+                                    fast_color_thres=0, rgbnet_dim=12, fourier_freq_num=F_).to(dev)
     g = torch.Generator(device=dev).manual_seed(SEED)
     with torch.no_grad():
         m.density.grid.copy_(torch.randn(m.density.grid.shape, generator=g, device=dev))
@@ -137,6 +140,7 @@ def main():
     ap.add_argument('--rounds', type=int, default=3)
     ap.add_argument('--warmup', type=int, default=1)
     ap.add_argument('--workloads', default='garden-dense,garden-opaque,truck-dense,truck-opaque')
+    ap.add_argument('--fused-slabs', type=int, default=1, help="set render_kwargs['fused_slabs'] for the Fourier-slab models")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit('bench_render.py needs a CUDA device')
@@ -149,7 +153,9 @@ def main():
         ro, rd, vd = _frame(dev, name)
         n = ro.shape[0]
         m = _model(name, scene, dev)
-        rk = {'garden': RK_GARDEN, 'truck': RK_TRUCK, 'lego': RK_LEGO, 'fern': RK_FERN}[name]
+        rk = {'garden': RK_GARDEN, 'truck': RK_TRUCK, 'fg7': RK_TRUCK, 'lego': RK_LEGO, 'fern': RK_FERN}[name]
+        if name in ('truck', 'fg7') and args.fused_slabs:
+            rk = dict(rk, fused_slabs=True)
         covered = m.render_fused_ok(ro, rk)
         if name == 'lego':
             S = int(m._box_cfg(rk).s_max)          # the bound of a ray's steps; its own n_steps may be fewer
@@ -159,7 +165,7 @@ def main():
             S = int(m._march_inputs(rk['stepsize'], dev)[0].numel())
         ns = torch.empty(n, dtype=torch.int32, device=dev)
         nm = torch.empty(n, dtype=torch.int32, device=dev)
-        if not covered:                       # the 9-slab truck-shaped model: render_rays keeps the chunk loop
+        if not covered:                       # Fourier slabs without fused_slabs: render_rays keeps the chunk loop
             _chunk_loop(m, ro, rd, vd, rk)
             t_l = [_timed(lambda: _chunk_loop(m, ro, rd, vd, rk))[1] for _ in range(args.rounds)]
             print(json.dumps({'workload': wl, 'rays': n, 'samples_per_ray': S, 'gpu': gpu, 'power_limit': power, 'fused': None,

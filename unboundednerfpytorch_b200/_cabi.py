@@ -127,6 +127,8 @@ _SIGNATURES = {
                                   c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
     'ubn_render_contracted': [c_p, c_p, c_p, c_p, c_p, ctypes.POINTER(UbnGridDesc), c_p, ctypes.POINTER(UbnGridDesc), c_p,
                               ctypes.POINTER(UbnMarchCfg), c_i64] + [c_p] * 6 + [c_int, c_int, c_int, c_f] + [c_p] * 6,
+    'ubn_render_fourier': [c_p, c_p, c_p, c_p, c_p, ctypes.POINTER(UbnGridDesc), c_p, ctypes.POINTER(UbnGridDesc), c_p,
+                           ctypes.POINTER(UbnMarchCfg), c_i64] + [c_p] * 6 + [c_int, c_int, c_int, c_f] + [c_p] * 6,
     'ubn_set_feature_kernel': [c_int],
     'ubn_get_feature_kernel': [],
     'ubn_set_density_scatter': [c_int],

@@ -12,7 +12,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libubnerf_b200.so')
-SOURCES = ['ray_ops.cu', 'alpha_ops.cu', 'grid_sweep.cu', 'trilinear.cu', 'march.cu', 'march_feature.cu', 'march_ndc.cu', 'shade.cu', 'shade_tc.cu', 'ray_gen.cu', 'loss.cu', 'grid_utils.cu', 'render_tma.cu', 'tensorf.cu', 'bounds.cu', 'metrics.cu', 'color.cu', 'render.cu', 'render_bounded.cu']
+SOURCES = ['ray_ops.cu', 'alpha_ops.cu', 'grid_sweep.cu', 'trilinear.cu', 'march.cu', 'march_feature.cu', 'march_ndc.cu', 'shade.cu', 'shade_tc.cu', 'ray_gen.cu', 'loss.cu', 'grid_utils.cu', 'render_tma.cu', 'tensorf.cu', 'bounds.cu', 'metrics.cu', 'color.cu', 'render.cu', 'render_bounded.cu', 'render_fourier.cu']
 HEADERS = ['common.cuh', 'trilinear.cuh', 'march_common.cuh', 'ray_gen.cuh', 'tensorf.cuh', 'rgbnet_tc.cuh', 'render_warp.cuh', os.path.join('..', '..', 'include', 'ubnerf_b200.h')]
 NVCC_FLAGS = ['-std=c++17', '-O3', '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo',
               '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=hidden', '--cudart', 'static']

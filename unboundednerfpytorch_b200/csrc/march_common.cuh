@@ -431,39 +431,53 @@ __device__ __forceinline__ void transmittance_scan(bool listed, float alpha, int
 // The k0 features of one sample at normalised coordinates (nx, ny, nz), lane = sample: every channel accumulated in ATen's corner
 // order (fma chain tnw .. bse) and the slabs combined in torch-CUDA's mean order (accumulator a = slab & 3, ((a0 + a1) + a2) + a3),
 // so the features are bit-identical to F.grid_sample(...).mean(0).  Records of C % 4 == 0 channels are read as float4.
-template <int kC, int kP>
+// kLean: the slab loop rolled and four corner records in flight instead of eight, for callers with a smaller register budget
+// (render_fourier.cu's march warps); the same arithmetic in the same order
+template <int kC, int kP, bool kLean = false>
 __device__ __forceinline__ void lane_features(const GridView& g, float nx, float ny, float nz, float (&out)[kC]) {
   const int dY = g.Z * kC, dX = g.Y * g.Z * kC;
   float tot[kC], grp[kC];
+  auto corner_add = [&](const float* rec, const CellR& cell, int corner, float (&val)[kC]) {   // tnw .. bse (z fastest)
+    const int bx = corner >> 2, by = (corner >> 1) & 1, bz = corner & 1;
+    const float wgt = ((bz ? cell.fz : 1.f - cell.fz) * (by ? cell.fy : 1.f - cell.fy)) * (bx ? cell.fx : 1.f - cell.fx);
+    const float* q = rec + bx * dX + by * dY + bz * kC;
+    if constexpr (kC % 4 == 0) {
+#pragma unroll
+      for (int c4 = 0; c4 < kC; c4 += 4) {
+        const float4 v = __ldg(reinterpret_cast<const float4*>(q + c4));
+        val[c4] = fmaf(v.x, wgt, val[c4]); val[c4 + 1] = fmaf(v.y, wgt, val[c4 + 1]);
+        val[c4 + 2] = fmaf(v.z, wgt, val[c4 + 2]); val[c4 + 3] = fmaf(v.w, wgt, val[c4 + 3]);
+      }
+    } else {
+#pragma unroll
+      for (int c = 0; c < kC; ++c) val[c] = fmaf(__ldg(q + c), wgt, val[c]);
+    }
+  };
+  auto slab_add = [&](int a, int sl) {
+    const CellR cell = make_cell(src_index(fourier_gamma(sl, nx), g.X), src_index(fourier_gamma(sl, ny), g.Y),
+                                 src_index(fourier_gamma(sl, nz), g.Z), g.X, g.Y, g.Z);
+    const float* rec = g.data + sl * g.sp + (int64_t)cell.v * kC;
+    float val[kC];
+#pragma unroll
+    for (int c = 0; c < kC; ++c) val[c] = 0.f;
+    if constexpr (kLean) {
+#pragma unroll 4
+      for (int corner = 0; corner < 8; ++corner) corner_add(rec, cell, corner, val);
+    } else {
+#pragma unroll
+      for (int corner = 0; corner < 8; ++corner) corner_add(rec, cell, corner, val);
+    }
+#pragma unroll
+    for (int c = 0; c < kC; ++c) grp[c] = (sl == a) ? __fadd_rn(0.f, val[c]) : __fadd_rn(grp[c], val[c]);
+  };
 #pragma unroll
   for (int a = 0; a < 4 && a < kP; ++a) {
+    if constexpr (kLean) {
+#pragma unroll 1
+      for (int sl = a; sl < kP; sl += 4) slab_add(a, sl);
+    } else {
 #pragma unroll
-    for (int sl = a; sl < kP; sl += 4) {
-      const CellR cell = make_cell(src_index(fourier_gamma(sl, nx), g.X), src_index(fourier_gamma(sl, ny), g.Y),
-                                   src_index(fourier_gamma(sl, nz), g.Z), g.X, g.Y, g.Z);
-      const float* rec = g.data + sl * g.sp + (int64_t)cell.v * kC;
-      float val[kC];
-#pragma unroll
-      for (int c = 0; c < kC; ++c) val[c] = 0.f;
-#pragma unroll
-      for (int corner = 0; corner < 8; ++corner) {        // tnw, tne, tsw, tse, bnw, bne, bsw, bse (z fastest)
-        const int bx = corner >> 2, by = (corner >> 1) & 1, bz = corner & 1;
-        const float wgt = ((bz ? cell.fz : 1.f - cell.fz) * (by ? cell.fy : 1.f - cell.fy)) * (bx ? cell.fx : 1.f - cell.fx);
-        const float* q = rec + bx * dX + by * dY + bz * kC;
-        if constexpr (kC % 4 == 0) {
-#pragma unroll
-          for (int c4 = 0; c4 < kC; c4 += 4) {
-            const float4 v = __ldg(reinterpret_cast<const float4*>(q + c4));
-            val[c4] = fmaf(v.x, wgt, val[c4]); val[c4 + 1] = fmaf(v.y, wgt, val[c4 + 1]);
-            val[c4 + 2] = fmaf(v.z, wgt, val[c4 + 2]); val[c4 + 3] = fmaf(v.w, wgt, val[c4 + 3]);
-          }
-        } else {
-#pragma unroll
-          for (int c = 0; c < kC; ++c) val[c] = fmaf(__ldg(q + c), wgt, val[c]);
-        }
-      }
-#pragma unroll
-      for (int c = 0; c < kC; ++c) grp[c] = (sl == a) ? __fadd_rn(0.f, val[c]) : __fadd_rn(grp[c], val[c]);
+      for (int sl = a; sl < kP; sl += 4) slab_add(a, sl);
     }
 #pragma unroll
     for (int c = 0; c < kC; ++c) tot[c] = (a == 0) ? grp[c] : __fadd_rn(tot[c], grp[c]);

@@ -2,8 +2,8 @@
 //
 // One-slab density and k0 grids only: DirectContractedVoxGO, and FourierGridModel at fourier_freq_num 0.  With Fourier slabs
 // (the reference's FourierGridModel configs: 7 - 11 slabs) a 9-slab instance of this kernel rendered an opaque frame 8x faster than
-// the chunk loop but a dense one 0.79x as fast (its slab reads are latency-bound at 12 warps per SM), and nothing observable before
-// the render tells the two apart, so those models keep the chunk loop.
+// the chunk loop but a dense one 0.79x as fast (its slab reads are latency-bound at 12 warps per SM).  Those models render through
+// render_fourier.cu's slab instances of this loop when the caller opts in (render_kwargs['fused_slabs']), else through the chunk loop.
 //
 // Rendering needs three numbers per ray: rgb_marched, depth and alphainv_last.  The training path (march.cu + march_feature.cu +
 // shade_tc.cu + composite) writes dense per-sample records, compacts the survivors, reads their features, runs the rgbnet and

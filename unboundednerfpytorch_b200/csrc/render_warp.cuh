@@ -51,6 +51,14 @@ __device__ __forceinline__ float render_density(const MarchParams& p, float d, f
   }
 }
 
+// The density grid's value at (x, y, z) as pass A reads it: grid_density_fast at the slab counts its fast path takes (1 - 9),
+// grid_density_at at 11 (pass A's generic read of FourierGridModel at fourier_freq_num 5)
+template <int kP>
+__device__ __forceinline__ float render_grid_density(const GridView& g, float x, float y, float z) {
+  if constexpr (kP <= 9) return grid_density_fast<kP>(g, x, y, z);
+  else return grid_density_at(g, x, y, z);
+}
+
 // Shared memory of one instance.  With an rgbnet: W2 and W1 as fp32 B fragments, b1, b2, W3; then one block per warp (floats):
 // slot rays [16] (int64), feature tile [16][C], rgb [16][4], w [16], s [16], row slot [16], slot sums [16][4], slot
 // alphainv_last [16], slot embeddings [16][kEs] (with an rgbnet: the k columns of layer 1 past C, zero past C + E)
@@ -72,8 +80,9 @@ struct Layout {
 };
 
 // The body of a render kernel of kWarps warps: kC-channel k0, rgbnet of width kW at viewbase_pe kPe (kNet) or sigmoid(k0).
-// One-slab density and k0 grids.
-template <class Smp, int kC, int kPe, bool kNet, int kW, int kWarps>
+// kP-slab density and k0 grids (kP > 1: FourierGridModel's Fourier slabs, render_fourier.cu; the k0 read in lane_features' lean
+// form, which keeps the kernel at 168 registers without spills).
+template <class Smp, int kC, int kPe, bool kNet, int kW, int kWarps, int kP = 1>
 __device__ __forceinline__ void render_warps(const Args& a) {
   using L = Layout<kC, kPe, kNet, kW, kWarps>;
   constexpr int kKS = L::kKS, kEs = L::kEs, kNT = L::kNT;
@@ -240,7 +249,7 @@ __device__ __forceinline__ void render_warps(const Args& a) {
       const MarchSample ms = march_chunk_point<Smp>(r, a.t_table, a.mask_world, p, base, lane, cum, carry_over);
       float alpha = 0.f;
       if (ms.queried) {
-        alpha = march_alpha(render_density<Smp>(p, grid_density_fast<1>(a.gd, ms.x, ms.y, ms.z), ms.x, ms.y, ms.z), p);
+        alpha = march_alpha(render_density<Smp>(p, render_grid_density<kP>(a.gd, ms.x, ms.y, ms.z), ms.x, ms.y, ms.z), p);
       }
       const bool listed = march_listed(ms.queried, alpha, p);
       float myT, myW;
@@ -255,7 +264,7 @@ __device__ __forceinline__ void render_warps(const Args& a) {
       float f[kC];
       float sv = 0.f;
       if (keep) {
-        lane_features<kC, 1>(a.gk, norm_coord(ms.x, a.gk.mn[0], a.gk.len[0]), norm_coord(ms.y, a.gk.mn[1], a.gk.len[1]),
+        lane_features<kC, kP, (kP > 1)>(a.gk, norm_coord(ms.x, a.gk.mn[0], a.gk.len[0]), norm_coord(ms.y, a.gk.mn[1], a.gk.len[1]),
                                norm_coord(ms.z, a.gk.mn[2], a.gk.len[2]), f);
         sv = render_depth_term<Smp>(a, base + lane);
       }

@@ -289,17 +289,22 @@ class _ContractedBase(_GridModel):
 
     def render_fused_ok(self, rays_o, render_kwargs):
         """Whether render_fused covers this model and call (render.render_rays takes it exactly then): one-slab density and k0
-        grids (DirectContractedVoxGO; FourierGridModel at fourier_freq_num 0 -- with Fourier slabs the fused pass was slower than
-        the chunk loop on dense scenes, DESIGN.md §7), a channels-last k0 of 12 or 3 channels, the reference's unbounded rgbnets
-        ((rgbnet_dim, viewbase_pe) = (12, 4) or (3, 8), width 128, depth 3) or none (sigmoid(k0), 3 channels), no gradient, CUDA
-        rays, and a background the fused composite reproduces: none for FourierGridModel (rand_bkgd draws a random one), a number
-        for DirectContractedVoxGO."""
+        grids (DirectContractedVoxGO; FourierGridModel at fourier_freq_num 0), a channels-last k0 of 12 or 3 channels, the
+        reference's unbounded rgbnets ((rgbnet_dim, viewbase_pe) = (12, 4) or (3, 8), width 128, depth 3) or none (sigmoid(k0),
+        3 channels), no gradient, CUDA rays, and a background the fused composite reproduces: none for FourierGridModel
+        (rand_bkgd draws a random one), a number for DirectContractedVoxGO.
+        With render_kwargs['fused_slabs'] = True also FourierGridModel with Fourier slabs: density and k0 of the same slab count
+        7, 9 or 11 (fourier_freq_num 3, 4, 5), a 12-channel k0 and the (12, 4) rgbnet (csrc/render_fourier.cu).  Opt-in: on dense
+        scenes the fused slab render is not always faster than the chunk loop (DESIGN.md §7), and its frames agree with the loop to
+        about 1e-6, not bit for bit."""
         kg, dg = self.k0.grid, self.density.grid
         if torch.is_grad_enabled() or not (rays_o.is_cuda and kg.is_cuda and dg.is_cuda and self._fused_ok()):
             return False
-        C = kg.shape[1]
-        if not (kg.shape[0] == 1 and C in (3, 12) and kg.stride(1) == 1 and kg.dtype == torch.float32
-                and tuple(dg.shape[:2]) == (1, 1) and dg.is_contiguous() and dg.dtype == torch.float32):
+        P, C = kg.shape[0], kg.shape[1]
+        if P != 1 and not (render_kwargs.get('fused_slabs', False) and P in (7, 9, 11) and C == 12 and self.rgbnet is not None):
+            return False
+        if not (C in (3, 12) and kg.stride(1) == 1 and kg.dtype == torch.float32
+                and tuple(dg.shape[:2]) == (P, 1) and dg.is_contiguous() and dg.dtype == torch.float32):
             return False
         if self.RENDER_USES_BG:
             if not isinstance(render_kwargs.get('bg', 0), (int, float)):
@@ -323,8 +328,9 @@ class _ContractedBase(_GridModel):
         """{'rgb_marched' [N,3], 'depth' [N], 'alphainv_last' [N]} of N rays in one launch (csrc/render.cu): the march, the k0
         read of the kept samples, the rgbnet and the composite with no per-sample buffers, so a whole frame is one call.  Same
         kept samples and alphainv_last (bit for bit) as forward; rgb_marched and depth as forward's composite, summed in step order.
-        n_shaded / n_marched: optional int32 [N] that receive each ray's kept samples / the samples of the 32-sample chunks
-        marched before the ray stopped.  Only where render_fused_ok holds."""
+        Fourier slabs (render_kwargs['fused_slabs']) run csrc/render_fourier.cu, the same kernel and contract instantiated on the
+        slab count.  n_shaded / n_marched: optional int32 [N] that receive each ray's kept samples / the samples of the
+        32-sample chunks marched before the ray stopped.  Only where render_fused_ok holds."""
         from . import _cabi
         from ._cabi import c_f, c_i64, c_int, check, ptr, stream_of
         N = rays_o.shape[0]
@@ -344,8 +350,9 @@ class _ContractedBase(_GridModel):
             net, pe = (None,) * 6, 0
         use_bg = 1 if self.RENDER_USES_BG else 0
         bg = float(render_kwargs.get('bg', 0)) if use_bg else 0.0
-        with _cabi.timed('render_contracted'):
-            check(_cabi.load().ubn_render_contracted(
+        name = 'render_fourier' if self.k0.grid.shape[0] > 1 else 'render_contracted'
+        with _cabi.timed(name):
+            check(getattr(_cabi.load(), 'ubn_' + name)(
                 ptr(rays_o), ptr(rays_d), ptr(viewdirs), ptr(t_table), ptr(self.density.grid), ddesc, ptr(self.k0.grid), kdesc,
                 ptr(mask), cfg, c_i64(N), *map(ptr, net), c_int(128), c_int(pe), c_int(use_bg), c_f(bg), ptr(rgb), ptr(depth),
                 ptr(last), ptr(n_shaded), ptr(n_marched), stream_of(rgb)))

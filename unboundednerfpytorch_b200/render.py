@@ -31,13 +31,21 @@ def render_rays(model, rays_o, rays_d, viewdirs, render_kwargs, chunk=8192, keys
 
     fused_frame: also take the fused whole-frame render of the models whose fused render is opt-in (DirectVoxGO, DirectMPIGO:
     ``FUSED_FRAME_BY_DEFAULT = False``) where their render_fused_ok holds.  Off by default: their chunk loop's frames are what
-    forward computes bit for bit, the fused frames agree with it to about 1e-6 (forward's view bias is a cuBLAS addmm)."""
+    forward computes bit for bit, the fused frames agree with it to about 1e-6 (forward's view bias is a cuBLAS addmm).
+
+    render_kwargs keys read here besides the model's own: ``coherent_rays`` (TMA-staged feature reads of image-ordered chunks) and
+    ``fused_slabs`` (FourierGridModel with 7, 9 or 11 Fourier slabs in one fused launch, models._ContractedBase.render_fused_ok);
+    both off by default and passed on to every call, so render_frame_sharded, render_blocks_idw and render_viewpoints take them
+    too."""
     rk = dict(render_kwargs)
     rk.setdefault('render_depth', True)
     # render_kwargs['coherent_rays']=True routes DenseGrid feature reads of image-ordered chunks through the TMA-staged brick
     # kernel (csrc/render_tma.cu).  Opt-in: the lane-per-sample gather stays the default (the TMA kernel was slower on a full
     # garden frame when it was last compared; not re-measured on the H100).
     rk.setdefault('coherent_rays', False)
+    # render_kwargs['fused_slabs']=True extends the fused render to FourierGridModel with Fourier slabs (7, 9 or 11 slabs, the
+    # (12, 4) rgbnet: csrc/render_fourier.cu).  Opt-in like fused_frame: its frames agree with the chunk loop to about 1e-6, and
+    # on dense scenes it is not always the faster path (DESIGN.md §7).
     # contracted models the fused render covers (models._ContractedBase.render_fused_ok) take the whole ray array in one launch
     # (memory O(n), no per-sample buffers), and so do DirectVoxGO / DirectMPIGO with fused_frame=True; every other model or
     # configuration keeps the chunk loop
